@@ -49,7 +49,7 @@ def make_sweeps(synth, n_points, n_sweeps, pattern="livox"):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read-only queries)."""
 
     def __init__(self, device_index=0):
         self.lines = []
@@ -96,7 +96,7 @@ class ClockSampler:
 def run_reference(args):
     """CPU arm, wall-clock timed on rank 0.
 
-    Default: the REFERENCE'S OWN CODE — oracle/_ref/libsrl_reference.so, /root/reference/src/optimize.cpp etc. compiled unmodified
+    Default: the REFERENCE'S OWN CODE — oracle/_ref/libsrl_reference.so, the reference's src/optimize.cpp etc. compiled unmodified
     where they lie (oracle/Makefile) — on all host threads.  The reference has no threading on this path, so the only way it
     can use more than one core is independent sweeps: a step is one batch of `cores` sweeps, each registered against the shared
     map by its own thread through the reference's single-threaded updateIEKF (ref_update_iekf_many).  Each sweep is a bounded
@@ -353,6 +353,14 @@ def run_cfg5(args, torch, tdist, dist, lio, synth, rank, world, local, stream, f
     return out
 
 
+def dump_outputs(out_dir, arrays):
+    """Writes each output of the timed path's last step as out_dir/<name>.npy in float64 (a few kB in all), so that two builds
+    run with the same arguments can be compared output for output."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), np.asarray(a, dtype=np.float64))
+
+
 _REAL_STDOUT = None
 
 
@@ -385,7 +393,14 @@ def main():
                                                         "on by default when --gpus > 1")
     ap.add_argument("--no-cfg5", action="store_true")
     ap.add_argument("--cfg5-steps", type=int, default=10)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step returned (frame pose, ESIKF state and covariance, "
+                         "per-pass trace, residual count) as DIR/<name>.npy in float64")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs writes the outputs of the GPU path; it does not apply to --impl reference")
+    if args.dump_outputs and args.steps < 1:
+        ap.error("--dump-outputs needs at least one timed step (--steps >= 1)")
     global N_PASSES
     N_PASSES = args.passes
     if args.impl == "reference":
@@ -424,7 +439,7 @@ def main():
     prm = bench_params(lio)
     P = synth.prior_covariance()
     d_raw = [torch.from_numpy(s.raw_xyz).to(f"cuda:{local}") for s in sweeps]
-    flush_buf = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=f"cuda:{local}")   # > 126 MB L2
+    flush_buf = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=f"cuda:{local}")   # > 50 MB L2 of the H100
     native = os.environ.get("SRL_DIST_NATIVE", "1") != "0"
     D = dist.DistributedLio(L, rank, world, native=native) if world > 1 else None
 
@@ -437,13 +452,21 @@ def main():
         L.eskf_pro = lio.EskfEstimator(p=sw.t_init.copy(), q=sw.q_init.copy(), cov=P.copy())
         return sw
 
+    last_out = {}   # what the caller of the timed path received in the latest step (--dump-outputs)
+
     def step_resident(sw):
         if world > 1:
             out = D.updateIEKF(prm, sw.t_last)
             assert out["success"] and out["passes"] == N_PASSES
+            fq, ft, trace, n_res = out["frame_q"], out["frame_t"], out["trace"], out["num_residuals_used"]
         else:
-            summ, _, _ = L.updateIEKF(prm, sw.t_last)
+            summ, fq, ft = L.updateIEKF(prm, sw.t_last)
             assert summ.success and summ.passes_run == N_PASSES, (summ.success, summ.passes_run)
+            trace, n_res = summ.trace, summ.num_residuals_used
+        if args.dump_outputs:
+            e = L.eskf_pro
+            last_out.update(frame_q=fq, frame_t=ft, trace=trace, num_residuals_used=np.array([n_res]),
+                            **{f"state_{f}": getattr(e, f) for f in ("p", "q", "v", "ba", "bg", "g", "cov")})
 
     # e2e leg: the host buffers a caller would hand over, in pinned memory (the contract's "from pinned host memory")
     pin_world = torch.empty((args.points, 3), dtype=torch.float64).pin_memory()
@@ -492,6 +515,8 @@ def main():
     clocks = ClockSampler(local)
     clocks.start()
     ms_res, _, _, launches = timed(step_resident, True)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last_out)
     step_cycles = L.ctx.counter("iekf_step_cycles_avg")
     loop_on_device = bool(L.ctx.counter("device_loop_active"))
     order_impl = {1: "single-launch cluster radix sort (k_sweep_order_cluster), verified against the CUB order at first use",
@@ -523,7 +548,7 @@ def main():
     if os.path.exists(peaks_path):
         peak = float(json.load(open(peaks_path))["hbm_gbs"]); peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)"
     else:
-        peak = 6650.0; peak_src = "fallback 6.65 TB/s (B200_PROFILING.md)"
+        peak = 3350.0; peak_src = "data sheet, H100 SXM HBM3 3.35 TB/s (not a measured peak)"
     sw0 = sweeps[0]
     n_shard = args.points if world == 1 else (dist.shard_range(args.points, rank, world)[1] - dist.shard_range(args.points, rank, world)[0])
     prepare(0)
@@ -604,12 +629,6 @@ def main():
                 "k1_share_of_step": k1_avg_ms * N_PASSES / ms_step_tim, "timing_leg_ms_per_step": ms_step_tim,
                 "note": "k1_avg_ms = CUDA events around each pass's launches (k1_scan incl. its wait for the pose ticket, k1_fit, "
                         "fallback), measured in a separate leg of the same resident steps"}
-    tp = os.path.join(ROOT, "profiles", "k1_traffic.json")
-    if os.path.exists(tp):
-        try:
-            roofline["traffic"] = json.load(open(tp)).get("dram_bytes_per_launch")
-        except Exception:
-            pass
 
     # ---- config 4 (extra, N=1 only): stream of sweeps, each registered (3 passes) and then inserted into the map
     streaming = None

@@ -1,5 +1,5 @@
 /*
- * srlivo_b200.h — C ABI of the B200-native LIO scan-matching hot path of SR-LIVO.
+ * srlivo_b200.h — C ABI of the H100-native (sm_90a) LIO scan-matching hot path of SR-LIVO.
  *
  * The reference (ZikangYuan/sr_livo) has no plugin/FFI layer: the path is a set of member
  * functions of `class lioOptimization` (include/lioOptimization.h:334-353) operating on

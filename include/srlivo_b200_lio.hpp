@@ -1,6 +1,6 @@
 // srlivo_b200_lio.hpp — C++ host mirror of the reference's scan-matching interface over the C ABI.
 //
-// The reference is C++ (class lioOptimization, include/lioOptimization.h:192-385); a maintainer who wants the B200
+// The reference is C++ (class lioOptimization, include/lioOptimization.h:192-385); a maintainer who wants the GPU
 // path swaps the bodies of four member functions for the calls below (INTEGRATION.md shows the diff).  Header-only,
 // Eigen-free by default; define SRL_HAVE_EIGEN before including to get overloads on the reference's own types
 // (point3D / icpOptions / Eigen::Quaterniond), which cannot be compiled in this repository's container.

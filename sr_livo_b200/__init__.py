@@ -1,1 +1,1 @@
-"""sr_livo_b200 — B200-native LIO scan-matching hot path of SR-LIVO (see DESIGN.md)."""
+"""sr_livo_b200 — H100-native (sm_90a) LIO scan-matching hot path of SR-LIVO (see DESIGN.md)."""

@@ -101,7 +101,7 @@ static void unpack32(const double* o, srl_normal_eq* out, long long n_keypoints)
     out->reserved = 0;
 }
 
-constexpr bool kDefaultSplit = true;    // variant 0 (auto): k1_scan + k1_fit (1.27x faster than k1_fast on the 100k-point sweep, profiles/README.md)
+constexpr bool kDefaultSplit = true;    // variant 0 (auto): k1_scan + k1_fit (H100, 100k-point sweep: 0.46 vs 0.75 ms per sweep for k1_fast in the same run, BASELINE.md)
 
 static int pass_grid(srl_ctx* ctx, long long n, int K, int nb) {
     const long long n_groups = (n + 31) / 32;
@@ -200,8 +200,16 @@ static bool pass_is_fast(const srl_ctx* ctx, const K1Args& a) {
 // running kernels) or a synchronous copy issued while that block spins would deadlock against it.
 static int prepare_pass(srl_ctx* ctx, srl_sweep* sw, const K1Args& a) {
     if (!ctx->kernels_preloaded) {
-        SRL_CUDA(ctx, preload_fast_kernels(ctx->device));
-        SRL_CUDA(ctx, preload_assoc_kernels(ctx->device, a.c.K));
+        size_t max_local = 0;
+        SRL_CUDA(ctx, preload_fast_kernels(ctx->device, &max_local));
+        SRL_CUDA(ctx, preload_assoc_kernels(ctx->device, a.c.K, &max_local));
+        // The first launch of a kernel whose local memory (spills) exceeds the context's reservation makes the driver
+        // grow that reservation, and the driver waits for the device to go idle to do it.  Launched behind the persistent
+        // ESIKF block, which spins until the pass finishes, that wait never ends (k1_fast keeps a ~1.6 KB spill frame on
+        // sm_90a).  So the reservation is grown here, while nothing spins, to fit every pass kernel.
+        size_t stack = 0;
+        SRL_CUDA(ctx, cudaDeviceGetLimit(&stack, cudaLimitStackSize));
+        if (max_local > stack) SRL_CUDA(ctx, cudaDeviceSetLimit(cudaLimitStackSize, max_local));
         ctx->kernels_preloaded = true;
     }
     if (!pass_is_fast(ctx, a)) return SRL_OK;
@@ -282,7 +290,7 @@ static int launch_pass(srl_ctx* ctx, srl_sweep* sw, const K1Args& a, bool debug,
 extern "C" {
 
 int srl_abi_version(void) { return SRL_ABI_VERSION; }
-const char* srl_build_info(void) { return "srlivo_b200 sm_100a, CUDA " __DATE__; }
+const char* srl_build_info(void) { return "srlivo_b200 sm_90a, CUDA " __DATE__; }
 
 int srl_ctx_create(int device, void* cuda_stream, srl_ctx** out) {
     if (!out) return SRL_BAD_ARG;

@@ -1,4 +1,4 @@
-// srl_assoc.cu — K1: the fused scan-matching pass for sm_100a.
+// srl_assoc.cu — K1: the fused scan-matching pass for sm_90a.
 //
 // One launch = one ESIKF pass over this rank's keypoint shard, replacing the body of
 // lioOptimization::buildPlaneResiduals (src/optimize.cpp:18-131) plus the H_x/h assembly and the
@@ -708,7 +708,7 @@ cudaError_t launch_k1(const K1Args& a, int grid, bool debug, int device, cudaStr
     return launch_pass_kernel(fn, a, (unsigned)grid, kK1Threads, smem, stream, pdl);
 }
 
-cudaError_t preload_assoc_kernels(int device, int K) {
+cudaError_t preload_assoc_kernels(int device, int K, size_t* max_local) {
     upload_offsets(device);
     cudaFuncAttributes at;
     const size_t smem = k1_smem_bytes(K > 0 ? K : 20);
@@ -717,6 +717,7 @@ cudaError_t preload_assoc_kernels(int device, int K) {
         cudaError_t e = cudaFuncGetAttributes(&at, fn);
         if (e == cudaSuccess) e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
+        if (at.localSizeBytes > *max_local) *max_local = at.localSizeBytes;
     }
     return cudaSuccess;
 }

@@ -1,6 +1,6 @@
 // srl_device.cuh — HBM layout of the voxel map and shared device helpers.
 //
-// Layout (B200-first, not a translation of tsl::robin_map<voxel, voxelBlock>, include/cloudMap.h:171):
+// Layout (GPU-first, not a translation of tsl::robin_map<voxel, voxelBlock>, include/cloudMap.h:171):
 //   slot table : open addressing, power-of-two capacity >= 2 x max_voxels (load <= 0.5), 16-byte slots
 //                { u64 key (x,y,z as u16 | valid bit 48), u32 block, u32 count } -> one LDG.128 per probe.
 //   block pool : one 320-byte block per voxel = 20 x float4 (x, y, z, w): a point is ONE 16-byte load for a

@@ -1,9 +1,8 @@
-// srl_fast.cu — k1_fast: the thread-per-keypoint form of the fused scan-matching pass (sm_100a),
+// srl_fast.cu — k1_fast: the thread-per-keypoint form of the fused scan-matching pass (sm_90a),
 // and the spatial ordering of a sweep's keypoints that makes it coalesce.
 //
 // Why a second form of K1: the warp-per-keypoint kernel (srl_assoc.cu) is a serial chain of warp shuffles per
-// keypoint (ncu, profiles/r02_*: ~1400 warp instructions per keypoint, 13 cycles between issues of a warp,
-// only ~21 working warps per SM on a 100k-point sweep).  Here one THREAD owns one keypoint:
+// keypoint (long dependent chains, few working warps per SM on a 100k-point sweep).  Here one THREAD owns one keypoint:
 //   * keypoints are processed in Morton order of their LiDAR-frame cell (sorted once per sweep), so the 32 lanes
 //     of a warp sit in the same few voxels and their 16-byte point loads hit the same L1 lines;
 //   * each thread probes its 27 voxels (16 B slot loads), keeps the present ones in a private list, and walks the
@@ -408,7 +407,7 @@ __global__ void __launch_bounds__(kFastThreads, MINB) k1_fast(const __grid_const
 // Split form of the pass: k1_scan (LPK lanes per keypoint, FP32 selection) -> k1_fit (thread per keypoint, FP64).
 //
 // k1_fast is bound by the length of ONE thread's dependent chain (a 100k-point sweep is a single wave of 21 warps per
-// SM: time = latency of a warp that probes, scans ~270 candidates, finishes and fits, profiles/README.md).  The split
+// SM: time = latency of a warp that probes, scans its candidates, finishes and fits).  The split
 // form cuts that chain where it can be cut:
 //   * k1_scan gives every keypoint LPK lanes: the 27 probes are dealt to the lanes (results shared through shared
 //     memory), every voxel's candidates are dealt round-robin, each lane keeps only its NLS best packed keys (NLS < NL:
@@ -1238,7 +1237,7 @@ k_sweep_order_cluster(const double* __restrict__ raw, int n, double cell, unsign
     }
 }
 
-// round-2 first version, kept selectable for the A/B in profiles/ (keys re-read from HBM in the scatter phase)
+// first version, kept selectable for A/B runs (keys re-read from HBM in the scatter phase)
 __global__ void __launch_bounds__(kSortThreads, 1)
 k_sweep_order_cluster_v1(const double* __restrict__ raw, long long n, double cell, unsigned* keys_a, unsigned* idx_a, unsigned* keys_b, unsigned* order_out) {
     cg::cluster_group cluster = cg::this_cluster();
@@ -1455,7 +1454,7 @@ static int fast_minb() {   // SRL_FAST_MINB=4|5|6|8 selects the compiled variant
     }
     return g_fast_minb;
 }
-int k1_fast_lanes_per_keypoint() {     // SRL_FAST_LPK=1|2|4 (default 1: measured fastest, profiles/README.md)
+int k1_fast_lanes_per_keypoint() {     // SRL_FAST_LPK=1|2|4 (default 1)
     if (g_fast_lpk < 0) {
         const char* e = getenv("SRL_FAST_LPK");
         const int v = e ? atoi(e) : 1;
@@ -1513,7 +1512,7 @@ cudaError_t launch_k1_split(const FastArgs& a, long long n, int max_grid, bool d
     return launch_pass_kernel(fit, a, (unsigned)grid_b, kFastThreads, 0, stream, pdl);
 }
 
-cudaError_t preload_fast_kernels(int device) {
+cudaError_t preload_fast_kernels(int device, size_t* max_local) {
     upload_fast_offsets(device);
     cudaFuncAttributes at;
     const FastFn fns[] = {k1_scan<4, 14, 8>, k1_scan<4, 14, 6>, k1_scan<2, 20, 8>, k1_scan<2, 20, 6>,
@@ -1522,6 +1521,7 @@ cudaError_t preload_fast_kernels(int device) {
     for (FastFn fn : fns) {
         const cudaError_t e = cudaFuncGetAttributes(&at, fn);
         if (e != cudaSuccess) return e;
+        if (at.localSizeBytes > *max_local) *max_local = at.localSizeBytes;
     }
     return cudaSuccess;
 }

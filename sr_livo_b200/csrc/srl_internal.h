@@ -263,9 +263,10 @@ __device__ __forceinline__ void publish_sums_to_loop(IekfDev* dev, unsigned long
 #endif
 
 cudaError_t launch_k1_fast(const FastArgs& a, int grid, bool debug, int device, cudaStream_t stream);
-// load every pass kernel (CUDA loads lazily at first launch, and a load waits for running kernels) and the offset tables
-cudaError_t preload_fast_kernels(int device);
-cudaError_t preload_assoc_kernels(int device, int K);
+// load every pass kernel (CUDA loads lazily at first launch, and a load waits for running kernels) and the offset tables;
+// *max_local is raised to the largest per-thread local memory (spill frame) of the kernels loaded
+cudaError_t preload_fast_kernels(int device, size_t* max_local);
+cudaError_t preload_assoc_kernels(int device, int K, size_t* max_local);
 constexpr int kSplitSlots = 23;   // = NS of srl_fast.cu: candidate slots k1_scan hands to k1_fit per keypoint
 cudaError_t launch_k1_split(const FastArgs& a, long long n, int max_grid, bool debug, int device, cudaStream_t stream, bool pdl);
 // <<<>>> with the programmatic-stream-serialization attribute when pdl is set
@@ -307,7 +308,7 @@ struct srl_ctx {
     int device = 0;
     cudaStream_t stream = nullptr;
     bool own_stream = false;
-    int sm_count = 148;
+    int sm_count = 132;
     std::string err;
     int64_t launches = 0;
     // optional CUDA-event timing of k1_assoc

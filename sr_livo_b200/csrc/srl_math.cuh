@@ -1,6 +1,6 @@
 // srl_math.cuh — per-keypoint FP64 math of the scan-matching kernel, host+device.
 //
-// Everything here is the B200 implementation of what the reference does per keypoint after the
+// Everything here is the GPU implementation of what the reference does per keypoint after the
 // neighbour search: computeNeighborhoodDistribution (src/optimize.cpp:316-353), the normal flip and
 // weight (src/optimize.cpp:42-61,87-88), the signed point-to-plane distance and the 1x6 Jacobian
 // (src/optimize.cpp:90-101).  It is compiled for the device (phase 2 of k1_assoc, one thread per

@@ -505,6 +505,46 @@ def test_device_resident_loop_equals_host_driven_loop(L, small_world, kw):
     assert np.allclose(qd, qh, atol=1e-11) and np.allclose(td, th, atol=1e-11)
 
 
+_FAST_LOOP_WORKER = r"""
+import sys
+sys.path.insert(0, sys.argv[1])
+import numpy as np
+from sr_livo_b200 import lio, synth
+pts = synth.sample_map_points(80.0, 60.0, seed=1)
+sw = synth.make_sweep(4000, seed=1000, yaw=0.5)
+L = lio.LioOptimization(max_voxels=1 << 16, sweep_capacity=8192)
+L.addPointsToMap(pts)
+L.ctx.set_option("k1_variant", 1)                       # k1_fast + exact fallback, first launched inside the device loop
+prm = lio.r3live_params(max_num_residuals=2 ** 31 - 1, threshold_translation_norm=0.0)
+out = {}
+for mode in (1, 0):
+    L.ctx.set_option("device_loop", mode)
+    L.setKeypoints(sw.raw_xyz)
+    L.eskf_pro = lio.EskfEstimator(p=sw.t_init.copy(), q=sw.q_init.copy(), cov=synth.prior_covariance())
+    summ, fq, ft = L.updateIEKF(prm, sw.t_last)
+    out[mode] = (summ, fq, ft, L.eskf_pro)
+(sd, qd, td, ed), (sh, qh, th, eh) = out[1], out[0]
+assert sd.success and (sd.passes_run, sd.num_residuals_used) == (sh.passes_run, sh.num_residuals_used)
+assert np.allclose(ed.p, eh.p, rtol=1e-9, atol=1e-11) and np.allclose(ed.q, eh.q, rtol=1e-9, atol=1e-11)
+assert np.allclose(qd, qh, atol=1e-11) and np.allclose(td, th, atol=1e-11)
+L.close()
+print("ok")
+"""
+
+
+def test_device_resident_loop_with_the_thread_per_keypoint_pass(tmp_path):
+    """k1_fast (k1_variant 1) launched for the first time in a process inside the device-resident loop: its spill frame is
+    larger than any kernel launched before, so the context's local-memory reservation must already fit it (the driver grows
+    it only on an idle device, which never happens while the persistent ESIKF block waits for the pass).  A fresh process,
+    because the reservation outlives every LioOptimization of the process."""
+    import os, subprocess, sys
+    script = tmp_path / "fast_loop_worker.py"
+    script.write_text(_FAST_LOOP_WORKER)
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    r = subprocess.run([sys.executable, str(script), root], capture_output=True, text=True, timeout=600)
+    assert r.returncode == 0 and "ok" in r.stdout, (r.stdout + r.stderr)[-3000:]
+
+
 def test_update_iekf_reports_too_few_residuals(L, small_world):
     from sr_livo_b200 import lio
     om, sw = _load_world(L, small_world)
@@ -1105,62 +1145,78 @@ def test_fused_peer_memory_exchange_ranks(tmp_path, world):
         assert p.returncode == 0, o[-3000:]
 
 
-# ---- the CUDA path against the REFERENCE'S OWN CODE (oracle/_ref/libsrl_reference.so, compiled where it lies) ------
-def _reference_or_skip():
-    from oracle import reference_py as Rf
-    if not Rf.available():
-        pytest.skip("oracle/_ref/libsrl_reference.so did not travel to this box")
-    return Rf
+# ---- the CUDA path against the REFERENCE'S OWN CODE -----------------------------------------------------------------
+# tests/golden/reference_small_world.npz holds what the reference's own sources (compiled by oracle/Makefile) returned on the
+# small_world fixture (tests/golden/make_reference_golden.py).  Pass rows and transformed keypoints are stored as digests: the
+# oracle must reproduce them bit for bit, and the GPU is then compared with the oracle's arrays.
+@pytest.fixture(scope="module")
+def ref_small():
+    import os
+    return np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_small_world.npz"))
 
 
-@pytest.mark.parametrize("kw", [dict(max_num_residuals=BIG), dict(max_num_residuals=BIG, frame_id=5), dict(max_num_residuals=600)])
-def test_gpu_pass_equals_the_compiled_reference(L, small_world, kw):
-    """One ESIKF pass on the GPU vs lioOptimization::buildPlaneResiduals of the reference's own src/optimize.cpp (no oracle in
-    between): transformed keypoints bit for bit, the same keypoints accepted in the same order, rows within 1e-5."""
+def _sha256(a):
+    import hashlib
+    return hashlib.sha256(np.ascontiguousarray(a, np.float64).tobytes()).hexdigest()
+
+
+_REF_PASS_KW = [dict(max_num_residuals=BIG), dict(max_num_residuals=BIG, frame_id=5), dict(max_num_residuals=600)]
+
+
+@pytest.mark.parametrize("kw", _REF_PASS_KW)
+def test_gpu_pass_equals_the_compiled_reference(L, small_world, ref_small, kw):
+    """One ESIKF pass on the GPU vs lioOptimization::buildPlaneResiduals of the reference's own src/optimize.cpp: transformed
+    keypoints bit for bit, the same keypoints accepted in the same order, rows within 1e-5."""
     from sr_livo_b200 import lio
-    Rf = _reference_or_skip()
+    i = _REF_PASS_KW.index(kw)
     om, sw = _load_world(L, small_world)
-    ref = Rf.Reference()
-    ref.load(*om.snapshot())
     L.setKeypoints(sw.raw_xyz)
     g = L.buildPlaneResiduals(lio.r3live_params(**kw), sw.q_init, sw.t_init, sw.t_last, debug=True)
-    r = ref.build_plane_residuals(sw.raw_xyz, sw.q_init, sw.t_init, sw.t_last, O.r3live_params(**kw))
-    assert not r["threw"] and r["success"] == g.success and r["num_residuals_used"] == g.num_residuals
+    o = om.build_plane_residuals(sw.raw_xyz, sw.q_init, sw.t_init, sw.t_last, O.r3live_params(**kw), debug=True)
+    want_rows = o.plane[o.status == 2][:, :15]
+    # the oracle's arrays are the reference's, bit for bit
+    assert _sha256(want_rows) == str(ref_small[f"pass{i}_rows_sha256"]) and _sha256(o.world_xyz) == str(ref_small[f"pass{i}_world_sha256"])
+    assert o.loss_sum == float(ref_small[f"pass{i}_loss"])
+    assert bool(ref_small[f"pass{i}_success"]) == g.success and int(ref_small[f"pass{i}_num_residuals"]) == g.num_residuals
     visited = g.status >= 0
-    assert np.array_equal(g.world_xyz[visited], r["world_xyz"][visited])
+    assert np.array_equal(g.world_xyz[visited], o.world_xyz[visited])
     got = g.plane[g.status == 2][:, :15]
-    assert got.shape == r["rows"].shape
-    scale = np.maximum(np.abs(r["rows"]).max(axis=0), 1e-12)
-    assert np.all(np.abs(got - r["rows"]) <= REL * scale)
-    assert abs(g.loss_sum - r["loss_sum"]) <= REL * r["loss_sum"]
+    assert got.shape == want_rows.shape
+    scale = np.maximum(np.abs(want_rows).max(axis=0), 1e-12)
+    assert np.all(np.abs(got - want_rows) <= REL * scale)
+    assert abs(g.loss_sum - o.loss_sum) <= REL * o.loss_sum
 
 
-def test_gpu_update_equals_the_compiled_reference(L, small_world):
+def test_gpu_update_equals_the_compiled_reference(L, small_world, ref_small):
     """updateIEKF on the GPU (device-resident loop) vs the reference's own updateIEKF + eskfEstimator::observe: state 1e-5."""
     from sr_livo_b200 import lio
-    Rf = _reference_or_skip()
     om, sw = _load_world(L, small_world)
-    ref = Rf.Reference()
-    ref.load(*om.snapshot())
     P = synth.prior_covariance()
-    for kw in (dict(max_num_residuals=BIG), dict(max_num_residuals=600)):
+    for i, kw in enumerate((dict(max_num_residuals=BIG), dict(max_num_residuals=600))):
         L.setKeypoints(sw.raw_xyz)
         L.eskf_pro = lio.EskfEstimator(p=sw.t_init.copy(), q=sw.q_init.copy(), v=np.array([0.3, 0.0, 0.0]), cov=P.copy())
         summ, fq, ft = L.updateIEKF(lio.r3live_params(**kw), sw.t_last)
-        r = ref.update_iekf(sw.raw_xyz, O.Eskf(p=sw.t_init.copy(), q=sw.q_init.copy(), v=np.array([0.3, 0.0, 0.0]), cov=P.copy()), sw.t_last,
-                            O.r3live_params(**kw))
-        assert not r["threw"] and summ.success == r["success"] and summ.num_residuals_used == r["num_residuals_used"]
+        r = {k: ref_small[f"update{i}_{k}"] for k in ("p", "q", "v", "ba", "bg", "g", "cov", "frame_q", "frame_t", "success", "num_residuals")}
+        assert summ.success == bool(r["success"]) and summ.num_residuals_used == int(r["num_residuals"])
         for f in ("p", "q", "v", "ba", "bg", "g"):
-            assert np.allclose(getattr(L.eskf_pro, f), getattr(r["eskf"], f), rtol=REL, atol=1e-9), f
-        assert np.allclose(L.eskf_pro.cov, r["eskf"].cov, rtol=1e-4, atol=1e-12)
+            assert np.allclose(getattr(L.eskf_pro, f), r[f], rtol=REL, atol=1e-9), f
+        assert np.allclose(L.eskf_pro.cov, r["cov"], rtol=1e-4, atol=1e-12)
         assert np.allclose(fq, r["frame_q"], atol=1e-9) and np.allclose(ft, r["frame_t"], atol=1e-9)
+
+
+def _reference_or_skip():
+    from oracle import reference_py as Rf
+    if not Rf.available():
+        pytest.skip("oracle/_ref/libsrl_reference.so not built (needs the reference source tree)")
+    return Rf
 
 
 def test_reference_runs_on_the_gpu_backend(small_world):
     """The maintainer patch of INTEGRATION.md section 2, for real: oracle/_ref/libsrl_reference_gpu.so is the reference's own objects
     with lioOptimization::updateIEKF and ::addPointsToMap replaced at link time by the product's C++ adapter
     (include/srlivo_b200_lio.hpp -> C ABI -> CUDA).  The reference's unmodified optimize() (gridSampling -> updateIEKF ->
-    transformPoint) then registers a sweep through its own call sites on the GPU; the result equals the unpatched reference's."""
+    transformPoint) then registers a sweep through its own call sites on the GPU; the result equals the unpatched reference's.
+    It links the reference's own objects, so it runs only where oracle/Makefile could build them."""
     Rf = _reference_or_skip()
     if not Rf.available(gpu=True):
         pytest.skip("oracle/_ref/libsrl_reference_gpu.so did not travel to this box")
