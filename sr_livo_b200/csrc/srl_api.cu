@@ -875,7 +875,8 @@ int srl_update_iekf_dist(srl_ctx* ctx, srl_comm* comm, srl_map* map, srl_sweep* 
         if ((rc = launch_pass(ctx, sw, a, false)) != SRL_OK) return rc;     // also valid for an empty shard
         double* h = ctx->h_out32;
         if ((rc = wait_host_result(ctx, a)) != SRL_OK) return rc;
-        if (h[0] != h[0]) return set_err(ctx, SRL_COMM_ERROR, "peer exchange timed out (a rank did not reach this pass)");
+        // a failed exchange makes all 32 sums NaN; [31] is a count, which a NaN Jacobian (NaN planarity) never turns into NaN
+        if (h[31] != h[31]) return set_err(ctx, SRL_COMM_ERROR, "peer exchange timed out (a rank did not reach this pass)");
         srl_normal_eq ne;
         unpack32(h, &ne, (long long)sw->n);
         ++passes;

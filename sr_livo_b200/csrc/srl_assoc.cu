@@ -488,6 +488,8 @@ __global__ void __launch_bounds__(kK1Threads, MINB) k1_assoc(const __grid_consta
 #pragma unroll
                 for (int i = 0; i < 6; ++i) rr[i] = row.J[i];
                 rr[6] = h; rr[7] = row.distance * row.distance;
+                // k2_cap_reduce reads NaN planarity from rr[0]: set it explicitly, the weight is finite when power_planarity == 0
+                if (row.nan_planarity) rr[0] = __longlong_as_double(0x7ff8000000000000ll);
             }
             if (DEBUG && A.dbg_plane) {
                 double* d = A.dbg_plane + 16 * k;
@@ -597,7 +599,7 @@ __global__ void __launch_bounds__(1024, 1) k2_cap_reduce(const double* __restric
         const long long kstar = s_found ? s_kstar : (long long)0x7fffffffffffffffLL;
         if (k < k_end && k <= kstar) {
             if (st >= 1) n_full += 1.0;
-            if (st >= 1 && rows[8 * k] != rows[8 * k]) n_nan += 1.0;   // NaN planarity -> NaN weight -> NaN Jacobian (the reference throws, :348)
+            if (st >= 1 && rows[8 * k] != rows[8 * k]) n_nan += 1.0;   // rows[8k] = NaN marks NaN planarity (the reference throws, :348)
             if (a) {
                 const double* r = rows + 8 * k;
                 int idx = 0;

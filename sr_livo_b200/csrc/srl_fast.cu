@@ -900,6 +900,7 @@ __global__ void __launch_bounds__(kFastThreads, MINB) k1_fit(const __grid_consta
 #pragma unroll
                 for (int i = 0; i < 6; ++i) rr[i] = row.J[i];
                 rr[6] = h; rr[7] = row.distance * row.distance;
+                if (row.nan_planarity) rr[0] = __longlong_as_double(0x7ff8000000000000ll);   // the flag k2_cap_reduce reads
             }
             if (DEBUG) {
                 if (A.dbg_plane) {

@@ -361,7 +361,8 @@ __global__ void __launch_bounds__(kIekfThreads, 1) k_iekf_loop(const __grid_cons
             // what srl_update_iekf checks before the step: exchange failure, NaN planarity (:348), too few residuals (:110-123,:155)
             const double nres = S.sums[28];
             int fail = SRL_OK;
-            if (S.sums[0] != S.sums[0] && A.world > 1) fail = SRL_COMM_ERROR;
+            // a failed exchange makes all 32 sums NaN; [31] is a count, which a NaN Jacobian (NaN planarity) never turns into NaN
+            if (S.sums[31] != S.sums[31] && A.world > 1) fail = SRL_COMM_ERROR;
             else if (S.sums[31] > 0.0) fail = SRL_NAN_PLANARITY;
             else if ((long long)llrint(nres) < (long long)init.min_neighbors) fail = SRL_TOO_FEW_RESIDUALS;
             passes_run += 1;

@@ -341,6 +341,21 @@ SRL_HD void plane_residual(const NB& nbv, int K, double n0x, double n0y, double 
         double dx = (double)x - mx, dy = (double)y - my, dz = (double)z - mz;
         c00 += dx * dx; c01 += dx * dy; c02 += dx * dz; c11 += dy * dy; c12 += dy * dz; c22 += dz * dz;
     }
+    // K copies of one point: the reference's scatter is exactly 0, its a2D 0 / 0, and it throws (:348).  The device's
+    // arithmetic (a rounded 1 / K, contracted products) can leave a scatter of a few FP64 ulp^2 instead -- k1_fast's fit
+    // returned a2D ~ -2e-9 for such a neighbourhood.  That residue stays below 2^-90 |nearest|^2 (a mean off by 2 ulp at
+    // most), so only a scatter that small has its points compared with the nearest one.
+    bool collapsed = false;
+    if (!(c00 + c11 + c22 > 8.0779356694631609e-28 * (n0x * n0x + n0y * n0y + n0z * n0z))) {
+        collapsed = true;
+#pragma unroll
+        for (int j = 0; j < (KS > 0 ? KS : K); ++j) {
+            if (!nbv.use(j)) continue;
+            float x, y, z;
+            nbv.get(j, x, y, z);
+            collapsed = collapsed && (double)x == n0x && (double)y == n0y && (double)z == n0z;
+        }
+    }
     double ev[3], nx, ny, nz;
 #if defined(__CUDA_ARCH__)
     if (!eig3_sym_closed(c00, c01, c11, c02, c12, c22, ev, nx, ny, nz))
@@ -353,6 +368,7 @@ SRL_HD void plane_residual(const NB& nbv, int K, double n0x, double n0y, double 
     double sigma_1 = sqrt(fabs(ev[2])), sigma_2 = sqrt(fabs(ev[1])), sigma_3 = sqrt(fabs(ev[0]));
     double a2D = (sigma_2 - sigma_3) / sigma_1;           // src/optimize.cpp:343-346
 #endif
+    if (collapsed) a2D = nan("");
     out.a2D = a2D;
     out.nan_planarity = (a2D != a2D) ? 1 : 0;
     double planarity_weight = (c.power == 2.0) ? a2D * a2D : pow(a2D, c.power);   // :47
