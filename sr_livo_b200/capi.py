@@ -84,7 +84,7 @@ EXPORTS = [
     "srl_sweep_set_shard", "srl_build_plane_residuals", "srl_build_plane_residuals_async", "srl_normal_eq_unpack",
     "srl_iekf_begin", "srl_iekf_step", "srl_update_iekf", "srl_comm_create", "srl_comm_destroy", "srl_comm_export", "srl_comm_connect",
     "srl_update_iekf_dist", "srl_optimize_host", "srl_optimize_host_dist", "srl_shard_range", "srl_sweep_transform_device",
-    "srl_grid_sampling", "srl_eskf_observe", "srl_host_plane_fit",
+    "srl_grid_sampling", "srl_eskf_observe", "srl_host_plane_fit", "srl_iekf_replay",
     "srl_distort_frame_by_constant", "srl_distort_frame_by_imu", "srl_transform_all_imu_point",
     "srl_color_map_create", "srl_color_map_destroy", "srl_color_map_voxels", "srl_color_map_stats", "srl_color_map_add_points",
     "srl_color_map_render_recent", "srl_color_map_download_state", "srl_color_map_download_lists",
@@ -163,6 +163,7 @@ def lib():
     L.srl_distort_frame_by_imu.argtypes = [vp, vp, vp, sz, vp, sz, dbl, vp, vp, vp, C.POINTER(i64)]
     L.srl_transform_all_imu_point.argtypes = [vp, vp, sz, vp, vp, vp, vp]
     L.srl_host_plane_fit.argtypes = [vp, i32, vp, vp, vp]
+    L.srl_iekf_replay.argtypes = [vp, C.POINTER(EskfState), vp, vp, C.POINTER(IcpParams), vp, i32, i64, C.POINTER(IekfSummary)]
     L.srl_color_map_create.argtypes = [vp, dbl, i32, sz, dbl, C.POINTER(vp)]
     L.srl_color_map_destroy.argtypes = [vp]
     L.srl_color_map_destroy.restype = None

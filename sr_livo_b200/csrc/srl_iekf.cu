@@ -18,8 +18,10 @@
 // columns of the result (:234-242).  With A = P/c and M = I6 + HTH * A[0:6,0:6] the Woodbury identity gives
 //     ((A^-1 + E HTH E^T)^-1)[:, 0:6] = A[:, 0:6] * M^-1        (E = first six columns of I17)
 // exactly, so the step needs one 6x6 Gauss-Jordan inverse (one warp, a row per lane) instead of two 17x17 inverses; the
-// result differs from the reference's double inversion by rounding only (the parity tests bound the difference at 1e-5
-// of the state, 1e-4 of the covariance).  Everything else keeps the reference's operation order, including the in-place
+// result differs from the reference's double inversion by rounding only.  Against a 50-digit evaluation of the reference's
+// formula (tests/test_iekf_device.py, DESIGN §4 "Algebra") the error of this form grows with cond(M), that of the double
+// inversion with cond(P) + cond(P^-1 + HTH): on ill-conditioned covariances the device sits closer to the exact result
+// than the host loop and the reference do.  Everything else keeps the reference's operation order, including the in-place
 // column loops of the posterior covariance that read the pre-update matrix (:287-297).  The 3x3 / quaternion chains that
 // do not depend on each other run on different warps.
 #include "srl_eskf_math.cuh"
@@ -440,6 +442,28 @@ __global__ void __launch_bounds__(kIekfThreads, 1) k_iekf_loop(const __grid_cons
         __syncthreads();
         iekf_pre(S, laser_cov);   // for the next pass, in the shadow of its kernels
     }
+}
+
+// ---- replay (srl_iekf_replay): one warp stands in for a pass.  It waits for the pass's pose exactly like a pass kernel
+//      (or leaves when the loop has ended), optionally spins a bounded number of clock ticks, then hands block `p` of the
+//      given sums to the loop the way a pass's last block does.  The pass constants it loads are never read.
+__global__ void __launch_bounds__(32) k_iekf_feed(const __grid_constant__ IekfFeedArgs A) {
+    __shared__ PassConst s_c;
+    if (!load_pass_const(A.dev, A.wait_pose, A.ticket, A.end_ticket, A.c, s_c)) return;
+    if (A.delay_cycles > 0) {
+        const long long t0 = clock64();
+        while (clock64() - t0 < A.delay_cycles) {}
+    }
+    __syncwarp();
+    publish_sums_to_loop(A.dev, A.ticket, A.sums[threadIdx.x], threadIdx.x);
+}
+cudaError_t preload_iekf_feed() {
+    cudaFuncAttributes at;
+    return cudaFuncGetAttributes(&at, k_iekf_feed);
+}
+cudaError_t launch_iekf_feed(const IekfFeedArgs& a, cudaStream_t stream) {
+    k_iekf_feed<<<1, 32, 0, stream>>>(a);
+    return cudaGetLastError();
 }
 
 __global__ void k_iekf_abort(IekfDev* D) { *reinterpret_cast<volatile int*>(&D->abort) = 1; }

@@ -86,6 +86,16 @@ struct IekfLoopArgs {
 };
 cudaError_t launch_iekf_loop(const IekfLoopArgs& a, cudaStream_t stream);
 cudaError_t launch_iekf_abort(IekfDev* dev, cudaStream_t stream);
+struct IekfFeedArgs {         // srl_iekf_replay: a one-warp stand-in for pass `ticket - base` (k_iekf_feed)
+    IekfDev* dev;
+    const double* sums;       // device, the 32 sums this pass hands to the loop
+    unsigned long long ticket, end_ticket;
+    int wait_pose;
+    long long delay_cycles;   // > 0: spin this many SM clock ticks before publishing
+    PassConst c;              // by-value constants of load_pass_const (unused)
+};
+cudaError_t preload_iekf_feed();
+cudaError_t launch_iekf_feed(const IekfFeedArgs& a, cudaStream_t stream);
 cudaError_t probe_concurrent_kernels(cudaStream_t side, cudaStream_t main_stream, int* d_two_ints, bool* concurrent);
 
 #if defined(__CUDACC__)
