@@ -144,12 +144,15 @@ int srl_ctx_set_timing(srl_ctx* ctx, int enable);
  * flagged nothing, 0: always in the fallback launch), "fast_force_ambiguous_mod" (N > 0:
  * k1_fast hands every N-th keypoint to k1_assoc, to test the hand-over), "device_loop" (1 default: srl_update_iekf[_dist]
  * keep the whole iterated update on the GPU — a persistent block runs the ESIKF algebra between the passes, all passes are
- * enqueued at once, one host wait; 0: the host-driven loop, which is also used under kernel-serialising tools and for the
- * residual cap), "pdl" (1 default: programmatic dependent launch of the pass kernels in the device loop), "eager_order"
+ * enqueued at once, one host wait, with or without the max_num_residuals cap; 0: the host-driven loop, which is also used
+ * under kernel-serialising tools), "pdl" (1 default: programmatic dependent launch of the pass kernels in the device loop), "eager_order"
  * (1 default: a sweep is Morton-ordered right behind its upload instead of at its first pass).  Counters: "exact_fallbacks"
  * (keypoints whose FP32 selection in k1_assoc was ambiguous and were redone exactly), "fast_ambiguous" (keypoints
  * k1_fast handed to k1_assoc), "kernel_launches", "device_loop_active" (1 when the device-resident loop is in use on this
- * ctx), "iekf_step_cycles_avg" (SM clock ticks of one ESIKF step, sums seen -> pose published; resets on read). */
+ * ctx), "iekf_step_cycles_avg" (SM clock ticks of one ESIKF step, sums seen -> pose published; resets on read),
+ * "cap_chunks_run" (keypoint chunks of the capped pass whose kernels did work: summed over the passes of the last
+ * srl_update_iekf, or those of the last srl_build_plane_residuals call, whichever came last; 0 without the cap; reading
+ * it after the device-resident loop synchronises the ctx stream). */
 int srl_ctx_set_option(srl_ctx* ctx, const char* name, int64_t value);
 int srl_ctx_get_counter(srl_ctx* ctx, const char* name, int64_t* value);
 int srl_ctx_pass_time(srl_ctx* ctx, double* total_ms, int64_t* launches, int reset);

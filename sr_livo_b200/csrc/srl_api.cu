@@ -101,6 +101,20 @@ static void unpack32(const double* o, srl_normal_eq* out, long long n_keypoints)
     out->reserved = 0;
 }
 
+// Chunk schedule of the ordered residual cap, shared by the host-driven and the device-resident loop: chunk 0 is
+// [0, max(4096, 2 max(cap, 1))), each later chunk twice as long, the last one clipped to n.  Returns the n_chunks + 1
+// boundaries.  k2_cap_reduce adds each chunk's block sum to the pass's sums, so the boundaries fix the summation order:
+// with the same schedule both loops' capped sums are bitwise equal whenever the pass constants are.
+static std::vector<long long> cap_chunk_bounds(long long n, long long cap) {
+    std::vector<long long> b(1, 0);
+    long long chunk = std::max<long long>(4096, 2 * std::max<long long>(cap, 1));
+    while (b.back() < n) {
+        b.push_back(std::min(n, b.back() + chunk));
+        chunk *= 2;
+    }
+    return b;
+}
+
 constexpr bool kDefaultSplit = true;    // variant 0 (auto): k1_scan + k1_fit (H100, 100k-point sweep: 0.46 vs 0.75 ms per sweep for k1_fast in the same run, BASELINE.md)
 
 static int pass_grid(srl_ctx* ctx, long long n, int K, int nb) {
@@ -258,6 +272,7 @@ static int launch_pass(srl_ctx* ctx, srl_sweep* sw, const K1Args& a, bool debug,
         f.dbg_world = a.dbg_world; f.dbg_nbr = a.dbg_nbr; f.dbg_nbr_dist = a.dbg_nbr_dist; f.dbg_plane = a.dbg_plane; f.stats = a.stats;
         f.force_amb_mod = ctx->force_amb_mod;
         f.dev = a.dev; f.pose_ticket = a.pose_ticket; f.end_ticket = a.end_ticket; f.wait_pose = a.wait_pose;
+        f.cap_state = a.cap_state;
         const bool split = ctx->variant == 3 || (ctx->variant == 0 && kDefaultSplit);
         if (split) {
             f.cand_rows = sw->d_cand_rows; f.scan_count = ctx->d_scan_count;
@@ -316,6 +331,8 @@ int srl_ctx_create(int device, void* cuda_stream, srl_ctx** out) {
               cudaMalloc(&ctx->d_chunk_sums, (size_t)(ctx->max_grid / 32 + 1) * 32 * sizeof(double)) == cudaSuccess &&
               cudaMalloc(&ctx->d_out32, 64 * sizeof(double)) == cudaSuccess &&
               cudaMalloc(&ctx->d_k2_state, 4 * sizeof(long long)) == cudaSuccess &&
+              cudaMalloc(&ctx->d_cap_chunks, sizeof(unsigned long long)) == cudaSuccess &&
+              cudaMemset(ctx->d_cap_chunks, 0, sizeof(unsigned long long)) == cudaSuccess &&
               cudaMalloc(&ctx->d_stats, 6 * sizeof(unsigned long long)) == cudaSuccess &&
               cudaMalloc(&ctx->d_fast_out, 32 * sizeof(double)) == cudaSuccess &&
               cudaMalloc(&ctx->d_scan_count, sizeof(unsigned long long)) == cudaSuccess &&
@@ -346,7 +363,7 @@ void srl_ctx_destroy(srl_ctx* ctx) {
     cudaSetDevice(ctx->device);
     if (ctx->stream) cudaStreamSynchronize(ctx->stream);
     if (ctx->loop_stream) { cudaStreamSynchronize(ctx->loop_stream); cudaStreamDestroy(ctx->loop_stream); }
-    cudaFree(ctx->d_partials); cudaFree(ctx->d_ticket); cudaFree(ctx->d_chunk_tickets); cudaFree(ctx->d_chunk_sums); cudaFree(ctx->d_out32); cudaFree(ctx->d_k2_state); cudaFree(ctx->d_stats); cudaFree(ctx->d_fast_out); cudaFree(ctx->d_scan_count);
+    cudaFree(ctx->d_partials); cudaFree(ctx->d_ticket); cudaFree(ctx->d_chunk_tickets); cudaFree(ctx->d_chunk_sums); cudaFree(ctx->d_out32); cudaFree(ctx->d_k2_state); cudaFree(ctx->d_cap_chunks); cudaFree(ctx->d_stats); cudaFree(ctx->d_fast_out); cudaFree(ctx->d_scan_count);
     cudaFree(ctx->d_scratch); cudaFree(ctx->d_iekf);
     if (ctx->h_iekf) cudaFreeHost(ctx->h_iekf);
     for (auto& e : ctx->loop_ev0) if (e) cudaEventDestroy(e);
@@ -418,6 +435,17 @@ int srl_ctx_get_counter(srl_ctx* ctx, const char* name, int64_t* value) {
         SRL_CUDA(ctx, cudaMemcpyAsync(&v, ctx->d_stats + 1, sizeof(v), cudaMemcpyDeviceToHost, ctx->stream));
         SRL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
         *value = (int64_t)v;
+        return SRL_OK;
+    }
+    if (n == "cap_chunks_run") {   // capped chunks whose kernels did work in the last update (all its passes) or pass call
+        if (ctx->cap_chunks_on_device) {
+            unsigned long long v = 0;
+            SRL_CUDA(ctx, cudaMemcpyAsync(&v, ctx->d_cap_chunks, sizeof(v), cudaMemcpyDeviceToHost, ctx->stream));
+            SRL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+            ctx->cap_chunks_run = (int64_t)v;
+            ctx->cap_chunks_on_device = false;
+        }
+        *value = ctx->cap_chunks_run;
         return SRL_OK;
     }
     if (n == "kernel_launches") { *value = ctx->launches; return SRL_OK; }
@@ -548,6 +576,7 @@ int srl_normal_eq_unpack(const double* h_out32, srl_normal_eq* out) {
 int srl_build_plane_residuals(srl_ctx* ctx, srl_map* map, srl_sweep* sw, const srl_frame* frame, const srl_icp_params* prm,
                               srl_normal_eq* out, srl_debug_out* dbg) {
     if (!ctx || !out) return SRL_BAD_ARG;
+    ctx->cap_chunks_run = 0; ctx->cap_chunks_on_device = false;   // counter "cap_chunks_run": this call's chunks
     K1Args a;
     int rc = fill_k1_args(ctx, map, sw, frame, prm, a);
     if (rc != SRL_OK) return rc;
@@ -595,24 +624,26 @@ int srl_build_plane_residuals(srl_ctx* ctx, srl_map* map, srl_sweep* sw, const s
         SRL_CUDA(ctx, cudaMemsetAsync(d_cap_out, 0, 32 * sizeof(double), ctx->stream));
         SRL_CUDA(ctx, cudaMemsetAsync(ctx->d_k2_state, 0, 4 * sizeof(long long), ctx->stream));
         const long long cap = prm->max_num_residuals;
-        long long chunk = std::max<long long>(4096, 2 * std::max<long long>(cap, 1));
+        const std::vector<long long> bounds = cap_chunk_bounds(n, cap);
         double scanned = 0, nanf = 0;
-        long long begin = 0;
         long long st[4] = {0, 0, 0, 0};
-        while (begin < n) {
-            const long long end = std::min(n, begin + chunk);
+        for (size_t j = 0; j + 1 < bounds.size(); ++j) {
+            const long long begin = bounds[j], end = bounds[j + 1];
             K1Args c = a;
             c.k_begin = begin; c.k_end = end;
             if ((rc = launch_pass(ctx, sw, c, debug)) != SRL_OK) return rc;
-            SRL_CUDA(ctx, launch_k2(sw->d_rows, sw->d_status, begin, end, (int)cap, ctx->d_k2_state, d_cap_out, 0, ctx->stream));
+            K2Args k2;
+            std::memset(&k2, 0, sizeof(k2));
+            k2.rows = sw->d_rows; k2.status = sw->d_status; k2.k_begin = begin; k2.k_end = end; k2.cap = (int)cap;
+            k2.chunk = (int)j; k2.state = ctx->d_k2_state; k2.out32 = d_cap_out;
+            SRL_CUDA(ctx, launch_k2(k2, ctx->stream));
             ctx->launches += 1;
+            ctx->cap_chunks_run += 1;
             SRL_CUDA(ctx, cudaMemcpyAsync(h, ctx->d_out32, 32 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
             SRL_CUDA(ctx, cudaMemcpyAsync(st, ctx->d_k2_state, sizeof(st), cudaMemcpyDeviceToHost, ctx->stream));
             SRL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
             scanned += h[30]; nanf += h[31];
-            begin = end;
             if (st[1]) break;   // k* found: the reference loop has hit its `break`
-            chunk *= 2;
         }
         // keypoints after k* were never visited
         if (st[1] && st[2] + 1 < n) {
@@ -748,12 +779,28 @@ static int update_iekf_device(srl_ctx* ctx, srl_comm* comm, srl_map* map, srl_sw
     }
     IekfLoopArgs la;
     if ((rc = iekf_loop_args(ctx, eskf, frame_q, frame_t, a.c, prm, comm ? comm->world : 1, la)) != SRL_OK) return rc;
-    if ((rc = prepare_pass(ctx, sw, a)) != SRL_OK) return rc;
+    // ordered residual cap (unsharded sweep, src/optimize.cpp:107): every pass is the chunk schedule of the host-driven loop,
+    // each chunk's pass kernels followed by k2_cap_reduce; the chunks after k* leave at once
+    const long long n = a.k_end - a.k_begin;
+    const bool cap_mode = (long long)prm->max_num_residuals < n;
+    std::vector<long long> bounds;
+    if (cap_mode) {
+        if (comm || sw->shard_begin != 0 || sw->shard_end != sw->n)
+            return set_err(ctx, SRL_BAD_ARG, "max_num_residuals < shard size is only supported on an unsharded sweep");
+        if ((rc = ensure_buf(ctx, &sw->d_rows, sw->capacity * 8)) != SRL_OK) return rc;
+        if ((rc = ensure_buf(ctx, &sw->d_status, sw->capacity)) != SRL_OK) return rc;
+        a.rows = sw->d_rows; a.status = sw->d_status;
+        bounds = cap_chunk_bounds(n, prm->max_num_residuals);
+        SRL_CUDA(ctx, cudaMemsetAsync(ctx->d_cap_chunks, 0, sizeof(unsigned long long), ctx->stream));
+        ctx->cap_chunks_on_device = true;
+    }
+    if ((rc = prepare_pass(ctx, sw, a)) != SRL_OK) return rc;   // (with rows set: the same pass form the chunks launch)
     if (ctx->timing && !ctx->loop_ev0[0])
         for (int i = 0; i < kLoopMaxPasses; ++i) { SRL_CUDA(ctx, cudaEventCreate(&ctx->loop_ev0[i])); SRL_CUDA(ctx, cudaEventCreate(&ctx->loop_ev1[i])); }
     // the persistent ESIKF block first (side stream): it is resident before any pass kernel can wait for it
     SRL_CUDA(ctx, launch_iekf_loop(la, ctx->loop_stream));
     ctx->launches += 1;
+    const bool pdl = ctx->pdl && !ctx->timing;
     for (int p = 0; p < la.n_pass; ++p) {
         K1Args ap = a;
         ap.dev = ctx->d_iekf;
@@ -761,7 +808,26 @@ static int update_iekf_device(srl_ctx* ctx, srl_comm* comm, srl_map* map, srl_sw
         ap.end_ticket = la.base + 63ull;
         ap.wait_pose = p ? 1 : 0;                                    // pass 0: pose by value
         if (ctx->timing) cudaEventRecord(ctx->loop_ev0[p], ctx->stream);
-        if ((rc = launch_pass(ctx, sw, ap, false, false, ctx->pdl && !ctx->timing)) != SRL_OK) return iekf_loop_abort(ctx, rc);
+        if (!cap_mode) {
+            if ((rc = launch_pass(ctx, sw, ap, false, false, pdl)) != SRL_OK) return iekf_loop_abort(ctx, rc);
+        } else {
+            for (size_t j = 0; j + 1 < bounds.size(); ++j) {
+                K1Args c = ap;
+                c.k_begin = bounds[j]; c.k_end = bounds[j + 1];
+                c.cap_state = j ? ctx->d_k2_state : nullptr;
+                if ((rc = launch_pass(ctx, sw, c, false, false, pdl)) != SRL_OK) return iekf_loop_abort(ctx, rc);
+                K2Args k2;
+                std::memset(&k2, 0, sizeof(k2));
+                k2.rows = sw->d_rows; k2.status = sw->d_status; k2.k_begin = c.k_begin; k2.k_end = c.k_end;
+                k2.cap = (int)prm->max_num_residuals; k2.chunk = (int)j; k2.state = ctx->d_k2_state; k2.out32 = ctx->d_out32 + 32;
+                k2.last = j + 2 == bounds.size() ? 1 : 0;
+                k2.pass_out32 = ctx->d_out32; k2.chunks_run = ctx->d_cap_chunks;
+                k2.dev = ctx->d_iekf; k2.pose_ticket = ap.pose_ticket; k2.end_ticket = ap.end_ticket; k2.wait_pose = ap.wait_pose;
+                const cudaError_t e = launch_k2(k2, ctx->stream, pdl);
+                if (e != cudaSuccess) return iekf_loop_abort(ctx, cuda_fail(ctx, e, "launch_k2"));
+                ctx->launches += 1;
+            }
+        }
         if (ctx->timing) cudaEventRecord(ctx->loop_ev1[p], ctx->stream);
     }
     return iekf_loop_finish(ctx, la, ctx->timing, eskf, frame_q, frame_t, summary);
@@ -815,8 +881,15 @@ int srl_update_iekf(srl_ctx* ctx, srl_map* map, srl_sweep* sw, srl_eskf_state* e
                     const double t_last[3], const double R_il[9], const double t_il[3], const srl_icp_params* prm,
                     srl_iekf_summary* summary) {
     if (!ctx || !eskf || !frame_q || !frame_t || !t_last || !R_il || !t_il || !prm) return SRL_BAD_ARG;
-    if (device_loop_usable(ctx) && map && sw && !((long long)prm->max_num_residuals < (long long)(sw->shard_end - sw->shard_begin)))
-        return update_iekf_device(ctx, nullptr, map, sw, eskf, frame_q, frame_t, t_last, R_il, t_il, prm, summary);
+    ctx->cap_chunks_run = 0; ctx->cap_chunks_on_device = false;
+    if (device_loop_usable(ctx) && map && sw) {
+        // the ordered cap runs on the device loop on an unsharded, non-empty sweep; a sharded one takes the host loop, whose
+        // pass rejects it
+        const long long n = (long long)(sw->shard_end - sw->shard_begin);
+        const bool capped = (long long)prm->max_num_residuals < n;
+        if (!capped || (n > 0 && sw->shard_begin == 0 && sw->shard_end == sw->n))
+            return update_iekf_device(ctx, nullptr, map, sw, eskf, frame_q, frame_t, t_last, R_il, t_il, prm, summary);
+    }
     srl_iekf_iter it;
     int rc = srl_iekf_begin(eskf, prm, &it);
     if (rc != SRL_OK) return rc;
@@ -826,11 +899,14 @@ int srl_update_iekf(srl_ctx* ctx, srl_map* map, srl_sweep* sw, srl_eskf_state* e
     std::memcpy(fr.R_il, R_il, sizeof(fr.R_il));
     std::memcpy(fr.t_il, t_il, sizeof(fr.t_il));
     int passes = 0;
+    int64_t chunks = 0;
     for (;;) {
         std::memcpy(fr.q_cur, frame_q, sizeof(fr.q_cur));
         std::memcpy(fr.t_cur, frame_t, sizeof(fr.t_cur));
         srl_normal_eq ne;
         rc = srl_build_plane_residuals(ctx, map, sw, &fr, prm, &ne, nullptr);       // src/optimize.cpp:153
+        chunks += ctx->cap_chunks_run;                 // the pass counted its own chunks; the counter reports the update's
+        ctx->cap_chunks_run = chunks;
         ++passes;
         if (summary) { summary->passes_run = passes; summary->num_residuals_used = (int32_t)ne.num_residuals; }
         if (rc == SRL_TOO_FEW_RESIDUALS) { if (summary) summary->success = 0; return rc; }   // :155

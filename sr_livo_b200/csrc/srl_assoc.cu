@@ -273,6 +273,7 @@ __global__ void __launch_bounds__(kK1Threads, MINB) k1_assoc(const __grid_consta
     const int warp = threadIdx.x >> 5;
     __shared__ PassConst s_c;
     if (!load_pass_const(A.dev, A.wait_pose, A.pose_ticket, A.end_ticket, A.c, s_c)) return;   // device-resident loop already ended: nothing to do
+    if (cap_chunk_done(A.cap_state)) return;   // capped pass: k* is in an earlier chunk
     const PassConst& c = s_c;
     const int K = c.K;
     const int nb = c.nb;
@@ -302,7 +303,7 @@ __global__ void __launch_bounds__(kK1Threads, MINB) k1_assoc(const __grid_consta
             if (lane == 0 && finalised) A.stats[3] = 0ull;
             A.out32[lane] = tot;
             publish_to_host(A, tot, lane);
-            if (!finalised) publish_sums_to_loop(A.dev, A.pose_ticket, tot, lane);
+            if (!finalised && !A.rows) publish_sums_to_loop(A.dev, A.pose_ticket, tot, lane);   // capped: k2_cap_reduce publishes
         }
         return;
     }
@@ -539,7 +540,7 @@ __global__ void __launch_bounds__(kK1Threads, MINB) k1_assoc(const __grid_consta
             A.out32[lane] = tot;
             if (lane == 0) { *A.ticket = 0u; if (A.only_flagged && A.stats) A.stats[2] = 0ull; }
             publish_to_host(A, tot, lane);
-            publish_sums_to_loop(A.dev, A.pose_ticket, tot, lane);
+            if (!A.rows) publish_sums_to_loop(A.dev, A.pose_ticket, tot, lane);   // capped: k2_cap_reduce publishes
         }
     }
 }
@@ -550,26 +551,29 @@ __global__ void __launch_bounds__(kK1Threads, MINB) k1_assoc(const __grid_consta
 // so the rows that count are the accepted ones with k <= k*.  cap >= 1: k* = the cap-th accepted
 // keypoint; cap <= 0 (the compiled default -1): k* = the first keypoint with a full neighbourhood.
 // state[0] = running accepted count, state[1] = k* found flag, state[2] = k*
+// The chunks of a pass run in stream order; chunk 0 starts from a zero state, chunk j >= 1 continues from chunk j - 1's.
+// In the device-resident loop this kernel is a pass kernel like the others (tickets, PDL): chunks after k* leave at once,
+// and the chunk that finds k* (or the pass's last chunk) hands the capped sums to the ESIKF block.
 // ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(1024, 1) k2_cap_reduce(const double* __restrict__ rows, int* __restrict__ status,
-                                                          long long k_begin, long long k_end, int cap,
-                                                          long long* __restrict__ state, double* __restrict__ out32,
-                                                          int mark_unvisited) {
+__global__ void __launch_bounds__(1024, 1) k2_cap_reduce(const __grid_constant__ K2Args A) {
     __shared__ int s_scan[1024];
     __shared__ double s_red[32][33];
     __shared__ long long s_kstar;
     __shared__ int s_found;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    long long run_acc = state[0];
-    if (tid == 0) { s_found = (int)state[1]; s_kstar = state[2]; }
+    if (!wait_pass_ticket(A.dev, A.wait_pose, A.pose_ticket, A.end_ticket)) return;   // the loop has ended
+    const bool fresh = A.chunk == 0;
+    if (!fresh && __ldcg(A.state + 1)) return;   // k* is in an earlier chunk of this pass
+    long long run_acc = fresh ? 0 : A.state[0];
+    if (tid == 0) { s_found = fresh ? 0 : (int)A.state[1]; s_kstar = fresh ? 0 : A.state[2]; }
     __syncthreads();
     double acc[29];
 #pragma unroll
     for (int i = 0; i < 29; ++i) acc[i] = 0.0;
     double n_full = 0.0, n_nan = 0.0;
-    for (long long base = k_begin; base < k_end && !s_found; base += 1024) {
+    for (long long base = A.k_begin; base < A.k_end && !s_found; base += 1024) {
         const long long k = base + tid;
-        const int st = (k < k_end) ? status[k] : 0;
+        const int st = (k < A.k_end) ? A.status[k] : 0;
         const int a = (st == 2) ? 1 : 0;
         // inclusive block scan of accepted flags
         s_scan[tid] = a;
@@ -582,7 +586,7 @@ __global__ void __launch_bounds__(1024, 1) k2_cap_reduce(const double* __restric
         }
         const long long incl = run_acc + s_scan[tid];
         // k* candidate: full neighbourhood and running count >= cap
-        const bool is_kstar_cand = (st >= 1) && (incl >= (long long)cap);
+        const bool is_kstar_cand = (st >= 1) && (incl >= (long long)A.cap);
         // first such k in this chunk
         unsigned long long cand = is_kstar_cand ? (unsigned long long)k : ~0ull;
         // block min via shared
@@ -597,11 +601,11 @@ __global__ void __launch_bounds__(1024, 1) k2_cap_reduce(const double* __restric
         }
         __syncthreads();
         const long long kstar = s_found ? s_kstar : (long long)0x7fffffffffffffffLL;
-        if (k < k_end && k <= kstar) {
+        if (k < A.k_end && k <= kstar) {
             if (st >= 1) n_full += 1.0;
-            if (st >= 1 && rows[8 * k] != rows[8 * k]) n_nan += 1.0;   // rows[8k] = NaN marks NaN planarity (the reference throws, :348)
+            if (st >= 1 && A.rows[8 * k] != A.rows[8 * k]) n_nan += 1.0;   // rows[8k] = NaN marks NaN planarity (the reference throws, :348)
             if (a) {
-                const double* r = rows + 8 * k;
+                const double* r = A.rows + 8 * k;
                 int idx = 0;
 #pragma unroll
                 for (int p = 0; p < 6; ++p)
@@ -617,8 +621,8 @@ __global__ void __launch_bounds__(1024, 1) k2_cap_reduce(const double* __restric
         __syncthreads();
     }
     // keypoints after k* were never visited by the reference loop
-    if (mark_unvisited && s_found)
-        for (long long k = s_kstar + 1 + tid; k < k_end; k += 1024) status[k] = -1;
+    if (A.mark_unvisited && s_found)
+        for (long long k = s_kstar + 1 + tid; k < A.k_end; k += 1024) A.status[k] = -1;
     // fixed-order block reduction of the 30 components
     double comps[31];
 #pragma unroll
@@ -631,12 +635,18 @@ __global__ void __launch_bounds__(1024, 1) k2_cap_reduce(const double* __restric
         if (lane == 0) s_red[warp][i] = x;
     }
     __syncthreads();
-    if (warp == 0 && lane < 31) {
+    if (warp == 0) {
+        // lane l owns out32[l]: [31] = NaN-planarity keypoints the reference loop reached, [30] = candidates scanned
         double tot = 0.0;
-        for (int w = 0; w < 32; ++w) tot += s_red[w][lane];
-        out32[lane == 30 ? 31 : lane] += tot;   // chunks append; [31] = NaN-planarity keypoints the reference loop reached
+        const bool own = lane != 30 || A.pass_out32;
+        if (lane != 30) for (int w = 0; w < 32; ++w) tot += s_red[w][lane == 31 ? 30 : lane];
+        else if (A.pass_out32) tot = __ldcg(A.pass_out32 + 30);
+        double v = 0.0;
+        if (own) { v = (fresh ? 0.0 : A.out32[lane]) + tot; A.out32[lane] = v; }   // chunks append
+        if (lane == 0 && A.chunks_run) *A.chunks_run += 1ull;
+        if (A.dev && (s_found || A.last)) publish_sums_to_loop(A.dev, A.pose_ticket, v, lane);
     }
-    if (tid == 0) { state[0] = run_acc; state[1] = s_found; state[2] = s_kstar; }
+    if (tid == 0) { A.state[0] = run_acc; A.state[1] = s_found; A.state[2] = s_kstar; }
 }
 
 // transformPoint over a sweep (src/utility.cpp:314-318): world = R(q) * (R_il * raw + t_il) + t
@@ -721,6 +731,9 @@ cudaError_t preload_assoc_kernels(int device, int K, size_t* max_local) {
         if (e != cudaSuccess) return e;
         if (at.localSizeBytes > *max_local) *max_local = at.localSizeBytes;
     }
+    cudaError_t e = cudaFuncGetAttributes(&at, k2_cap_reduce);   // the capped pass's reduction runs behind the ESIKF block too
+    if (e != cudaSuccess) return e;
+    if (at.localSizeBytes > *max_local) *max_local = at.localSizeBytes;
     return cudaSuccess;
 }
 
@@ -733,10 +746,8 @@ int k1_max_blocks_per_sm(int K, int nb) {
     return nblk < 1 ? 1 : nblk;
 }
 
-cudaError_t launch_k2(const double* rows, int* status, long long k_begin, long long k_end, int cap, long long* state,
-                      double* out32, int mark_unvisited, cudaStream_t stream) {
-    k2_cap_reduce<<<1, 1024, 0, stream>>>(rows, status, k_begin, k_end, cap, state, out32, mark_unvisited);
-    return cudaGetLastError();
+cudaError_t launch_k2(const K2Args& a, cudaStream_t stream, bool pdl) {
+    return launch_pass_kernel(k2_cap_reduce, a, 1u, 1024u, 0, stream, pdl);
 }
 
 cudaError_t launch_transform(const double* raw, long long n, const PassConst& c, double* out, cudaStream_t stream) {

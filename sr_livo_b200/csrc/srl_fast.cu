@@ -485,6 +485,7 @@ __global__ void __launch_bounds__(kScanThreads, MINB) k1_scan(const __grid_const
     //  the compiler serialise them over the 32 / LPK distinct masks)
     __shared__ PassConst s_c;
     if (!load_pass_const(A.dev, A.wait_pose, A.pose_ticket, A.end_ticket, A.c, s_c)) return;   // device-resident loop already ended: nothing to do
+    if (cap_chunk_done(A.cap_state)) return;   // capped pass: k* is in an earlier chunk
     const PassConst& c = s_c;
     const int nb = c.nb;
     const int W = 2 * nb + 1;
@@ -791,6 +792,7 @@ __global__ void __launch_bounds__(kFastThreads, MINB) k1_fit(const __grid_consta
     const int warp = threadIdx.x >> 5;
     __shared__ PassConst s_c;
     if (!load_pass_const(A.dev, A.wait_pose, A.pose_ticket, A.end_ticket, A.c, s_c)) return;   // device-resident loop already ended: nothing to do
+    if (cap_chunk_done(A.cap_state)) return;   // capped pass: k* is in an earlier chunk
     const PassConst& c = s_c;
     const int nb = c.nb;
     const int W = 2 * nb + 1;
@@ -941,7 +943,7 @@ __global__ void __launch_bounds__(kFastThreads, MINB) k1_fit(const __grid_consta
                 }
             }
         }
-        if (valid && A.status && !ambiguous) A.status[k] = status;
+        if (valid && A.status && !ambiguous) A.status[k] = status;   // the fallback launch writes the flagged (ambiguous) ones
         __syncwarp();
         // components 0..20 = upper triangle of J^T J, 21..26 = J^T h, 27 d^2, 28 residuals, 29 full, 30 (scan count), 31 NaN
         {
@@ -1040,7 +1042,7 @@ __global__ void __launch_bounds__(kFastThreads, MINB) k1_fit(const __grid_consta
             if (final_here && lane == 0) A.stats[3] = 1ull;   // tells the fallback launch that the pass is already finalised
             A.out32[lane] = tot;
             if (lane == 0) *A.ticket = 0u;
-            if (final_here) publish_sums_to_loop(A.dev, A.pose_ticket, tot, lane);   // device-resident loop: the ESIKF block takes over
+            if (final_here && !A.rows) publish_sums_to_loop(A.dev, A.pose_ticket, tot, lane);   // device-resident loop: the ESIKF block takes over (capped: k2_cap_reduce does)
             if (A.host_out && final_here) {
                 A.host_out[lane] = tot;
                 __syncwarp();

@@ -186,6 +186,8 @@ struct K1Args {
     unsigned long long pose_ticket;   // with wait_pose the kernel first waits for pose_seq >= pose_ticket and takes its constants from
     unsigned long long end_ticket;   // dev->pc; pose_seq >= end_ticket says the loop has ended: the kernel leaves at once
     int wait_pose;
+    const long long* cap_state;  // chunk j >= 1 of a capped pass in the device-resident loop: k2_cap_reduce's state; the grid
+                                 // leaves when k* is already found (with rows set, k2_cap_reduce alone publishes the pass)
 };
 
 constexpr int kFastWarps = 4;
@@ -225,6 +227,24 @@ struct FastArgs {               // k1_fast (srl_fast.cu)
     double* rows;                     // optional n*8 per-keypoint rows (J6, h, d^2) for the ordered residual cap (k2_cap_reduce)
     unsigned int* chunk_tickets;      // k1_fit's two-level grid reduction: one ticket and one 32-double sum per chunk of 32 blocks
     double* chunk_sums;
+    const long long* cap_state;       // see K1Args::cap_state
+};
+
+struct K2Args {                 // k2_cap_reduce: one chunk of the ordered residual cap (srl_assoc.cu)
+    const double* rows;         // n*8 per-keypoint rows (J6, h, d^2) written by the chunk's pass kernels
+    int* status;                // n: 0 no full neighbourhood, 1 full, 2 accepted
+    long long k_begin, k_end;   // the chunk
+    int cap;
+    int chunk;                  // index of the chunk in its pass: chunk 0 starts from a zero state, so nothing is reset between passes
+    long long* state;           // [0] accepted so far, [1] k* found, [2] k*
+    double* out32;              // the pass's capped sums: chunk 0 writes them, later chunks add to them
+    int mark_unvisited;         // status -1 for the chunk's keypoints after k*
+    int last;                   // the pass's last chunk: it publishes even when k* was not found
+    const double* pass_out32;   // optional: the chunk's pass sums; their [30] (candidates scanned) is added to out32[30]
+    unsigned long long* chunks_run;   // optional device counter of the chunks that did work
+    IekfDev* dev;               // device-resident loop (see K1Args::dev): the chunk that finds k*, or the last one, publishes out32
+    unsigned long long pose_ticket, end_ticket;
+    int wait_pose;
 };
 
 #if defined(__CUDACC__)
@@ -237,10 +257,9 @@ __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;"
 // Every pass kernel reads its constants from shared memory: filled from the by-value argument (host-driven pass, pass 0
 // of the device-resident loop) or from the loop state once the ESIKF block has published them.  Returns false when the
 // loop has already ended (the whole grid leaves).
-__device__ __forceinline__ bool load_pass_const(const IekfDev* dev, int wait_pose, unsigned long long ticket, unsigned long long end_ticket,
-                                                const PassConst& by_value, PassConst& s_c) {
-    constexpr int ND = (int)(sizeof(PassConst) / sizeof(double));
-    static_assert(sizeof(PassConst) % sizeof(double) == 0, "PassConst is copied as doubles");
+// The ticket half of load_pass_const: lets the successor launch, waits for the predecessor, then (wait_pose) for the pose
+// of pass `ticket`.  Returns false when the loop has already ended (the whole grid leaves).
+__device__ __forceinline__ bool wait_pass_ticket(const IekfDev* dev, int wait_pose, unsigned long long ticket, unsigned long long end_ticket) {
     pdl_trigger();
     pdl_wait();
     if (dev && wait_pose) {
@@ -255,6 +274,20 @@ __device__ __forceinline__ bool load_pass_const(const IekfDev* dev, int wait_pos
         }
         __syncthreads();
         if (!s_go) return false;
+    }
+    return true;
+}
+// Chunk j >= 1 of a capped pass (device-resident loop): k* was found by an earlier chunk's k2_cap_reduce, which completed
+// before this kernel passed pdl_wait, so every thread reads the same word and the whole grid leaves together.
+__device__ __forceinline__ bool cap_chunk_done(const long long* cap_state) {
+    return cap_state && __ldcg(cap_state + 1) != 0;
+}
+__device__ __forceinline__ bool load_pass_const(const IekfDev* dev, int wait_pose, unsigned long long ticket, unsigned long long end_ticket,
+                                                const PassConst& by_value, PassConst& s_c) {
+    constexpr int ND = (int)(sizeof(PassConst) / sizeof(double));
+    static_assert(sizeof(PassConst) % sizeof(double) == 0, "PassConst is copied as doubles");
+    if (!wait_pass_ticket(dev, wait_pose, ticket, end_ticket)) return false;
+    if (dev && wait_pose) {
         if (threadIdx.x < ND) reinterpret_cast<double*>(&s_c)[threadIdx.x] = __ldcg(reinterpret_cast<const double*>(&dev->pc) + threadIdx.x);
     } else if (threadIdx.x < ND) {   // by value: the kernel argument is __grid_constant__, so it can be indexed like memory (a
         // copy by thread 0 alone kept every warp of the block at the barrier below for ~10 % of k1_fit's duration)
@@ -304,8 +337,7 @@ size_t k1_smem_bytes(int K);
 int k1_max_blocks_per_sm(int K, int nb);
 void k1_set_min_blocks(int v);
 cudaError_t launch_k1(const K1Args& a, int grid, bool debug, int device, cudaStream_t stream, bool pdl = false);
-cudaError_t launch_k2(const double* rows, int* status, long long k_begin, long long k_end, int cap, long long* state,
-                      double* out32, int mark_unvisited, cudaStream_t stream);
+cudaError_t launch_k2(const K2Args& a, cudaStream_t stream, bool pdl = false);
 cudaError_t launch_transform(const double* raw, long long n, const PassConst& c, double* out, cudaStream_t stream);
 
 // host-side pass constants from the reference's per-pass inputs (src/optimize.cpp:21-28,55-61)
@@ -341,6 +373,9 @@ struct srl_ctx {
     bool exchange_in_fit = true;    // option "exchange_in_fit" / SRL_EXCHANGE_IN_FIT: multi-GPU, k1_fit runs the exchange when it flagged nothing
     bool mapped_result = true;      // option "mapped_result": read a pass's sums through the mapped buffer (default) or by memcpy + sync
     long long* d_k2_state = nullptr;
+    unsigned long long* d_cap_chunks = nullptr;   // device-resident loop: k2_cap_reduce counts the capped chunks that did work
+    int64_t cap_chunks_run = 0;              // counter "cap_chunks_run": capped chunks processed by the last update's passes
+    bool cap_chunks_on_device = false;       // ... still to be read from d_cap_chunks
     unsigned long long* d_stats = nullptr;   // 4 counters
     double* d_fast_out = nullptr;            // k1_fast's 32 sums, added by the exact-fallback launch
     bool force_exact = false;
