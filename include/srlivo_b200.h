@@ -316,6 +316,14 @@ typedef struct srl_camera {      /* the state fields cloudFrame::project3dTo2d /
     double fov_margin;
     int32_t cols, rows;          /* image_cols, image_rows */
 } srl_camera;
+/* 1 <= max_num_points_in_voxel <= 128 (the shipped map_options use 50 and 100) and max_voxels * max(cap, 20) < 2^32 (32-bit
+ * point ids), else SRL_BAD_ARG.  Up to 20 points the voxel map keeps the LIO block layout (20 points per block; it also works
+ * with the LIO entry points); above 20 a block holds cap points and the LIO entry points (srl_map_insert*, srl_map_upload,
+ * srl_map_remove_far, srl_build_plane_residuals*, srl_update_iekf*, srl_optimize_host*) reject the map with SRL_BAD_ARG.
+ * HBM per point slot (max_voxels * max(cap, 20) slots): 16 B position + 40 B colour state + 4 B rgb id + 32-64 B fine-cell
+ * slot, i.e. about 10-13 GB for 2^20 voxels at cap 100; the caller sizes max_voxels.
+ * Keys (voxel and fine cell) are static_cast<short>(x / size) as the reference compiles on x86-64: the low 16 bits of the
+ * int32 truncation, so they wrap past |x / size| = 32767 like the reference's; NaN, +-inf and |x / size| >= 2^31 drop the point. */
 int srl_color_map_create(srl_ctx* ctx, double voxel_size, int32_t max_num_points_in_voxel, size_t max_voxels,
                          double min_distance_points, srl_color_map** out);
 void srl_color_map_destroy(srl_color_map* cm);

@@ -542,6 +542,7 @@ static int fill_k1_args(srl_ctx* ctx, srl_map* map, srl_sweep* sw, const srl_fra
     if (rc != SRL_OK) return rc;
     if (!map || !sw || !frame) return set_err(ctx, SRL_BAD_ARG, "null map/sweep/frame");
     if (map->ctx != ctx || sw->ctx != ctx) return set_err(ctx, SRL_BAD_ARG, "map/sweep belong to another ctx");
+    if ((rc = check_lio_map(ctx, map)) != SRL_OK) return rc;
     if (std::fabs(prm->size_voxel_map - map->voxel_size) > 0) return set_err(ctx, SRL_BAD_ARG, "icp size_voxel_map differs from the map's voxel size");
     std::memset(&a, 0, sizeof(a));
     make_pass_const(*frame, *prm, a.c);
@@ -881,6 +882,7 @@ int srl_update_iekf(srl_ctx* ctx, srl_map* map, srl_sweep* sw, srl_eskf_state* e
                     const double t_last[3], const double R_il[9], const double t_il[3], const srl_icp_params* prm,
                     srl_iekf_summary* summary) {
     if (!ctx || !eskf || !frame_q || !frame_t || !t_last || !R_il || !t_il || !prm) return SRL_BAD_ARG;
+    if (map && check_lio_map(ctx, map) != SRL_OK) return SRL_BAD_ARG;
     ctx->cap_chunks_run = 0; ctx->cap_chunks_on_device = false;
     if (device_loop_usable(ctx) && map && sw) {
         // the ordered cap runs on the device loop on an unsharded, non-empty sweep; a sharded one takes the host loop, whose
@@ -982,6 +984,7 @@ int srl_update_iekf_dist(srl_ctx* ctx, srl_comm* comm, srl_map* map, srl_sweep* 
                          const srl_icp_params* prm, srl_iekf_summary* summary) {
     if (!ctx || !comm || !eskf || !frame_q || !frame_t || !t_last || !R_il || !t_il || !prm) return SRL_BAD_ARG;
     if (comm->ctx != ctx || !comm->connected) return set_err(ctx, SRL_COMM_ERROR, "srl_comm is not connected");
+    if (map && check_lio_map(ctx, map) != SRL_OK) return SRL_BAD_ARG;
     SRL_CUDA(ctx, cudaSetDevice(ctx->device));
     if (map && sw && (long long)prm->max_num_residuals < (long long)sw->n)
         return set_err(ctx, SRL_BAD_ARG, "the sharded update does not implement the max_num_residuals cap");
@@ -1056,6 +1059,7 @@ int srl_optimize_host(srl_ctx* ctx, srl_map* map, srl_sweep* sw, const double* r
                       double frame_q[4], double frame_t[3], const double t_last[3], const double R_il[9], const double t_il[3],
                       const srl_icp_params* prm, srl_iekf_summary* summary, double* world_xyz_out) {
     if (!ctx || !sw) return SRL_BAD_ARG;
+    if (map && check_lio_map(ctx, map) != SRL_OK) return SRL_BAD_ARG;
     int rc = srl_sweep_upload(sw, raw_xyz, n);                                   // H2D of the keypoints
     if (rc != SRL_OK) return rc;
     rc = srl_update_iekf(ctx, map, sw, eskf, frame_q, frame_t, t_last, R_il, t_il, prm, summary);   // src/optimize.cpp:435
@@ -1087,6 +1091,7 @@ int srl_optimize_host_dist(srl_ctx* ctx, srl_comm* comm, srl_map* map, srl_sweep
                            const double t_il[3], const srl_icp_params* prm, srl_iekf_summary* summary, double* world_xyz_out,
                            size_t* shard_begin, size_t* shard_end) {
     if (!ctx || !comm || !sw || (n && !raw_xyz)) return SRL_BAD_ARG;
+    if (map && check_lio_map(ctx, map) != SRL_OK) return SRL_BAD_ARG;
     size_t b = 0, e = 0;
     srl_shard_range(n, comm->rank, comm->world, &b, &e);
     if (shard_begin) *shard_begin = b;

@@ -408,6 +408,8 @@ struct srl_map {
     srl_ctx* ctx = nullptr;
     double voxel_size = 1.0;
     int cap = 20;
+    int block_pts = srl::kBlockCap; // points per block of the pool (block stride = 4 * block_pts floats): kBlockCap for
+                                    // every map the LIO path accepts; cap for a colour map of cap > kBlockCap
     size_t max_voxels = 0;
     size_t capacity = 0;            // slots (power of two)
     srl::Slot* d_slots = nullptr;
@@ -453,6 +455,8 @@ int cuda_fail(srl_ctx* ctx, cudaError_t e, const char* where);
 int ensure_scratch(srl_ctx* ctx, size_t bytes);
 int ensure_pinned(srl_ctx* ctx, size_t bytes);
 void timing_collect(srl_ctx* ctx);
+// SRL_OK for a map laid out with kBlockCap points per block (the layout every LIO kernel addresses), else SRL_BAD_ARG
+int check_lio_map(srl_ctx* ctx, const srl_map* m);
 }  // namespace srl
 
 #define SRL_CUDA(ctx, call)                                             \

@@ -57,12 +57,12 @@ __global__ void k_upload_points(float* blocks, const float* xyz, long long n_vox
     float* b = blocks + (size_t)v * kBlockFloats + 4 * i;
     b[0] = xyz[3 * e]; b[1] = xyz[3 * e + 1]; b[2] = xyz[3 * e + 2];
 }
-__global__ void k_download(const float* blocks, long long n_voxels, int cap, short* keys, int* counts, float* xyz) {
+__global__ void k_download(const float* blocks, int block_pts, long long n_voxels, int cap, short* keys, int* counts, float* xyz) {
     const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= n_voxels * cap) return;
     const long long v = e / cap;
     const int i = (int)(e % cap);
-    const float* b = blocks + (size_t)v * kBlockFloats;
+    const float* b = blocks + (size_t)v * (4 * block_pts);
     const unsigned int* meta = reinterpret_cast<const unsigned int*>(b);
     const int cnt = (int)meta[kMetaCount];
     if (i == 0) {
@@ -112,10 +112,11 @@ __global__ void k_seg_lookup(const Slot* slots, unsigned int mask, const unsigne
     is_new[s] = (slot < 0 && allow_new) ? 1u : 0u;
 }
 
-__global__ void k_seg_claim(Slot* slots, unsigned int mask, float* blocks, const unsigned long long* __restrict__ keys,
-                            const unsigned int* __restrict__ seg_start, const int* n_seg_p,
-                            const unsigned int* __restrict__ is_new, const unsigned int* __restrict__ new_rank,
-                            long long block_base, int* seg_slot) {
+// a new voxel of segment s takes the next free block: slot claimed, key and count 0 written into the block's metadata
+__device__ __forceinline__ void seg_claim(Slot* slots, unsigned int mask, float* blocks, size_t block_floats, const unsigned long long* __restrict__ keys,
+                                          const unsigned int* __restrict__ seg_start, const int* n_seg_p,
+                                          const unsigned int* __restrict__ is_new, const unsigned int* __restrict__ new_rank,
+                                          long long block_base, int* seg_slot) {
     const int s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= *n_seg_p || !is_new[s]) return;
     const unsigned long long key = keys[seg_start[s]];
@@ -123,8 +124,14 @@ __global__ void k_seg_claim(Slot* slots, unsigned int mask, float* blocks, const
     unpack_key(key, x, y, z);
     const unsigned int blk = (unsigned int)(block_base + new_rank[s]);
     seg_slot[s] = slot_claim(slots, mask, key, x, y, z, blk, 0u);
-    unsigned int* meta = reinterpret_cast<unsigned int*>(blocks + (size_t)blk * kBlockFloats);
+    unsigned int* meta = reinterpret_cast<unsigned int*>(blocks + (size_t)blk * block_floats);
     meta[kMetaKeyLo] = (unsigned int)(key & 0xffffffffu); meta[kMetaKeyHi] = (unsigned int)(key >> 32); meta[kMetaCount] = 0;
+}
+__global__ void k_seg_claim(Slot* slots, unsigned int mask, float* blocks, const unsigned long long* __restrict__ keys,
+                            const unsigned int* __restrict__ seg_start, const int* n_seg_p,
+                            const unsigned int* __restrict__ is_new, const unsigned int* __restrict__ new_rank,
+                            long long block_base, int* seg_slot) {
+    seg_claim(slots, mask, blocks, kBlockFloats, keys, seg_start, n_seg_p, is_new, new_rank, block_base, seg_slot);
 }
 
 // one warp per touched voxel: the reference's per-point rule, replayed in sweep order
@@ -207,14 +214,19 @@ __global__ void k_first_in_cell(const unsigned long long* __restrict__ keys_sort
 // addPointToColorMap is sequential in the reference; the same (sort by voxel, replay per voxel in sweep order) scheme as K3
 // reproduces it: a voxel accepts the first (cap - count) offered points, a fine cell is claimed by the first ACCEPTED
 // point of the sweep that falls into it, and both lists are emitted in sweep order.
-struct ColorPoint {            // colour state of one stored point (rgbPoint minus position), index = block * cap + i
+struct ColorPoint {            // colour state of one stored point (rgbPoint minus position), index = block * block_pts + i
     short rgb[3]; short n_rgb;
     float cov[3]; float pad;
     double obs_dist, last_obs;
 };
 constexpr unsigned kNoIndex = 0xffffffffu;
+constexpr int kColorMaxCap = 128;   // largest max_num_points_in_voxel of a colour map (the shipped configs use 20, 50 and 100)
 
-// selected points (every step-th of the frame): voxel key + fine key from the float-rounded position (getPosition())
+// selected points (every step-th of the frame): voxel key + fine key from the float-rounded position (getPosition()).
+// Both keys are static_cast<short>(q) as the reference is compiled for x86-64: truncation to int32 (cvttsd2si), then the low
+// 16 bits, so a key wraps past |q| = 32767 (0.01 m fine cells: |x| >= 327.68 m) and cells 655.36 m apart share a key.
+// pack_key keeps those 16 bits, so a wrapped key is an ordinary key: valid bit 48 set, never 0 (empty slot) or kInvalidKey.
+// NaN, +-inf and |q| >= 2^31 (where the int32 conversion itself is undefined) drop the point.
 __global__ void k_color_keys(const double* __restrict__ xyz, long long m, int step, double size, double fine, unsigned long long* vkeys,
                              unsigned long long* fkeys, unsigned int* idx, float* fxyz) {
     const long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -224,10 +236,19 @@ __global__ void k_color_keys(const double* __restrict__ xyz, long long m, int st
     fxyz[3 * j] = fx; fxyz[3 * j + 1] = fy; fxyz[3 * j + 2] = fz;
     const double qx = __ddiv_rn((double)fx, size), qy = __ddiv_rn((double)fy, size), qz = __ddiv_rn((double)fz, size);
     const double gx = __ddiv_rn((double)fx, fine), gy = __ddiv_rn((double)fy, fine), gz = __ddiv_rn((double)fz, fine);
-    const bool ok = fabs(qx) < 32765.0 && fabs(qy) < 32765.0 && fabs(qz) < 32765.0 && fabs(gx) < 32765.0 && fabs(gy) < 32765.0 && fabs(gz) < 32765.0;
+    constexpr double kI32 = 2147483648.0;
+    const bool ok = fabs(qx) < kI32 && fabs(qy) < kI32 && fabs(qz) < kI32 && fabs(gx) < kI32 && fabs(gy) < kI32 && fabs(gz) < kI32;
     vkeys[j] = ok ? pack_key((int)qx, (int)qy, (int)qz) : kInvalidKey;
     fkeys[j] = ok ? pack_key((int)gx, (int)gy, (int)gz) : kInvalidKey;
     idx[j] = (unsigned int)j;
+}
+
+// k_seg_claim with the colour map's block stride
+__global__ void k_color_seg_claim(Slot* slots, unsigned int mask, float* blocks, int block_pts, const unsigned long long* __restrict__ keys,
+                                  const unsigned int* __restrict__ seg_start, const int* n_seg_p,
+                                  const unsigned int* __restrict__ is_new, const unsigned int* __restrict__ new_rank,
+                                  long long block_base, int* seg_slot) {
+    seg_claim(slots, mask, blocks, (size_t)(4 * block_pts), keys, seg_start, n_seg_p, is_new, new_rank, block_base, seg_slot);
 }
 
 // one thread per touched voxel: append the first (cap - count) offered points in sweep order, note the visit
@@ -235,7 +256,7 @@ __global__ void k_color_seg_process(Slot* slots, float* blocks, ColorPoint* cpts
                                     const unsigned long long* __restrict__ keys, const unsigned int* __restrict__ idx,
                                     const float* __restrict__ fxyz, const unsigned int* __restrict__ seg_start, const int* n_seg_p,
                                     const int* __restrict__ seg_slot, const unsigned int* __restrict__ is_new, long long m, int cap,
-                                    double t_end, double t_last_process, unsigned int* accept_id, unsigned int* seg_first,
+                                    int block_pts, double t_end, double t_last_process, unsigned int* accept_id, unsigned int* seg_first,
                                     long long* n_points) {
     const int s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= *n_seg_p) return;
@@ -244,7 +265,7 @@ __global__ void k_color_seg_process(Slot* slots, float* blocks, ColorPoint* cpts
     if (slot < 0) return;
     const unsigned int blk = slots[slot].block;
     int count = (int)slots[slot].count;
-    float* bp = blocks + (size_t)blk * kBlockFloats;
+    float* bp = blocks + (size_t)blk * (4 * block_pts);
     const long long start = seg_start[s];
     const unsigned long long key = keys[start];
     if (is_new[s]) last_visited[blk] = 0.0;                       // voxelBlock::last_visited_time = 0.0 (include/cloudMap.h:153)
@@ -254,8 +275,8 @@ __global__ void k_color_seg_process(Slot* slots, float* blocks, ColorPoint* cpts
         bp[4 * count] = fxyz[3 * (size_t)i]; bp[4 * count + 1] = fxyz[3 * (size_t)i + 1]; bp[4 * count + 2] = fxyz[3 * (size_t)i + 2];
         ColorPoint cp;                                            // rgbPoint::reset() (src/cloudMap.cpp:12-19)
         cp.rgb[0] = cp.rgb[1] = cp.rgb[2] = 0; cp.n_rgb = 0; cp.cov[0] = cp.cov[1] = cp.cov[2] = 0.f; cp.pad = 0.f; cp.obs_dist = 0.0; cp.last_obs = 0.0;
-        cpts[(size_t)blk * kBlockCap + count] = cp;
-        accept_id[i] = blk * (unsigned)kBlockCap + (unsigned)count;
+        cpts[(size_t)blk * block_pts + count] = cp;
+        accept_id[i] = blk * (unsigned)block_pts + (unsigned)count;
         ++count; ++added;
     }
     if (added) {
@@ -319,34 +340,21 @@ __device__ __forceinline__ unsigned char sat_u8(double v) {       // cv::saturat
     return (unsigned char)(r < 0 ? 0 : (r > 255 ? 255 : r));
 }
 __device__ __forceinline__ unsigned char sat_add_u8(unsigned char a, unsigned char b) { const int r = (int)a + (int)b; return (unsigned char)(r > 255 ? 255 : r); }
-// one warp per distinct recent voxel, a lane per stored point; a voxel listed `mult` times is rendered `mult` times in a row
-__global__ void __launch_bounds__(256) k_color_render(const Slot* slots, unsigned int mask, const float* __restrict__ blocks, ColorPoint* cpts,
-                                                       const unsigned long long* __restrict__ uniq_keys, const int* __restrict__ mult,
-                                                       const int* n_uniq_p, CamConst c, const unsigned char* __restrict__ img, double obs_time,
-                                                       unsigned long long* n_rendered) {
-    const int lane = threadIdx.x & 31;
-    const int u_i = (int)(((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5);
-    if (u_i >= *n_uniq_p) return;
-    const unsigned long long key = uniq_keys[u_i];
-    short kx, ky, kz;
-    unpack_key(key, kx, ky, kz);
-    const int slot = slot_find_rw(slots, mask, key, kx, ky, kz);
-    if (slot < 0) return;
-    const unsigned blk = slots[slot].block;
-    const int count = (int)slots[slot].count;
-    if (lane >= count) return;
-    const float* bp = blocks + (size_t)blk * kBlockFloats + 4 * lane;
+// one stored point: project, sample the image, fuse `reps` times in a row (the voxel's repetitions in the recent list);
+// returns how many of those fusions updateRgb counted
+__device__ __forceinline__ unsigned render_point(const float* __restrict__ bp, ColorPoint* cpt, const CamConst& c,
+                                                 const unsigned char* __restrict__ img, double obs_time, int reps) {
     const double px = (double)bp[0], py = (double)bp[1], pz = (double)bp[2];
     // project3dTo2d (src/lioOptimization.cpp:132-152), scale 1: products and sums rounded one by one like the host code
     double cxm, cym, czm;
     matvec3_exact(c.R, px, py, pz, cxm, cym, czm);
     const double pcx = __dadd_rn(cxm, c.t_cw[0]), pcy = __dadd_rn(cym, c.t_cw[1]), pcz = __dadd_rn(czm, c.t_cw[2]);
-    if (pcz < 0.001) return;
+    if (pcz < 0.001) return 0;
     const double u = __dadd_rn(__ddiv_rn(__dmul_rn(pcx, c.fx), pcz), c.cx);
     const double v = __dadd_rn(__ddiv_rn(__dmul_rn(pcy, c.fy), pcz), c.cy);
     // if2dPointsAvailable (:49-60)
     if (!((u >= __dadd_rn(__dmul_rn(c.fov, (double)c.cols), 1.0)) && (ceil(u) < __dmul_rn(__dsub_rn(1.0, c.fov), (double)c.cols)) &&
-          (v >= __dadd_rn(__dmul_rn(c.fov, (double)c.rows), 1.0)) && (ceil(v) < __dmul_rn(__dsub_rn(1.0, c.fov), (double)c.rows)))) return;
+          (v >= __dadd_rn(__dmul_rn(c.fov, (double)c.rows), 1.0)) && (ceil(v) < __dmul_rn(__dsub_rn(1.0, c.fov), (double)c.rows)))) return 0;
     const double dx = __dsub_rn(px, c.t_wc[0]), dy = __dsub_rn(py, c.t_wc[1]), dz = __dsub_rn(pz, c.t_wc[2]);
     const double dist = __dsqrt_rn(__dadd_rn(__dmul_rn(dx, dx), __dadd_rn(__dmul_rn(dy, dy), __dmul_rn(dz, dz))));
     // getSubPixel<cv::Vec3b> (:71-98): four saturated products, three saturated sums per channel
@@ -364,10 +372,9 @@ __global__ void __launch_bounds__(256) k_color_render(const Slot* slots, unsigne
         color[ch] = (double)sat_add_u8(sat_add_u8(sat_add_u8(a, b), cc), d);
     }
     // rgbPoint::updateRgb (src/cloudMap.cpp:59-101), mixed float / double arithmetic as written there
-    ColorPoint cp = cpts[(size_t)blk * kBlockCap + lane];
+    ColorPoint cp = *cpt;
     const double sigma = 15.0, process_noise_sigma = 0.1;
     unsigned rendered = 0;
-    const int reps = mult[u_i];
     for (int rep = 0; rep < reps; ++rep) {
         if (cp.obs_dist != 0 && (dist > __dmul_rn(cp.obs_dist, 1.2))) continue;
         if (cp.n_rgb == 0) {
@@ -392,36 +399,60 @@ __global__ void __launch_bounds__(256) k_color_render(const Slot* slots, unsigne
         cp.n_rgb = (short)(cp.n_rgb + 1);
         ++rendered;
     }
-    cpts[(size_t)blk * kBlockCap + lane] = cp;
+    *cpt = cp;
+    return rendered;
+}
+// one warp per distinct recent voxel; its lanes walk the block in strides of 32 (point lane, lane + 32, ...), so a block of up
+// to kColorMaxCap points takes up to 4 rounds.  Points are independent; a voxel listed `mult` times is fused `mult` times in a
+// row, which is the list order for each of its points.
+__global__ void __launch_bounds__(256) k_color_render(const Slot* slots, unsigned int mask, const float* __restrict__ blocks, int block_pts,
+                                                       ColorPoint* cpts, const unsigned long long* __restrict__ uniq_keys,
+                                                       const int* __restrict__ mult, const int* n_uniq_p, CamConst c,
+                                                       const unsigned char* __restrict__ img, double obs_time, unsigned long long* n_rendered) {
+    const int lane = threadIdx.x & 31;
+    const int u_i = (int)(((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+    if (u_i >= *n_uniq_p) return;
+    const unsigned long long key = uniq_keys[u_i];
+    short kx, ky, kz;
+    unpack_key(key, kx, ky, kz);
+    const int slot = slot_find_rw(slots, mask, key, kx, ky, kz);
+    if (slot < 0) return;
+    const unsigned blk = slots[slot].block;
+    const int count = (int)slots[slot].count;
+    const int reps = mult[u_i];
+    const float* bp = blocks + (size_t)blk * (4 * block_pts);
+    ColorPoint* cb = cpts + (size_t)blk * block_pts;
+    unsigned rendered = 0;
+    for (int i = lane; i < count; i += 32) rendered += render_point(bp + 4 * i, cb + i, c, img, obs_time, reps);
     if (rendered) atomicAdd(n_rendered, (unsigned long long)rendered);
 }
 // colour state + last visited time in the block order of srl_map_download
 __global__ void k_color_download(const ColorPoint* __restrict__ cpts, const float* __restrict__ blocks, const double* __restrict__ last_visited,
-                                 long long n_voxels, int cap, short* rgb, short* n_rgb, float* cov, double* obs_dist, double* last_obs,
-                                 double* visited) {
+                                 int block_pts, long long n_voxels, int cap, short* rgb, short* n_rgb, float* cov, double* obs_dist,
+                                 double* last_obs, double* visited) {
     const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= n_voxels * cap) return;
     const long long v = e / cap;
     const int i = (int)(e % cap);
-    const int cnt = (int)reinterpret_cast<const unsigned int*>(blocks + (size_t)v * kBlockFloats)[kMetaCount];
+    const int cnt = (int)reinterpret_cast<const unsigned int*>(blocks + (size_t)v * (4 * block_pts))[kMetaCount];
     const bool on = i < cnt;
-    const ColorPoint cp = cpts[(size_t)v * kBlockCap + i];
+    const ColorPoint cp = cpts[(size_t)v * block_pts + i];
     for (int a = 0; a < 3; ++a) { rgb[3 * e + a] = on ? cp.rgb[a] : (short)0; cov[3 * e + a] = (on && cp.n_rgb > 0) ? cp.cov[a] : 0.f; }
     n_rgb[e] = on ? cp.n_rgb : (short)0;
     obs_dist[e] = on ? cp.obs_dist : 0.0;
     last_obs[e] = on ? cp.last_obs : 0.0;
     if (i == 0) visited[v] = last_visited[v];
 }
-// rgb_points_vec entries as (voxel key, index in block)
-__global__ void k_color_rgb_ids(const unsigned int* __restrict__ rgb_points, long long n, const float* __restrict__ blocks, int cap, short* out) {
+// rgb_points_vec entries (point ids block * block_pts + i) as (voxel key, index in block)
+__global__ void k_color_rgb_ids(const unsigned int* __restrict__ rgb_points, long long n, const float* __restrict__ blocks, int block_pts, short* out) {
     const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= n) return;
     const unsigned id = rgb_points[t];
-    const unsigned blk = id / (unsigned)kBlockCap;
-    const unsigned int* meta = reinterpret_cast<const unsigned int*>(blocks + (size_t)blk * kBlockFloats);
+    const unsigned blk = id / (unsigned)block_pts;
+    const unsigned int* meta = reinterpret_cast<const unsigned int*>(blocks + (size_t)blk * (4 * block_pts));
     short x, y, z;
     unpack_key((unsigned long long)meta[kMetaKeyLo] | ((unsigned long long)meta[kMetaKeyHi] << 32), x, y, z);
-    out[4 * t] = x; out[4 * t + 1] = y; out[4 * t + 2] = z; out[4 * t + 3] = (short)(id - blk * (unsigned)kBlockCap);
+    out[4 * t] = x; out[4 * t + 1] = y; out[4 * t + 2] = z; out[4 * t + 3] = (short)(id - blk * (unsigned)block_pts);
 }
 
 __global__ void k_gather_points(const double* __restrict__ xyz, const unsigned int* __restrict__ sel, int m, double* out) {
@@ -437,6 +468,30 @@ static inline size_t align_up(size_t x, size_t a = 256) { return (x + a - 1) / a
 
 using namespace srl;
 
+int srl::check_lio_map(srl_ctx* ctx, const srl_map* m) {
+    if (m->block_pts == kBlockCap) return SRL_OK;
+    return set_err(ctx, SRL_BAD_ARG, "map has " + std::to_string(m->block_pts) + " points per block; the LIO path needs " + std::to_string(kBlockCap));
+}
+
+// the pool holds max_voxels blocks of block_pts float4 (arguments already checked)
+static int map_create(srl_ctx* ctx, double voxel_size, int32_t max_num_points_in_voxel, int block_pts, size_t max_voxels, srl_map** out) {
+    SRL_CUDA(ctx, cudaSetDevice(ctx->device));
+    srl_map* m = new srl_map();
+    m->ctx = ctx; m->voxel_size = voxel_size; m->cap = max_num_points_in_voxel; m->block_pts = block_pts; m->max_voxels = max_voxels;
+    size_t capacity = 1024;
+    while (capacity < 2 * max_voxels) capacity <<= 1;
+    m->capacity = capacity;
+    cudaError_t e;
+    if ((e = cudaMalloc(&m->d_slots, capacity * sizeof(Slot))) != cudaSuccess ||
+        (e = cudaMalloc(&m->d_blocks, max_voxels * 4 * (size_t)block_pts * sizeof(float))) != cudaSuccess ||
+        (e = cudaMalloc(&m->d_counters, 4 * sizeof(long long))) != cudaSuccess) {
+        srl_map_destroy(m);
+        return cuda_fail(ctx, e, "srl_map_create/cudaMalloc");
+    }
+    *out = m;
+    return srl_map_clear(m);
+}
+
 extern "C" {
 
 int srl_map_create(srl_ctx* ctx, double voxel_size, int32_t max_num_points_in_voxel, size_t max_voxels, srl_map** out) {
@@ -445,21 +500,7 @@ int srl_map_create(srl_ctx* ctx, double voxel_size, int32_t max_num_points_in_vo
         return set_err(ctx, SRL_BAD_ARG, "srl_map_create: voxel_size>0, 1<=max_num_points_in_voxel<=20, max_voxels>0 required");
     // the pass kernels address points as 32-bit float indices into the block pool (block * 80 + 4 * i)
     if (max_voxels > (size_t(1) << 25)) return set_err(ctx, SRL_BAD_ARG, "srl_map_create: max_voxels is limited to 2^25 (33.5 M voxels, 10.7 GB of blocks)");
-    SRL_CUDA(ctx, cudaSetDevice(ctx->device));
-    srl_map* m = new srl_map();
-    m->ctx = ctx; m->voxel_size = voxel_size; m->cap = max_num_points_in_voxel; m->max_voxels = max_voxels;
-    size_t capacity = 1024;
-    while (capacity < 2 * max_voxels) capacity <<= 1;
-    m->capacity = capacity;
-    cudaError_t e;
-    if ((e = cudaMalloc(&m->d_slots, capacity * sizeof(Slot))) != cudaSuccess ||
-        (e = cudaMalloc(&m->d_blocks, max_voxels * kBlockFloats * sizeof(float))) != cudaSuccess ||
-        (e = cudaMalloc(&m->d_counters, 4 * sizeof(long long))) != cudaSuccess) {
-        srl_map_destroy(m);
-        return cuda_fail(ctx, e, "srl_map_create/cudaMalloc");
-    }
-    *out = m;
-    return srl_map_clear(m);
+    return map_create(ctx, voxel_size, max_num_points_in_voxel, kBlockCap, max_voxels, out);
 }
 
 void srl_map_destroy(srl_map* m) {
@@ -516,6 +557,7 @@ __global__ void k_rebuild_slots(Slot* slots, unsigned int mask, const float* __r
 int srl_map_remove_far(srl_map* m, const double location[3], double distance, int64_t* n_removed) {
     if (!m || !location) return SRL_BAD_ARG;
     srl_ctx* ctx = m->ctx;
+    if (int rc = check_lio_map(ctx, m)) return rc;
     SRL_CUDA(ctx, cudaSetDevice(ctx->device));
     if (n_removed) *n_removed = 0;
     const long long nv = (long long)m->n_voxels;
@@ -574,6 +616,7 @@ int srl_map_stats(srl_map* m, int64_t* n_voxels, int64_t* n_points) {
 int srl_map_upload(srl_map* m, const int16_t* keys, const int32_t* counts, const float* xyz, size_t n_voxels) {
     if (!m || (n_voxels && (!keys || !counts || !xyz))) return SRL_BAD_ARG;
     srl_ctx* ctx = m->ctx;
+    if (int rc = check_lio_map(ctx, m)) return rc;
     if (n_voxels > m->max_voxels) return set_err(ctx, SRL_MAP_FULL, "srl_map_upload: more voxels than max_voxels");
     int rc = srl_map_clear(m);
     if (rc != SRL_OK || n_voxels == 0) return rc;
@@ -626,7 +669,7 @@ int srl_map_download(srl_map* m, int16_t* keys, int32_t* counts, float* xyz, siz
     int* d_cnt = reinterpret_cast<int*>(base + b_keys);
     float* d_xyz = reinterpret_cast<float*>(base + b_keys + b_cnt);
     const int T = 256;
-    k_download<<<(unsigned)((nv * cap + T - 1) / T), T, 0, ctx->stream>>>(m->d_blocks, (long long)nv, cap, d_keys, d_cnt, d_xyz);
+    k_download<<<(unsigned)((nv * cap + T - 1) / T), T, 0, ctx->stream>>>(m->d_blocks, m->block_pts, (long long)nv, cap, d_keys, d_cnt, d_xyz);
     ctx->launches += 1;
     SRL_CUDA(ctx, cudaGetLastError());
     SRL_CUDA(ctx, cudaMemcpyAsync(keys, d_keys, nv * 3 * sizeof(short), cudaMemcpyDeviceToHost, ctx->stream));
@@ -805,11 +848,11 @@ struct srl_color_map {
     srl_ctx* ctx = nullptr;
     srl_map* vox = nullptr;                 // color_voxel_map (include/lioOptimization.h:275)
     double min_dist = 0.15;
-    srl::ColorPoint* d_cpts = nullptr;      // max_voxels * 20
+    srl::ColorPoint* d_cpts = nullptr;      // max_voxels * block_pts
     double* d_last_visited = nullptr;       // max_voxels
     srl::Slot* d_fine = nullptr;            // hashmap_3d_points as an occupancy set: key = fine cell, block = index into rgb_points
     size_t fine_capacity = 0;
-    unsigned int* d_rgb_points = nullptr;   // rgb_points_vec: point ids (block * 20 + index)
+    unsigned int* d_rgb_points = nullptr;   // rgb_points_vec: point ids (block * block_pts + index)
     size_t max_rgb_points = 0;
     unsigned long long* d_recent_temp = nullptr;   // voxels_recent_visited_temp (packed keys)
     unsigned long long* d_recent = nullptr;        // map_tracker->voxels_recent_visited
@@ -822,17 +865,27 @@ int srl_color_map_create(srl_ctx* ctx, double voxel_size, int32_t max_num_points
                          srl_color_map** out) {
     if (!ctx || !out || !(min_distance_points > 0)) return SRL_BAD_ARG;
     *out = nullptr;
+    if (!(voxel_size > 0) || max_num_points_in_voxel < 1 || max_num_points_in_voxel > kColorMaxCap || max_voxels == 0)
+        return set_err(ctx, SRL_BAD_ARG, "srl_color_map_create: voxel_size>0, 1<=max_num_points_in_voxel<=128, max_voxels>0 required");
+    // up to kBlockCap points the pool keeps the LIO layout (the map also works with the LIO entry points), beyond it a block
+    // holds exactly cap points
+    const int block_pts = std::max(max_num_points_in_voxel, kBlockCap);
+    // point ids block * block_pts + i are 32-bit and kNoIndex stays free
+    if (max_voxels >= ((size_t(1) << 32) + block_pts - 1) / block_pts)
+        return set_err(ctx, SRL_BAD_ARG, "srl_color_map_create: max_voxels * points per block must stay below 2^32 (32-bit point ids)");
     srl_color_map* cm = new srl_color_map();
     cm->ctx = ctx; cm->min_dist = min_distance_points;
-    int rc = srl_map_create(ctx, voxel_size, max_num_points_in_voxel, max_voxels, &cm->vox);
+    int rc = block_pts == kBlockCap ? srl_map_create(ctx, voxel_size, max_num_points_in_voxel, max_voxels, &cm->vox)
+                                    : map_create(ctx, voxel_size, max_num_points_in_voxel, block_pts, max_voxels, &cm->vox);
     if (rc != SRL_OK) { delete cm; return rc; }
-    cm->max_rgb_points = max_voxels * (size_t)kBlockCap;
+    const size_t n_slots = max_voxels * (size_t)block_pts;
+    cm->max_rgb_points = n_slots;
     cm->recent_capacity = 4 * max_voxels + 1024;
-    size_t cap = 1024;
-    while (cap < 2 * cm->max_rgb_points) cap <<= 1;
+    size_t cap = 1024;   // load <= 0.5; at most 2^32 slots, so the 32-bit probe mask stays exact (load < 1 even then)
+    while (cap < 2 * cm->max_rgb_points && cap < (size_t(1) << 32)) cap <<= 1;
     cm->fine_capacity = cap;
     cudaError_t e;
-    if ((e = cudaMalloc(&cm->d_cpts, max_voxels * kBlockCap * sizeof(ColorPoint))) != cudaSuccess ||
+    if ((e = cudaMalloc(&cm->d_cpts, n_slots * sizeof(ColorPoint))) != cudaSuccess ||
         (e = cudaMalloc(&cm->d_last_visited, max_voxels * sizeof(double))) != cudaSuccess ||
         (e = cudaMalloc(&cm->d_fine, cap * sizeof(Slot))) != cudaSuccess ||
         (e = cudaMalloc(&cm->d_rgb_points, cm->max_rgb_points * sizeof(unsigned int))) != cudaSuccess ||
@@ -840,7 +893,7 @@ int srl_color_map_create(srl_ctx* ctx, double voxel_size, int32_t max_num_points
         (e = cudaMalloc(&cm->d_recent, cm->recent_capacity * sizeof(unsigned long long))) != cudaSuccess ||
         (e = cudaMalloc(&cm->d_counters, 8 * sizeof(long long))) != cudaSuccess ||
         (e = cudaMemsetAsync(cm->d_fine, 0, cap * sizeof(Slot), ctx->stream)) != cudaSuccess ||
-        (e = cudaMemsetAsync(cm->d_cpts, 0, max_voxels * kBlockCap * sizeof(ColorPoint), ctx->stream)) != cudaSuccess ||
+        (e = cudaMemsetAsync(cm->d_cpts, 0, n_slots * sizeof(ColorPoint), ctx->stream)) != cudaSuccess ||
         (e = cudaMemsetAsync(cm->d_last_visited, 0, max_voxels * sizeof(double), ctx->stream)) != cudaSuccess ||
         (e = cudaMemsetAsync(cm->d_counters, 0, 8 * sizeof(long long), ctx->stream)) != cudaSuccess ||
         (e = cudaStreamSynchronize(ctx->stream)) != cudaSuccess) {
@@ -958,10 +1011,11 @@ int srl_color_map_add_points(srl_color_map* cm, const double* xyz_world, size_t 
             long long before = 0, after = 0;
             SRL_CUDA(ctx, cudaMemcpyAsync(&before, m->d_counters, sizeof(long long), cudaMemcpyDeviceToHost, st));
             if (total_new > 0)
-                k_seg_claim<<<gs, T, 0, st>>>(m->d_slots, vmask, m->d_blocks, vk_b, seg_start, d_nseg, is_new, new_rank, (long long)m->n_voxels, seg_slot);
+                k_color_seg_claim<<<gs, T, 0, st>>>(m->d_slots, vmask, m->d_blocks, m->block_pts, vk_b, seg_start, d_nseg, is_new, new_rank,
+                                                    (long long)m->n_voxels, seg_slot);
             k_color_seg_process<<<gs, T, 0, st>>>(m->d_slots, m->d_blocks, cm->d_cpts, cm->d_last_visited, vk_b, idx_b, fxyz, seg_start, d_nseg,
-                                                  seg_slot, is_new, (long long)msel, m->cap, time_sweep_end, time_last_process, accept_id,
-                                                  seg_first, m->d_counters);
+                                                  seg_slot, is_new, (long long)msel, m->cap, m->block_pts, time_sweep_end, time_last_process,
+                                                  accept_id, seg_first, m->d_counters);
             m->n_voxels += total_new;
             // ---- recent list: the voxels this sweep visited for the first time, in the order of their first point
             k_color_seg_keys<<<gs, T, 0, st>>>(vk_b, seg_start, d_nseg, seg_key);
@@ -1053,8 +1107,8 @@ int srl_color_map_render_recent(srl_color_map* cm, const srl_camera* cam, const 
     for (int i = 0; i < 3; ++i) { c.t_cw[i] = cam->t_camera_world[i]; c.t_wc[i] = cam->t_world_camera[i]; }
     c.fx = cam->fx; c.fy = cam->fy; c.cx = cam->cx; c.cy = cam->cy; c.fov = cam->fov_margin; c.cols = cam->cols; c.rows = cam->rows;
     const int T = 256;
-    k_color_render<<<(unsigned)((nr * 32 + T - 1) / T), T, 0, st>>>(m->d_slots, (unsigned)(m->capacity - 1), m->d_blocks, cm->d_cpts, uniq, mult, d_nuniq, c, d_img,
-                                                               obs_time, d_count);
+    k_color_render<<<(unsigned)((nr * 32 + T - 1) / T), T, 0, st>>>(m->d_slots, (unsigned)(m->capacity - 1), m->d_blocks, m->block_pts, cm->d_cpts, uniq, mult,
+                                                               d_nuniq, c, d_img, obs_time, d_count);
     SRL_CUDA(ctx, cudaGetLastError());
     unsigned long long cnt = 0;
     SRL_CUDA(ctx, cudaMemcpyAsync(&cnt, d_count, 8, cudaMemcpyDeviceToHost, st));
@@ -1086,7 +1140,8 @@ int srl_color_map_download_state(srl_color_map* cm, size_t max_voxels, int16_t* 
     double* d_lo = reinterpret_cast<double*>(take(e * 8));
     double* d_lv = reinterpret_cast<double*>(take(nv * 8));
     const int T = 256;
-    k_color_download<<<(unsigned)((e + T - 1) / T), T, 0, ctx->stream>>>(cm->d_cpts, m->d_blocks, cm->d_last_visited, (long long)nv, cap, d_rgb, d_n, d_cov, d_od, d_lo, d_lv);
+    k_color_download<<<(unsigned)((e + T - 1) / T), T, 0, ctx->stream>>>(cm->d_cpts, m->d_blocks, cm->d_last_visited, m->block_pts, (long long)nv, cap, d_rgb, d_n, d_cov,
+                                                                         d_od, d_lo, d_lv);
     SRL_CUDA(ctx, cudaGetLastError());
     SRL_CUDA(ctx, cudaMemcpyAsync(rgb, d_rgb, e * 6, cudaMemcpyDeviceToHost, ctx->stream));
     SRL_CUDA(ctx, cudaMemcpyAsync(n_rgb, d_n, e * 2, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1108,7 +1163,7 @@ int srl_color_map_download_lists(srl_color_map* cm, int16_t* rgb_points /* n_rgb
         if (rc != SRL_OK) return rc;
         short* d_out = static_cast<short*>(ctx->d_scratch);
         const int T = 256;
-        k_color_rgb_ids<<<(unsigned)((n + T - 1) / T), T, 0, ctx->stream>>>(cm->d_rgb_points, (long long)n, m->d_blocks, m->cap, d_out);
+        k_color_rgb_ids<<<(unsigned)((n + T - 1) / T), T, 0, ctx->stream>>>(cm->d_rgb_points, (long long)n, m->d_blocks, m->block_pts, d_out);
         SRL_CUDA(ctx, cudaGetLastError());
         SRL_CUDA(ctx, cudaMemcpyAsync(rgb_points, d_out, n * 8, cudaMemcpyDeviceToHost, ctx->stream));
     }
@@ -1126,8 +1181,9 @@ int srl_map_insert_device(srl_map* m, const double* d_xyz_world, size_t n, doubl
                           int64_t* n_added) {
     if (!m || (n && !d_xyz_world)) return SRL_BAD_ARG;
     if (n_added) *n_added = 0;
-    if (n == 0) return SRL_OK;
     srl_ctx* ctx = m->ctx;
+    if (int rc = check_lio_map(ctx, m)) return rc;
+    if (n == 0) return SRL_OK;
     if (n > 0x7fffffffULL) return set_err(ctx, SRL_BAD_ARG, "srl_map_insert: n must fit in int32");
     SRL_CUDA(ctx, cudaSetDevice(ctx->device));
     int rc;
@@ -1140,6 +1196,7 @@ int srl_map_insert_sweep(srl_map* m, srl_sweep* sw, const double q[4], const dou
     if (!m || !sw || !q || !t || !R_il || !t_il) return SRL_BAD_ARG;
     if (n_added) *n_added = 0;
     srl_ctx* ctx = m->ctx;
+    if (int rc = check_lio_map(ctx, m)) return rc;
     if (sw->ctx != ctx) return set_err(ctx, SRL_BAD_ARG, "map and sweep belong to different contexts");
     const size_t n = sw->n;
     if (n == 0) return SRL_OK;
@@ -1156,8 +1213,9 @@ int srl_map_insert(srl_map* m, const double* xyz_world, size_t n, double min_dis
                    int64_t* n_added) {
     if (!m || (n && !xyz_world)) return SRL_BAD_ARG;
     if (n_added) *n_added = 0;
-    if (n == 0) return SRL_OK;
     srl_ctx* ctx = m->ctx;
+    if (int rc = check_lio_map(ctx, m)) return rc;
+    if (n == 0) return SRL_OK;
     if (n > 0x7fffffffULL) return set_err(ctx, SRL_BAD_ARG, "srl_map_insert: n must fit in int32");
     SRL_CUDA(ctx, cudaSetDevice(ctx->device));
     const size_t pts_bytes = align_up(n * 3 * sizeof(double));
