@@ -35,7 +35,7 @@ typedef enum srl_status {
     SRL_NAN_PLANARITY = 2,     /* the reference throws std::runtime_error("error") (src/optimize.cpp:348-350) */
     SRL_CUDA_ERROR = 3,
     SRL_BAD_ARG = 4,
-    SRL_MAP_FULL = 5,          /* more voxels than srl_map_create's max_voxels */
+    SRL_MAP_FULL = 5,          /* more voxels than the map's max_voxels */
     SRL_SINGULAR = 6,          /* a 17x17 inverse failed (src/optimize.cpp:234,237) */
     SRL_COMM_ERROR = 7
 } srl_status;
@@ -158,9 +158,21 @@ int srl_ctx_get_counter(srl_ctx* ctx, const char* name, int64_t* value);
 int srl_ctx_pass_time(srl_ctx* ctx, double* total_ms, int64_t* launches, int reset);
 
 /* ---- map: voxelHashMap + addPointsToMap (include/cloudMap.h:124-184, src/lioOptimization.cpp:400-446,520-554)
- * max_num_points_in_voxel <= 20 (block layout), max_voxels <= 2^25 (32-bit point indices in the kernels) */
+ * max_num_points_in_voxel <= 20 (block layout), max_voxels <= 2^25 (32-bit point indices in the kernels).
+ * max_voxels is the hard limit: an insert or upload past it returns SRL_MAP_FULL.  Memory is committed for initial_voxels
+ * at creation and grows on demand inside srl_map_insert*, srl_map_upload (and srl_color_map_add_points for a colour map's
+ * voxels): the committed voxel count doubles (or jumps to what the call needs), capped at max_voxels.  The block pool sits
+ * on address space reserved for max_voxels, so growing copies no point; the slot table is rebuilt at the next power of two
+ * that keeps load <= 0.5.  Nothing shrinks (srl_map_remove_far and srl_map_clear keep what is committed).  A growth that
+ * fails (SRL_CUDA_ERROR when the device is out of memory) leaves the map's contents unchanged and usable.
+ * 1 <= initial_voxels <= max_voxels, else SRL_BAD_ARG.  srl_map_create is initial_voxels = max_voxels: everything committed
+ * up front, no growth. */
 int srl_map_create(srl_ctx* ctx, double voxel_size, int32_t max_num_points_in_voxel, size_t max_voxels,
                    srl_map** out);
+int srl_map_create_growable(srl_ctx* ctx, double voxel_size, int32_t max_num_points_in_voxel, size_t initial_voxels,
+                            size_t max_voxels, srl_map** out);
+/* what is committed now: voxels backed by blocks, slots of the slot table, device bytes of both */
+int srl_map_capacity(srl_map* map, size_t* committed_voxels, size_t* slot_capacity, size_t* committed_bytes);
 void srl_map_destroy(srl_map* map);
 int srl_map_clear(srl_map* map);
 int srl_map_stats(srl_map* map, int64_t* n_voxels, int64_t* n_points); /* mapSize (src/lioOptimization.cpp:574-581) */
@@ -320,12 +332,23 @@ typedef struct srl_camera {      /* the state fields cloudFrame::project3dTo2d /
  * point ids), else SRL_BAD_ARG.  Up to 20 points the voxel map keeps the LIO block layout (20 points per block; it also works
  * with the LIO entry points); above 20 a block holds cap points and the LIO entry points (srl_map_insert*, srl_map_upload,
  * srl_map_remove_far, srl_build_plane_residuals*, srl_update_iekf*, srl_optimize_host*) reject the map with SRL_BAD_ARG.
- * HBM per point slot (max_voxels * max(cap, 20) slots): 16 B position + 40 B colour state + 4 B rgb id + 32-64 B fine-cell
- * slot, i.e. about 10-13 GB for 2^20 voxels at cap 100; the caller sizes max_voxels.
+ * HBM per committed point slot (committed voxels * max(cap, 20) slots): 16 B position + 40 B colour state; per committed
+ * rgb point 4 B rgb id + 32-64 B fine-cell slot.  srl_color_map_create commits everything for max_voxels up front (about
+ * 10.6 GB for 2^20 voxels at cap 100); srl_color_map_create_growable commits initial_voxels (and initial_voxels * max(cap,
+ * 20) rgb points) and grows like srl_map_create_growable: the voxel arrays with the voxels, the rgb list and the fine set
+ * with the rgb points, the two recent-voxel lists with their length, each doubling up to its limit (max_voxels, max_voxels
+ * * max(cap, 20) rgb points, 4 * max_voxels + 1024 recent entries).  Growth happens inside srl_color_map_add_points and,
+ * for cap <= 20, inside srl_map_insert / srl_map_upload on srl_color_map_voxels(cm); never inside the renderer.
+ * 1 <= initial_voxels <= max_voxels, else SRL_BAD_ARG.
  * Keys (voxel and fine cell) are static_cast<short>(x / size) as the reference compiles on x86-64: the low 16 bits of the
  * int32 truncation, so they wrap past |x / size| = 32767 like the reference's; NaN, +-inf and |x / size| >= 2^31 drop the point. */
 int srl_color_map_create(srl_ctx* ctx, double voxel_size, int32_t max_num_points_in_voxel, size_t max_voxels,
                          double min_distance_points, srl_color_map** out);
+int srl_color_map_create_growable(srl_ctx* ctx, double voxel_size, int32_t max_num_points_in_voxel, size_t initial_voxels,
+                                  size_t max_voxels, double min_distance_points, srl_color_map** out);
+/* what is committed now: voxels, fine-set slots, rgb points, and the device bytes of the whole colour map */
+int srl_color_map_capacity(srl_color_map* cm, size_t* committed_voxels, size_t* fine_capacity, size_t* committed_rgb_points,
+                           size_t* committed_bytes);
 void srl_color_map_destroy(srl_color_map* cm);
 srl_map* srl_color_map_voxels(srl_color_map* cm);
 int srl_color_map_stats(srl_color_map* cm, int64_t* n_voxels, int64_t* n_points, int64_t* n_rgb_points, int64_t* n_recent,

@@ -40,11 +40,13 @@ struct optimizeSummary {   // include/lioOptimization.h (same fields the path fi
 
 class LioBackend {
 public:
-    // device: CUDA ordinal; stream: cudaStream_t or nullptr; max_voxels / sweep_capacity size the HBM pools
+    // device: CUDA ordinal; stream: cudaStream_t or nullptr; max_voxels: the map's limit; sweep_capacity sizes the sweep
+    // buffers; initial_voxels: voxels committed at creation, the map grows from there up to max_voxels (0 = max_voxels)
     LioBackend(int device, void* stream, size_t max_voxels, size_t sweep_capacity, double size_voxel_map = 1.0,
-               int max_num_points_in_voxel = 20) {
+               int max_num_points_in_voxel = 20, size_t initial_voxels = 0) {
         check(srl_ctx_create(device, stream, &ctx_), "srl_ctx_create (no CPU fallback: a CUDA device is required)");
-        check(srl_map_create(ctx_, size_voxel_map, max_num_points_in_voxel, max_voxels, &map_), "srl_map_create");
+        check(srl_map_create_growable(ctx_, size_voxel_map, max_num_points_in_voxel, initial_voxels ? initial_voxels : max_voxels,
+                                      max_voxels, &map_), "srl_map_create_growable");
         check(srl_sweep_create(ctx_, sweep_capacity, &sweep_), "srl_sweep_create");
         const double I[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
         std::memcpy(R_imu_lidar, I, sizeof(I));
@@ -172,8 +174,11 @@ public:
 
     // ---- row N4: color_voxel_map + hashmap_3d_points + rgb_points_vec + voxels_recent_visited (include/lioOptimization.h:275-291)
     // created on first use with the LiDAR map's voxel size and cap (src/lioOptimization.cpp:539 passes map_options' values)
-    void enableColorMap(double size_voxel_map, int max_num_points_in_voxel, size_t max_voxels, double min_distance_points) {
-        if (!color_) check(srl_color_map_create(ctx_, size_voxel_map, max_num_points_in_voxel, max_voxels, min_distance_points, &color_), "srl_color_map_create");
+    // (initial_voxels as in the constructor: 0 = commit max_voxels up front)
+    void enableColorMap(double size_voxel_map, int max_num_points_in_voxel, size_t max_voxels, double min_distance_points,
+                        size_t initial_voxels = 0) {
+        if (!color_) check(srl_color_map_create_growable(ctx_, size_voxel_map, max_num_points_in_voxel, initial_voxels ? initial_voxels : max_voxels,
+                                                         max_voxels, min_distance_points, &color_), "srl_color_map_create_growable");
     }
     // the colour branch of addPointsToMap (src/lioOptimization.cpp:533-551): every add_point_step-th point of the registered frame
     long long addPointsToColorMap(const double* xyz_world, size_t n, int add_point_step, double time_sweep_end, double time_last_process,

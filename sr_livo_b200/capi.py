@@ -88,6 +88,7 @@ EXPORTS = [
     "srl_distort_frame_by_constant", "srl_distort_frame_by_imu", "srl_transform_all_imu_point",
     "srl_color_map_create", "srl_color_map_destroy", "srl_color_map_voxels", "srl_color_map_stats", "srl_color_map_add_points",
     "srl_color_map_render_recent", "srl_color_map_download_state", "srl_color_map_download_lists",
+    "srl_map_create_growable", "srl_map_capacity", "srl_color_map_create_growable", "srl_color_map_capacity",
 ]
 
 _lib = None
@@ -118,6 +119,8 @@ def lib():
     L.srl_ctx_set_timing.argtypes = [vp, C.c_int]
     L.srl_ctx_pass_time.argtypes = [vp, C.POINTER(dbl), C.POINTER(i64), C.c_int]
     L.srl_map_create.argtypes = [vp, dbl, i32, sz, C.POINTER(vp)]
+    L.srl_map_create_growable.argtypes = [vp, dbl, i32, sz, sz, C.POINTER(vp)]
+    L.srl_map_capacity.argtypes = [vp] + [C.POINTER(sz)] * 3
     L.srl_map_destroy.argtypes = [vp]
     L.srl_map_destroy.restype = None
     L.srl_map_clear.argtypes = [vp]
@@ -165,6 +168,8 @@ def lib():
     L.srl_host_plane_fit.argtypes = [vp, i32, vp, vp, vp]
     L.srl_iekf_replay.argtypes = [vp, C.POINTER(EskfState), vp, vp, C.POINTER(IcpParams), vp, i32, i64, C.POINTER(IekfSummary)]
     L.srl_color_map_create.argtypes = [vp, dbl, i32, sz, dbl, C.POINTER(vp)]
+    L.srl_color_map_create_growable.argtypes = [vp, dbl, i32, sz, sz, dbl, C.POINTER(vp)]
+    L.srl_color_map_capacity.argtypes = [vp] + [C.POINTER(sz)] * 4
     L.srl_color_map_destroy.argtypes = [vp]
     L.srl_color_map_destroy.restype = None
     L.srl_color_map_voxels.argtypes = [vp]

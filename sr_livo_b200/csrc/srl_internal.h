@@ -404,18 +404,32 @@ struct srl_ctx {
     size_t pinned_bytes = 0;
 };
 
+namespace srl {
+// Device array that grows in place: virtual address space for its limit is reserved once, and physical memory is mapped
+// behind it on demand (CUDA VMM), so its address never changes and growing copies nothing.  Newly mapped bytes are zero.
+struct VmArray {
+    unsigned long long base = 0;    // CUdeviceptr
+    size_t granularity = 0, reserved = 0, mapped = 0;
+    std::vector<std::pair<unsigned long long, size_t>> chunks;   // (CUmemGenericAllocationHandle, bytes), in address order
+};
+}  // namespace srl
+
 struct srl_map {
     srl_ctx* ctx = nullptr;
     double voxel_size = 1.0;
     int cap = 20;
     int block_pts = srl::kBlockCap; // points per block of the pool (block stride = 4 * block_pts floats): kBlockCap for
                                     // every map the LIO path accepts; cap for a colour map of cap > kBlockCap
-    size_t max_voxels = 0;
-    size_t capacity = 0;            // slots (power of two)
+    size_t max_voxels = 0;          // hard limit (SRL_MAP_FULL beyond it)
+    size_t committed_voxels = 0;    // blocks backed by memory; grows inside the insert / upload entry points only
+    size_t capacity = 0;            // slots (power of two, >= 2 x committed_voxels): rebuilt when the map grows, so the
+                                    // pass kernels take d_slots / capacity from the map at every call
     srl::Slot* d_slots = nullptr;
-    float* d_blocks = nullptr;
+    srl::VmArray blocks_mem;
+    float* d_blocks = nullptr;      // == blocks_mem.base
     int64_t n_voxels = 0;           // host mirror of the block count
     long long* d_counters = nullptr;   // [0] n_points, [1] scratch
+    srl_color_map* owner = nullptr; // the colour map whose voxel map this is: its per-voxel arrays grow with the blocks
 };
 
 struct srl_comm {
