@@ -313,6 +313,64 @@ int srl_distort_frame_by_imu(srl_ctx* ctx, const double* raw_xyz, const double* 
 int srl_transform_all_imu_point(srl_ctx* ctx, const double* imu_xyz, size_t n, const srl_imu_state* last_state,
                                 const double R_imu_lidar[9], const double t_imu_lidar[3], double* raw_xyz_out);
 
+/* ---- buildFrame (src/lioOptimization.cpp:786-893): from a cut sweep to the frame stateEstimation receives ---------------
+ * In the reference's order: makePointTimestamp (point time enabled: every point kept, alpha > 1 clamped to 1 - 1e-5; else the
+ * points outside [begin, end] are erased, order kept, no clamp), undistortion (motion_compensation 0 = IMU: distortFrameByImu,
+ * 1 = CONSTANT_VELOCITY: distortFrameByConstant, anything else SRL_BAD_ARG), std::shuffle with a default-seeded
+ * std::mt19937_64 (boost::mt19937_64), subSampleFrame only when voxel_size > 0 at (index_frame < init_num_frames ?
+ * init_voxel_size : voxel_size) over point = the raw LiDAR coordinate, a second shuffle with the same engine, transformAllImuPoint,
+ * then alpha_time = 1 and the identity pose for index_frame <= 2, the predicted pose after.  imu_point starts at 0: points an
+ * IMU walk never reaches keep 0 (the reference keeps whatever the cut sweep held).  The shuffles' draws follow context option
+ * "shuffle_rule" (0 default: Lemire's method, libstdc++ built with __int128; 1: the division downscale of libstdc++ without
+ * __int128 and of libstdc++ <= 10).  raw_xyz (n*3) and timestamp (n) are host or device memory (detected per pointer); states[]
+ * is host memory, n_states >= 1.  The frame stays in HBM; its buffers chain into srl_grid_sampling / srl_map_insert_device
+ * (point) and srl_sweep_set_device (raw_point, after the caller's gather of keypoints). */
+typedef struct srl_cloud_frame srl_cloud_frame;
+typedef struct srl_build_frame_params {
+    double timestamp_begin, timestamp_offset;
+    int32_t point_time_enable;     /* cloudProcessing::isPointTimeEnable() (given_offset_time) */
+    int32_t motion_compensation;   /* 0 IMU, 1 CONSTANT_VELOCITY (include/utility.h:82-86) */
+    int32_t index_frame, init_num_frames;
+    double init_voxel_size, voxel_size;
+    double R_il[9], t_il[3];       /* R_imu_lidar, t_imu_lidar */
+    double q_pred[4], t_pred[3];   /* cur_state->rotation (x, y, z, w), cur_state->translation */
+    double prev_time_sweep_end;    /* all_cloud_frame.back()->time_sweep_end, read when index_frame > 1 (dt_offset) */
+} srl_build_frame_params;
+typedef struct srl_build_frame_info {   /* the cloudFrame scalars (:880-889) and what each stage did */
+    double time_sweep_begin, time_sweep_end, time_frame_begin, time_frame_end, offset_begin, offset_end, dt_offset;
+    double sample_size;            /* subSampleFrame's cell (unused when voxel_size <= 0) */
+    int32_t frame_id;              /* index_frame */
+    int32_t reserved;
+    int64_t n_input, n_timestamped, n_imu_written, n_points;   /* n_imu_written: leading points the undistortion wrote */
+    int64_t engine_words;          /* mt19937_64 outputs the shuffles consumed */
+    int64_t shuffle_rejections;    /* draws that had to take another word */
+    double stage_ms[6];            /* host clock: timestamps, undistortion, shuffle 1, subsample, shuffle 2, transforms */
+} srl_build_frame_info;
+typedef struct srl_cloud_frame_ptrs {   /* device buffers, final frame order, valid until the next srl_build_frame on the frame */
+    double* raw_point;      /* n*3, after transformAllImuPoint */
+    double* point;          /* n*3, world under the predicted (or identity) pose */
+    double* imu_point;      /* n*3 */
+    double* relative_time;  /* n, ms */
+    double* alpha_time;     /* n */
+    double* timestamp;      /* n */
+    int32_t* source_index;  /* n, the point's index in the cut sweep */
+} srl_cloud_frame_ptrs;
+/* capacity: points reserved up front; a larger sweep grows the frame inside srl_build_frame */
+int srl_cloud_frame_create(srl_ctx* ctx, size_t capacity, srl_cloud_frame** out);
+void srl_cloud_frame_destroy(srl_cloud_frame* frame);
+size_t srl_cloud_frame_size(const srl_cloud_frame* frame);
+int srl_cloud_frame_device(srl_cloud_frame* frame, srl_cloud_frame_ptrs* ptrs);
+/* host copies; any pointer may be NULL */
+int srl_cloud_frame_download(srl_cloud_frame* frame, double* raw_point, double* point, double* imu_point, double* relative_time,
+                             double* alpha_time, double* timestamp, int32_t* source_index);
+int srl_build_frame(srl_ctx* ctx, const double* raw_xyz, const double* timestamp, size_t n, const srl_imu_state* states,
+                    size_t n_states, const srl_build_frame_params* params, srl_cloud_frame* frame, srl_build_frame_info* info);
+/* the device shuffle alone, for tests: std::shuffle's permutation of n elements (perm_out[p] = element that ends at p) drawn
+ * from `words` (host, n_words engine outputs) or, with words == NULL, from a default-seeded mt19937_64; *words_used and
+ * *next_word (the engine's next output) may be NULL.  rule as option "shuffle_rule". */
+int srl_shuffle_replay(srl_ctx* ctx, const uint64_t* words, size_t n_words, size_t n, int32_t rule, uint32_t* perm_out,
+                       size_t* words_used, uint64_t* next_word);
+
 /* ---- row N4: the colour map fed by the map update (src/lioOptimization.cpp:448-551, colour branch) and the renderer that
  * colours its points from a camera frame (src/rgbMapTracker.cpp:181-237 with rgbPoint::updateRgb, src/cloudMap.cpp:59-101).
  * A colour map = a voxel map (same HBM layout as srl_map; srl_color_map_voxels exposes it for download / stats) whose

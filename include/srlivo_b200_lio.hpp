@@ -14,6 +14,7 @@
 //   lioOptimization::removePointsFarFromLocation  src/lioOptimization.cpp:556   srl::LioBackend::removePointsFarFromLocation
 //   gridSampling                      src/utility.cpp:188           srl::LioBackend::gridSampling (keypoint indices)
 //   distortFrameByConstant / ByImu    src/utility.cpp:203,238       srl::LioBackend::distortFrameByConstant / distortFrameByImu
+//   buildFrame (+ makePointTimestamp) src/lioOptimization.cpp:786,821 srl::LioBackend::buildFrame (frame stays in HBM: frame())
 //   transformAllImuPoint              src/utility.cpp:320           srl::LioBackend::transformAllImuPoint
 //   addPointToColorMap (loop :533-551) src/lioOptimization.cpp:448  srl::LioBackend::addPointsToColorMap
 //   rgbMapTracker::renderPointsInRecentVoxel  src/rgbMapTracker.cpp:216  srl::LioBackend::renderPointsInRecentVoxel
@@ -53,6 +54,7 @@ public:
         std::memset(t_imu_lidar, 0, sizeof(t_imu_lidar));
     }
     ~LioBackend() {
+        if (frame_) srl_cloud_frame_destroy(frame_);
         if (color_) srl_color_map_destroy(color_);
         if (sweep_) srl_sweep_destroy(sweep_);
         if (map_) srl_map_destroy(map_);
@@ -147,6 +149,19 @@ public:
     void transformAllImuPoint(const double* imu_xyz, size_t n, const srl_imu_state& last_state, double* raw_xyz_out) {
         check(srl_transform_all_imu_point(ctx_, imu_xyz, n, &last_state, R_imu_lidar, t_imu_lidar, raw_xyz_out), "srl_transform_all_imu_point");
     }
+    // src/lioOptimization.cpp:786-893 — the cut sweep (raw_xyz n*3, timestamp n; host or device) becomes the device-resident frame
+    // (created on first use, reused after: its device pointers change only when a larger sweep grows it).  params.R_il / t_il
+    // are taken from this backend's extrinsics.  Returns the cloudFrame scalars.
+    srl_build_frame_info buildFrame(const double* raw_xyz, const double* timestamp, size_t n, const std::vector<srl_imu_state>& imu_states,
+                                    srl_build_frame_params params) {
+        if (!frame_) check(srl_cloud_frame_create(ctx_, n, &frame_), "srl_cloud_frame_create");
+        for (int i = 0; i < 9; ++i) params.R_il[i] = R_imu_lidar[i];
+        for (int i = 0; i < 3; ++i) params.t_il[i] = t_imu_lidar[i];
+        srl_build_frame_info info;
+        check(srl_build_frame(ctx_, raw_xyz, timestamp, n, imu_states.data(), imu_states.size(), &params, frame_, &info), "srl_build_frame");
+        return info;
+    }
+    srl_cloud_frame* frame() { return frame_; }
 
 #ifdef SRL_HAVE_EIGEN
     // overloads on the reference's types (cloudMap.h / parameters.h must be included first)
@@ -201,6 +216,7 @@ private:
     srl_map* map_ = nullptr;
     srl_sweep* sweep_ = nullptr;
     srl_color_map* color_ = nullptr;
+    srl_cloud_frame* frame_ = nullptr;
 
     void check(int rc, const char* what) {
         if (rc != SRL_OK) throw std::runtime_error(std::string(what) + ": " + (ctx_ ? srl_last_error(ctx_) : "no context"));

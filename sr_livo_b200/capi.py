@@ -71,6 +71,28 @@ class Camera(C.Structure):
                 ("cols", C.c_int32), ("rows", C.c_int32)]
 
 
+class BuildFrameParams(C.Structure):
+    """srl_build_frame_params: buildFrame's inputs (src/lioOptimization.cpp:821-893)."""
+    _fields_ = [("timestamp_begin", C.c_double), ("timestamp_offset", C.c_double), ("point_time_enable", C.c_int32),
+                ("motion_compensation", C.c_int32), ("index_frame", C.c_int32), ("init_num_frames", C.c_int32),
+                ("init_voxel_size", C.c_double), ("voxel_size", C.c_double), ("R_il", C.c_double * 9), ("t_il", C.c_double * 3),
+                ("q_pred", C.c_double * 4), ("t_pred", C.c_double * 3), ("prev_time_sweep_end", C.c_double)]
+
+
+class BuildFrameInfo(C.Structure):
+    """srl_build_frame_info: the cloudFrame scalars and what each stage did."""
+    _fields_ = [("time_sweep_begin", C.c_double), ("time_sweep_end", C.c_double), ("time_frame_begin", C.c_double),
+                ("time_frame_end", C.c_double), ("offset_begin", C.c_double), ("offset_end", C.c_double), ("dt_offset", C.c_double),
+                ("sample_size", C.c_double), ("frame_id", C.c_int32), ("reserved", C.c_int32), ("n_input", C.c_int64),
+                ("n_timestamped", C.c_int64), ("n_imu_written", C.c_int64), ("n_points", C.c_int64), ("engine_words", C.c_int64),
+                ("shuffle_rejections", C.c_int64), ("stage_ms", C.c_double * 6)]
+
+
+class CloudFramePtrs(C.Structure):
+    _fields_ = [("raw_point", C.c_void_p), ("point", C.c_void_p), ("imu_point", C.c_void_p), ("relative_time", C.c_void_p),
+                ("alpha_time", C.c_void_p), ("timestamp", C.c_void_p), ("source_index", C.c_void_p)]
+
+
 class IekfIter(C.Structure):
     _fields_ = [("predict", EskfState), ("pass_index", C.c_int32), ("max_num_iter", C.c_int32)]
 
@@ -89,6 +111,8 @@ EXPORTS = [
     "srl_color_map_create", "srl_color_map_destroy", "srl_color_map_voxels", "srl_color_map_stats", "srl_color_map_add_points",
     "srl_color_map_render_recent", "srl_color_map_download_state", "srl_color_map_download_lists",
     "srl_map_create_growable", "srl_map_capacity", "srl_color_map_create_growable", "srl_color_map_capacity",
+    "srl_cloud_frame_create", "srl_cloud_frame_destroy", "srl_cloud_frame_size", "srl_cloud_frame_device", "srl_cloud_frame_download",
+    "srl_build_frame", "srl_shuffle_replay",
 ]
 
 _lib = None
@@ -179,6 +203,15 @@ def lib():
     L.srl_color_map_render_recent.argtypes = [vp, C.POINTER(Camera), vp, dbl, C.POINTER(i64)]
     L.srl_color_map_download_state.argtypes = [vp, sz, vp, vp, vp, vp, vp, vp]
     L.srl_color_map_download_lists.argtypes = [vp, vp, vp]
+    L.srl_cloud_frame_create.argtypes = [vp, sz, C.POINTER(vp)]
+    L.srl_cloud_frame_destroy.argtypes = [vp]
+    L.srl_cloud_frame_destroy.restype = None
+    L.srl_cloud_frame_size.argtypes = [vp]
+    L.srl_cloud_frame_size.restype = sz
+    L.srl_cloud_frame_device.argtypes = [vp, C.POINTER(CloudFramePtrs)]
+    L.srl_cloud_frame_download.argtypes = [vp] + [vp] * 7
+    L.srl_build_frame.argtypes = [vp, vp, vp, sz, vp, sz, C.POINTER(BuildFrameParams), vp, C.POINTER(BuildFrameInfo)]
+    L.srl_shuffle_replay.argtypes = [vp, vp, sz, sz, i32, vp, C.POINTER(sz), C.POINTER(C.c_uint64)]
     for name in EXPORTS:
         fn = getattr(L, name)
         if fn.restype is C.c_int and name not in ("srl_abi_version",):

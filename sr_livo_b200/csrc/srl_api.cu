@@ -395,6 +395,12 @@ int srl_ctx_set_option(srl_ctx* ctx, const char* name, int64_t value) {
     if (n == "mapped_result") { ctx->mapped_result = value != 0; return SRL_OK; }
     if (n == "device_loop") { ctx->device_loop = value != 0; return SRL_OK; }
     if (n == "eager_order") { ctx->eager_order = value != 0; return SRL_OK; }
+    if (n == "shuffle_rule") {
+        if (value != 0 && value != 1) return set_err(ctx, SRL_BAD_ARG, "shuffle_rule must be 0 (Lemire) or 1 (division)");
+        ctx->shuffle_rule = (int)value;
+        return SRL_OK;
+    }
+    if (n == "shuffle_on_host") { ctx->shuffle_on_host = value != 0; return SRL_OK; }
     if (n == "pdl") { ctx->pdl = value != 0; return SRL_OK; }
     if (n == "cluster_order") { sweep_order_set_impl((int)value); return SRL_OK; }   // process-wide
     if (n == "exchange_in_fit") { ctx->exchange_in_fit = value != 0; return SRL_OK; }

@@ -386,6 +386,8 @@ struct srl_ctx {
     bool kernels_preloaded = false;
     bool pdl = true;                         // option "pdl" / SRL_PDL: programmatic dependent launch of the pass kernels
     bool eager_order = true;                 // option "eager_order": Morton-order a sweep right behind its upload (default) or at its first pass
+    int shuffle_rule = 0;                    // option "shuffle_rule": srl_build_frame's draws, 0 Lemire (libstdc++ with __int128), 1 division
+    bool shuffle_on_host = false;            // option "shuffle_on_host": srl_build_frame's shuffles as a host Fisher-Yates + upload
     int concurrent_kernels = -1;             // -1 not probed yet; 0: kernels of this process are serialised (profiler): host loop
     bool device_loop = true;                 // option "device_loop" / SRL_DEVICE_LOOP: 0 = the host-driven loop of round 1
     srl::IekfDev* d_iekf = nullptr;

@@ -278,6 +278,46 @@ class Sweep:
         _check(self.ctx.h, lib().srl_sweep_set_shard(self.h, begin, end))
 
 
+class CloudFrame:
+    """The frame buildFrame hands to stateEstimation, resident in HBM (srl_cloud_frame), final frame order."""
+
+    FIELDS = (("raw_point", 3, np.float64), ("point", 3, np.float64), ("imu_point", 3, np.float64), ("relative_time", 1, np.float64),
+              ("alpha_time", 1, np.float64), ("timestamp", 1, np.float64), ("source_index", 1, np.int32))
+
+    def __init__(self, ctx: Context, capacity: int = 1 << 17):
+        self.ctx = ctx
+        self.info = None
+        h = C.c_void_p()
+        _check(ctx.h, lib().srl_cloud_frame_create(ctx.h, capacity, C.byref(h)))
+        self.h = h
+
+    def close(self):
+        if getattr(self, "h", None):
+            lib().srl_cloud_frame_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def __len__(self) -> int:
+        return int(lib().srl_cloud_frame_size(self.h))
+
+    def device_ptrs(self) -> dict:
+        """Device addresses of the fields (valid until the next build into this frame)."""
+        p = capi.CloudFramePtrs()
+        _check(self.ctx.h, lib().srl_cloud_frame_device(self.h, C.byref(p)))
+        return {name: getattr(p, name) for name, _, _ in self.FIELDS}
+
+    def download(self) -> dict:
+        n = len(self)
+        out = {name: np.zeros((n, k) if k > 1 else n, dt) for name, k, dt in self.FIELDS}
+        _check(self.ctx.h, lib().srl_cloud_frame_download(self.h, *[ptr(out[name]) for name, _, _ in self.FIELDS]))
+        return out
+
+
 @dataclass
 class EskfEstimator:
     """eskfEstimator state (src/eskfEstimator.cpp:3-21); q = (x, y, z, w)."""
@@ -375,6 +415,34 @@ class LioOptimization:
         _check(self.ctx.h, lib().srl_map_insert_sweep(self.voxel_map.h, self.sweep.h, ptr(q), ptr(t), ptr(R), ptr(ti),
                                                       min_distance_points, min_num_points, C.byref(added)))
         return added.value
+
+    # ---- src/lioOptimization.cpp:786-893
+    def buildFrame(self, raw_xyz, timestamp, imu_states, timestamp_begin: float, timestamp_offset: float, index_frame: int,
+                   q_pred=None, t_pred=None, point_time_enable: bool = True, motion_compensation: int = 1, init_num_frames: int = 20,
+                   init_voxel_size: float = 0.2, voxel_size: float = 0.5, prev_time_sweep_end: float = 0.0,
+                   frame: "CloudFrame | None" = None) -> CloudFrame:
+        """buildFrame over a cut sweep given as host arrays (raw_xyz n*3, timestamp n; capi.lib().srl_build_frame takes device
+        pointers too).  imu_states: a list of capi.ImuState.  motion_compensation: 0 IMU, 1 CONSTANT_VELOCITY.  Returns the
+        device-resident frame (into `frame` when given), with the cloudFrame scalars in frame.info (capi.BuildFrameInfo)."""
+        raw = f64(raw_xyz).reshape(-1, 3)
+        ts = f64(timestamp).reshape(-1)
+        assert ts.shape[0] == raw.shape[0]
+        states = (capi.ImuState * len(imu_states))(*imu_states)
+        p = capi.BuildFrameParams()
+        p.timestamp_begin, p.timestamp_offset = float(timestamp_begin), float(timestamp_offset)
+        p.point_time_enable, p.motion_compensation = int(bool(point_time_enable)), int(motion_compensation)
+        p.index_frame, p.init_num_frames = int(index_frame), int(init_num_frames)
+        p.init_voxel_size, p.voxel_size = float(init_voxel_size), float(voxel_size)
+        p.prev_time_sweep_end = float(prev_time_sweep_end)
+        for name, val in (("R_il", f64(self.R_imu_lidar).reshape(9)), ("t_il", f64(self.t_imu_lidar)),
+                          ("q_pred", f64([0, 0, 0, 1] if q_pred is None else q_pred)), ("t_pred", f64(np.zeros(3) if t_pred is None else t_pred))):
+            getattr(p, name)[:] = list(val)
+        frame = frame if frame is not None else CloudFrame(self.ctx, max(raw.shape[0], 1))
+        info = capi.BuildFrameInfo()
+        _check(self.ctx.h, lib().srl_build_frame(self.ctx.h, ptr(raw), ptr(ts), raw.shape[0], states, len(imu_states), C.byref(p),
+                                                 frame.h, C.byref(info)))
+        frame.info = info
+        return frame
 
     # ---- src/lioOptimization.cpp:574-581
     def mapSize(self) -> int:
