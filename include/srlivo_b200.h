@@ -138,15 +138,11 @@ int srl_ctx_set_timing(srl_ctx* ctx, int enable);
  * "k1_variant" (0 auto; 1: k1_fast, 3: k1_scan + k1_fit, both with the exact fallback where applicable; 2: k1_assoc
  * only), "split_lanes_per_keypoint" (2|4: lanes per keypoint in k1_scan), "k1_min_blocks" (2|3|4) and
  * "fast_min_blocks" (4|5|6|8): resident-blocks-per-SM variants of the two kernels, "fast_lanes_per_keypoint" (1|2|4:
- * lanes that share one keypoint's candidate scan in k1_fast), "mapped_result" (1 default: a pass's sums
- * reach the host through a mapped pinned buffer + sequence flag; 0: cudaMemcpyAsync + stream synchronize),
- * "exchange_in_fit" (1 default: on several GPUs k1_fit's last block runs the NVLink exchange itself when the rank
- * flagged nothing, 0: always in the fallback launch), "fast_force_ambiguous_mod" (N > 0:
+ * lanes that share one keypoint's candidate scan in k1_fast), "fast_force_ambiguous_mod" (N > 0:
  * k1_fast hands every N-th keypoint to k1_assoc, to test the hand-over), "device_loop" (1 default: srl_update_iekf[_dist]
  * keep the whole iterated update on the GPU — a persistent block runs the ESIKF algebra between the passes, all passes are
  * enqueued at once, one host wait, with or without the max_num_residuals cap; 0: the host-driven loop, which is also used
- * under kernel-serialising tools), "pdl" (1 default: programmatic dependent launch of the pass kernels in the device loop), "eager_order"
- * (1 default: a sweep is Morton-ordered right behind its upload instead of at its first pass).  Counters: "exact_fallbacks"
+ * under kernel-serialising tools).  Counters: "exact_fallbacks"
  * (keypoints whose FP32 selection in k1_assoc was ambiguous and were redone exactly), "fast_ambiguous" (keypoints
  * k1_fast handed to k1_assoc), "kernel_launches", "device_loop_active" (1 when the device-resident loop is in use on this
  * ctx), "iekf_step_cycles_avg" (SM clock ticks of one ESIKF step, sums seen -> pose published; resets on read),

@@ -1031,14 +1031,10 @@ __global__ void __launch_bounds__(kFastThreads, MINB) k1_fit(const __grid_consta
             for (int w = 0; w < kFastWarps; ++w) tot += s_acc[w][lane];
             if (lane == 30) { tot += (double)__ldcg(A.scan_count); *A.scan_count = 0ull; }   // k1_scan's visit count
             // nothing flagged in this pass on this rank (the usual case): these ARE the rank's sums.  Single GPU: hand them to
-            // the host now; multi-GPU (exchange_in_fit): run the NVLink exchange here.  The fallback launch that follows
-            // then only forwards the totals again (same values, same sequence number).
-            const bool none_flagged = A.stats && __ldcg(A.stats + 2) == 0ull;
-            bool final_here = none_flagged && A.comm.world <= 1;
-            if (none_flagged && A.comm.world > 1 && A.exchange_in_fit) {
-                tot = comm_exchange(A.comm, tot, lane);
-                final_here = true;
-            }
+            // the host now; multi-GPU: run the NVLink exchange here.  The fallback launch that follows then only forwards
+            // the totals again (same values, same sequence number).
+            const bool final_here = A.stats && __ldcg(A.stats + 2) == 0ull;   // nothing flagged
+            if (final_here && A.comm.world > 1) tot = comm_exchange(A.comm, tot, lane);
             if (final_here && lane == 0) A.stats[3] = 1ull;   // tells the fallback launch that the pass is already finalised
             A.out32[lane] = tot;
             if (lane == 0) *A.ticket = 0u;

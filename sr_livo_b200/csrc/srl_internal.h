@@ -219,8 +219,7 @@ struct FastArgs {               // k1_fast (srl_fast.cu)
     unsigned long long* scan_count;   // candidates visited by k1_scan, folded into component 30 by k1_fit's last block
     double* host_out;                 // optional: mapped host buffer; k1_fit publishes the final sums there when no keypoint
     unsigned long long host_seq;      // was flagged in this pass (see K1Args::host_out)
-    CommDev comm;                     // multi-GPU with exchange_in_fit: k1_fit's last block runs the exchange in that case
-    int exchange_in_fit;
+    CommDev comm;                     // multi-GPU: k1_fit's last block runs the exchange in that case
     IekfDev* dev;                     // device-resident loop (see K1Args::dev)
     unsigned long long pose_ticket, end_ticket;
     int wait_pose;
@@ -370,8 +369,6 @@ struct srl_ctx {
     double* h_out32 = nullptr;      // pinned + mapped: [0,32) sums, [32] sequence flag written by the pass's last kernel, [33..64) scratch
     double* d_h_out32 = nullptr;    // device-side address of h_out32
     unsigned long long host_seq = 0;
-    bool exchange_in_fit = true;    // option "exchange_in_fit" / SRL_EXCHANGE_IN_FIT: multi-GPU, k1_fit runs the exchange when it flagged nothing
-    bool mapped_result = true;      // option "mapped_result": read a pass's sums through the mapped buffer (default) or by memcpy + sync
     long long* d_k2_state = nullptr;
     unsigned long long* d_cap_chunks = nullptr;   // device-resident loop: k2_cap_reduce counts the capped chunks that did work
     int64_t cap_chunks_run = 0;              // counter "cap_chunks_run": capped chunks processed by the last update's passes
@@ -384,8 +381,6 @@ struct srl_ctx {
     unsigned long long* d_scan_count = nullptr;
     // device-resident updateIEKF loop (row N1)
     bool kernels_preloaded = false;
-    bool pdl = true;                         // option "pdl" / SRL_PDL: programmatic dependent launch of the pass kernels
-    bool eager_order = true;                 // option "eager_order": Morton-order a sweep right behind its upload (default) or at its first pass
     int shuffle_rule = 0;                    // option "shuffle_rule": srl_build_frame's draws, 0 Lemire (libstdc++ with __int128), 1 division
     bool shuffle_on_host = false;            // option "shuffle_on_host": srl_build_frame's shuffles as a host Fisher-Yates + upload
     int concurrent_kernels = -1;             // -1 not probed yet; 0: kernels of this process are serialised (profiler): host loop

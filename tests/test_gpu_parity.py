@@ -1088,23 +1088,39 @@ L = lio.LioOptimization(device=dev, max_voxels=1 << 16, sweep_capacity=8192)
 L.addPointsToMap(pts)                                   # every rank builds its replica
 D = dist.DistributedLio(L, rank, world, native=True)
 prm = lio.r3live_params(max_num_residuals=2**31-1)
-for rep in range(3):                                    # several updates in a row: sequence numbers / double buffering
-    D.set_keypoints(sw.raw_xyz)
-    L.eskf_pro = lio.EskfEstimator(p=sw.t_init.copy(), q=sw.q_init.copy(), cov=synth.prior_covariance())
-    # last repetition: rank 1 hands every 7th keypoint to the exact kernel, rank 0 none: the two ranks then finish a pass
-    # (and run their side of the exchange) in different kernels
-    L.ctx.set_option("fast_force_ambiguous_mod", 7 if (rep == 2 and rank == world - 1) else 0)
-    out = D.updateIEKF(prm, sw.t_last)
 om = O.OracleMap(); om.add_points(pts)
 ref = om.update_iekf(sw.raw_xyz, O.Eskf(p=sw.t_init.copy(), q=sw.q_init.copy(), cov=synth.prior_covariance()), sw.t_last,
                      O.r3live_params(max_num_residuals=2**31-1))
-assert out["success"] and out["passes"] == ref["passes"], (out["passes"], ref["passes"])
-assert np.allclose(out["trace"], ref["trace"], rtol=1e-5, atol=1e-9)
-assert np.allclose(L.eskf_pro.p, ref["eskf"].p, atol=1e-9) and np.allclose(L.eskf_pro.q, ref["eskf"].q, atol=1e-9)
-t = torch.from_numpy(np.concatenate([L.eskf_pro.p, L.eskf_pro.q, L.eskf_pro.cov.reshape(-1)]))
-lst = [torch.zeros_like(t) for _ in range(world)]
-tdist.all_gather(lst, t)
-assert all(torch.equal(lst[0], x) for x in lst)         # every rank ends bit-identical
+# native device-resident loop, native host-driven loop (DistributedLio already chose the host loop on every rank when some
+# rank cannot run the device loop)
+modes = (1, 0) if L.ctx.counter("device_loop_active") else (0,)
+res = {}
+for mode in modes:
+    L.ctx.set_option("device_loop", mode)
+    for rep in range(3):                                # several updates in a row: sequence numbers / double buffering
+        D.set_keypoints(sw.raw_xyz)
+        L.eskf_pro = lio.EskfEstimator(p=sw.t_init.copy(), q=sw.q_init.copy(), cov=synth.prior_covariance())
+        # last repetition: rank 1 hands every 7th keypoint to the exact kernel, rank 0 none: the two ranks then finish a pass
+        # (and run their side of the exchange) in different kernels
+        L.ctx.set_option("fast_force_ambiguous_mod", 7 if (rep == 2 and rank == world - 1) else 0)
+        out = D.updateIEKF(prm, sw.t_last)
+    assert out["success"] and out["passes"] == ref["passes"], (mode, out["passes"], ref["passes"])
+    assert np.allclose(out["trace"], ref["trace"], rtol=1e-5, atol=1e-9), mode
+    assert np.allclose(L.eskf_pro.p, ref["eskf"].p, atol=1e-9) and np.allclose(L.eskf_pro.q, ref["eskf"].q, atol=1e-9), mode
+    t = torch.from_numpy(np.concatenate([L.eskf_pro.p, L.eskf_pro.q, L.eskf_pro.cov.reshape(-1)]))
+    lst = [torch.zeros_like(t) for _ in range(world)]
+    tdist.all_gather(lst, t)
+    assert all(torch.equal(lst[0], x) for x in lst), mode   # every rank ends bit-identical
+    res[mode] = (out, L.eskf_pro)
+L.ctx.set_option("device_loop", modes[0])
+if len(modes) == 2:                                     # the two loops agree as on one GPU (test_device_resident_loop_equals_host_driven_loop)
+    (od, ed), (oh, eh) = res[1], res[0]
+    assert (od["success"], od["passes"], od["converged"], od["num_residuals_used"]) == (oh["success"], oh["passes"], oh["converged"], oh["num_residuals_used"])
+    assert np.allclose(od["trace"], oh["trace"], rtol=1e-7, atol=1e-11)
+    for f in ("p", "q", "v", "ba", "bg", "g"):
+        assert np.allclose(getattr(ed, f), getattr(eh, f), rtol=1e-9, atol=1e-11), f
+    assert np.allclose(ed.cov, eh.cov, rtol=1e-6, atol=1e-13)
+    assert np.allclose(od["frame_q"], oh["frame_q"], atol=1e-11) and np.allclose(od["frame_t"], oh["frame_t"], atol=1e-11)
 # config 3 end to end in C (srl_optimize_host_dist): host buffers in, this rank's rows of the registered sweep out
 L.ctx.set_option("fast_force_ambiguous_mod", 0)
 L.eskf_pro = lio.EskfEstimator(p=sw.t_init.copy(), q=sw.q_init.copy(), cov=synth.prior_covariance())
@@ -1123,14 +1139,14 @@ L.eskf_pro = lio.EskfEstimator(p=sw.t_init.copy(), q=sw.q_init.copy(), cov=synth
 ob = Db.updateIEKF(prm, sw.t_last)
 assert ob["passes"] == ref["passes"] and np.allclose(ob["frame_t"], o2["frame_t"], atol=1e-9) and np.allclose(ob["frame_q"], o2["frame_q"], atol=1e-9)
 D.close(); L.close(); tdist.destroy_process_group()
-print("rank", rank, "ok")
+print("rank", rank, "ok, device_loop modes", modes)
 """
 
 
 @pytest.mark.parametrize("world", [2, 4])
 def test_fused_peer_memory_exchange_ranks(tmp_path, world):
     """The sharded update with the exchange fused into the pass's last kernel (CUDA IPC mailboxes) and the ESIKF update
-    in each rank's persistent block: `world` processes (one GPU each if the box has them, else sharing GPUs), each owning
+    in each rank's persistent block, then in the host-driven loop: `world` processes (one GPU each if the box has them, else sharing GPUs), each owning
     a contiguous range of the keypoints; then the same end to end from host buffers (srl_optimize_host_dist)."""
     import os, subprocess, sys
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
