@@ -190,6 +190,22 @@ int srl_map_insert_device(srl_map* map, const double* d_xyz_world, size_t n, dou
 int srl_map_insert_sweep(srl_map* map, srl_sweep* sweep, const double q[4], const double t[3], const double R_il[9],
                          const double t_il[3], double min_distance_points, int32_t min_num_points, int64_t* n_added);
 
+/* addPointsToMap + the cloud it publishes (publishCLoudWorld, src/lioOptimization.cpp:552; addPointToPcl :432, :1346-1355).
+ * The map is updated exactly as by srl_map_insert / srl_map_insert_sweep.  The cloud holds, in sweep order, the points that
+ * were appended to a voxel map.find found: one present before the call (an uploaded voxel with count 0 included) or created
+ * by an earlier point of the same call.  A point that creates its voxel is stored but not published.  Each point is 4 floats:
+ * x, y, z as stored, intensity = (float)(50 * ((double)z - translation_z)) evaluated in FP64 and rounded once;
+ * srl_map_insert_sweep_published uses translation_z = t[2].  xyz_world and xyzi_out are host or device memory (detected per
+ * pointer; a pageable host output is staged through pinned memory).  max_out >= n always suffices; max_out < n returns
+ * SRL_BAD_ARG before the map is touched. */
+int srl_map_insert_published(srl_map* map, const double* xyz_world, size_t n, double min_distance_points,
+                             int32_t min_num_points, double translation_z, float* xyzi_out, size_t max_out,
+                             int64_t* n_added, int64_t* n_published);
+int srl_map_insert_sweep_published(srl_map* map, srl_sweep* sweep, const double q[4], const double t[3],
+                                   const double R_il[9], const double t_il[3], double min_distance_points,
+                                   int32_t min_num_points, float* xyzi_out, size_t max_out, int64_t* n_added,
+                                   int64_t* n_published);
+
 /* ---- sweep: the keypoints vector of optimize() (src/optimize.cpp:430) ------------------------ */
 int srl_sweep_create(srl_ctx* ctx, size_t capacity, srl_sweep** out);
 void srl_sweep_destroy(srl_sweep* sweep);
@@ -422,6 +438,16 @@ int srl_color_map_download_state(srl_color_map* cm, size_t max_voxels, int16_t* 
                                  double* last_obs, double* last_visited);
 /* rgb_points_vec as (voxel key x,y,z, index in block) per entry, voxels_recent_visited as voxel keys */
 int srl_color_map_download_lists(srl_color_map* cm, int16_t* rgb_points, int16_t* recent);
+/* the coloured map as the reference publishes and saves it: the rgb_points_vec entries with N_rgb >= min_views (a short
+ * against an int, so min_views <= 0 keeps points never rendered), each as x, y, z (the stored floats) and r, g, b = rgb[2],
+ * rgb[1], rgb[0] (the BGR state swapped; short -> double -> uint8_t as g++ compiles it on x86-64: the low 8 bits).
+ * order 0: pubColorPoints (src/lioOptimization.cpp:1210-1241; also one round of threadPubColorPoints' topics, concatenated),
+ * index 0 upward.  order 1: saveColorPoints (:1386-1426), index n-1 down to 1: index 0 is never saved.
+ * xyz (n*3 floats) and rgb (n*3 bytes) are host or device memory (detected per pointer; host output is staged through
+ * pinned memory in chunks); both NULL counts only.  *n_out = the number of points; with outputs, max_points smaller than
+ * that returns SRL_BAD_ARG and writes nothing. */
+int srl_color_map_export(srl_color_map* cm, int32_t min_views, int32_t order, float* xyz, uint8_t* rgb, size_t max_points,
+                         int64_t* n_out);
 
 /* eskfEstimator::observe (src/eskfEstimator.cpp:219-230) — host math, exported for parity tests */
 int srl_eskf_observe(srl_eskf_state* eskf, const double d_x[17]);

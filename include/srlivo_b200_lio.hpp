@@ -18,6 +18,8 @@
 //   transformAllImuPoint              src/utility.cpp:320           srl::LioBackend::transformAllImuPoint
 //   addPointToColorMap (loop :533-551) src/lioOptimization.cpp:448  srl::LioBackend::addPointsToColorMap
 //   rgbMapTracker::renderPointsInRecentVoxel  src/rgbMapTracker.cpp:216  srl::LioBackend::renderPointsInRecentVoxel
+//   addPointToPcl + publishCLoudWorld src/lioOptimization.cpp:432,552 srl::LioBackend::addPointsToMapPublished
+//   pubColorPoints / saveColorPoints  src/lioOptimization.cpp:1210,1386 srl::LioBackend::pubColorPoints / saveColorPoints
 #pragma once
 
 #include <array>
@@ -71,6 +73,17 @@ public:
     long long addPointsToMap(const double* xyz_world, size_t n, double min_distance_points, int min_num_points = 0) {
         int64_t added = 0;
         check(srl_map_insert(map_, xyz_world, n, min_distance_points, min_num_points, &added), "srl_map_insert");
+        return added;
+    }
+    // the same insert + the cloud publishCLoudWorld sends (src/lioOptimization.cpp:432,552, addPointToPcl :1346-1355): xyzi gets
+    // x, y, z, intensity of each published point, sweep order; translation_z = p_frame->p_state->translation.z()
+    long long addPointsToMapPublished(const double* xyz_world, size_t n, double min_distance_points, int min_num_points,
+                                      double translation_z, std::vector<float>& xyzi) {
+        xyzi.resize(n * 4);
+        int64_t added = 0, n_pub = 0;
+        check(srl_map_insert_published(map_, xyz_world, n, min_distance_points, min_num_points, translation_z, xyzi.data(), n, &added,
+                                       &n_pub), "srl_map_insert_published");
+        xyzi.resize((size_t)n_pub * 4);
         return added;
     }
     // src/lioOptimization.cpp:574-581
@@ -209,6 +222,12 @@ public:
         check(srl_color_map_render_recent(color_, &cam, image_bgr, obs_time, &rendered), "srl_color_map_render_recent");
         return rendered;
     }
+    // pubColorPoints (src/lioOptimization.cpp:1210-1241) / saveColorPoints (:1386-1426): the rgb_points_vec entries with
+    // N_rgb >= min_views (map_options.pub_point_minimum_views: 1 in config/r3live.yaml, 3 in r3live_compressed.yaml), as xyz
+    // (3 floats per point) and r, g, b bytes; publish order from index 0 up, save order from the last index down to 1
+    struct ColorPoints { std::vector<float> xyz; std::vector<uint8_t> rgb; };
+    ColorPoints pubColorPoints(int min_views) { return exportColorPoints(min_views, 0); }
+    ColorPoints saveColorPoints(int min_views) { return exportColorPoints(min_views, 1); }
     srl_color_map* colorMap() { return color_; }
 
 private:
@@ -218,6 +237,15 @@ private:
     srl_color_map* color_ = nullptr;
     srl_cloud_frame* frame_ = nullptr;
 
+    ColorPoints exportColorPoints(int min_views, int order) {
+        ColorPoints out;
+        int64_t n = 0;
+        check(srl_color_map_export(color_, min_views, order, nullptr, nullptr, 0, &n), "srl_color_map_export");
+        out.xyz.resize((size_t)n * 3);
+        out.rgb.resize((size_t)n * 3);
+        if (n) check(srl_color_map_export(color_, min_views, order, out.xyz.data(), out.rgb.data(), (size_t)n, &n), "srl_color_map_export");
+        return out;
+    }
     void check(int rc, const char* what) {
         if (rc != SRL_OK) throw std::runtime_error(std::string(what) + ": " + (ctx_ ? srl_last_error(ctx_) : "no context"));
     }

@@ -112,7 +112,7 @@ EXPORTS = [
     "srl_color_map_render_recent", "srl_color_map_download_state", "srl_color_map_download_lists",
     "srl_map_create_growable", "srl_map_capacity", "srl_color_map_create_growable", "srl_color_map_capacity",
     "srl_cloud_frame_create", "srl_cloud_frame_destroy", "srl_cloud_frame_size", "srl_cloud_frame_device", "srl_cloud_frame_download",
-    "srl_build_frame", "srl_shuffle_replay",
+    "srl_build_frame", "srl_shuffle_replay", "srl_map_insert_published", "srl_map_insert_sweep_published", "srl_color_map_export",
 ]
 
 _lib = None
@@ -155,6 +155,8 @@ def lib():
     L.srl_map_insert.argtypes = [vp, vp, sz, dbl, i32, C.POINTER(i64)]
     L.srl_map_insert_device.argtypes = [vp, vp, sz, dbl, i32, C.POINTER(i64)]
     L.srl_map_insert_sweep.argtypes = [vp, vp, vp, vp, vp, vp, dbl, i32, C.POINTER(i64)]
+    L.srl_map_insert_published.argtypes = [vp, vp, sz, dbl, i32, dbl, vp, sz, C.POINTER(i64), C.POINTER(i64)]
+    L.srl_map_insert_sweep_published.argtypes = [vp, vp, vp, vp, vp, vp, dbl, i32, vp, sz, C.POINTER(i64), C.POINTER(i64)]
     L.srl_sweep_create.argtypes = [vp, sz, C.POINTER(vp)]
     L.srl_sweep_destroy.argtypes = [vp]
     L.srl_sweep_destroy.restype = None
@@ -203,6 +205,7 @@ def lib():
     L.srl_color_map_render_recent.argtypes = [vp, C.POINTER(Camera), vp, dbl, C.POINTER(i64)]
     L.srl_color_map_download_state.argtypes = [vp, sz, vp, vp, vp, vp, vp, vp]
     L.srl_color_map_download_lists.argtypes = [vp, vp, vp]
+    L.srl_color_map_export.argtypes = [vp, i32, i32, vp, vp, sz, C.POINTER(i64)]
     L.srl_cloud_frame_create.argtypes = [vp, sz, C.POINTER(vp)]
     L.srl_cloud_frame_destroy.argtypes = [vp]
     L.srl_cloud_frame_destroy.restype = None

@@ -148,17 +148,22 @@ __global__ void k_seg_claim(Slot* slots, unsigned int mask, float* blocks, const
     seg_claim(slots, mask, blocks, kBlockFloats, keys, seg_start, n_seg_p, is_new, new_rank, block_base, seg_slot);
 }
 
-// one warp per touched voxel: the reference's per-point rule, replayed in sweep order
+// one warp per touched voxel: the reference's per-point rule, replayed in sweep order.
+// pub (nullable, one byte per sweep point, zeroed by the caller): set for a point appended to a voxel that map.find found,
+// i.e. one that was in the slot table before this call or was created by an earlier point of the sweep; those are the points
+// addPointToPcl puts into the published cloud (:432).  A point that creates its voxel (:437-444) is stored but not published.
 __global__ void __launch_bounds__(256) k_seg_process(Slot* slots, float* blocks, const unsigned long long* __restrict__ keys,
                                                       const unsigned int* __restrict__ idx, const float* __restrict__ fxyz,
                                                       const unsigned int* __restrict__ seg_start, const int* n_seg_p,
                                                       const int* __restrict__ seg_slot, long long n, double size, int cap,
-                                                      double min_dist, int min_num_points, long long* n_points) {
+                                                      double min_dist, int min_num_points, long long* n_points,
+                                                      const unsigned int* __restrict__ is_new, unsigned char* pub) {
     const int lane = threadIdx.x & 31;
     const int s = (int)(((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5);
     if (s >= *n_seg_p) return;
     const int slot = seg_slot[s];
     if (slot < 0) return;   // voxel absent and min_num_points > 0: nothing is ever created (:437)
+    bool found = pub ? !is_new[s] : false;
     const unsigned int blk = slots[slot].block;
     int count = (int)slots[slot].count;
     float* bp = blocks + (size_t)blk * kBlockFloats;
@@ -190,6 +195,10 @@ __global__ void __launch_bounds__(256) k_seg_process(Slot* slots, float* blocks,
         }
         if (add) {
             if (lane == count) { ex = fx; ey = fy; ez = fz; bp[4 * count] = fx; bp[4 * count + 1] = fy; bp[4 * count + 2] = fz; }
+            if (pub) {
+                if (found && lane == 0) pub[i] = 1;
+                found = true;
+            }
             ++count; ++added;
         }
     }
@@ -476,7 +485,79 @@ __global__ void k_gather_points(const double* __restrict__ xyz, const unsigned i
     out[3 * j] = xyz[3 * i]; out[3 * j + 1] = xyz[3 * i + 1]; out[3 * j + 2] = xyz[3 * i + 2];
 }
 
+// ---- the published maps ----------------------------------------------------------------------------------------------
+// addPointToPcl (src/lioOptimization.cpp:1346-1355) over the published points in sweep order: x, y, z the stored floats,
+// intensity = 50 * (z - translation.z()) in FP64 (float z widened), rounded once to float
+__global__ void k_publish_gather(const float* __restrict__ fxyz, const unsigned int* __restrict__ sel, const int* n_sel_p, double tz,
+                                 float* out) {
+    const long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= *n_sel_p) return;
+    const size_t i = sel[j];
+    const float z = fxyz[3 * i + 2];
+    out[4 * j] = fxyz[3 * i]; out[4 * j + 1] = fxyz[3 * i + 1]; out[4 * j + 2] = z;
+    out[4 * j + 3] = __double2float_rn(__dmul_rn(50.0, __dsub_rn((double)z, tz)));
+}
+// position p of the export (publish order: rgb_points_vec index p; save order: index n - 1 - p, so index 0 is never reached)
+// -> flag N_rgb >= min_views (short against int, :1221, :1404); the flagged count is added to *count
+__global__ void k_color_export_flags(const unsigned int* __restrict__ rgb_points, const ColorPoint* __restrict__ cpts, long long m,
+                                     long long n, int order, int min_views, unsigned char* flags, unsigned long long* count) {
+    const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    bool f = false;
+    if (p < m) {
+        const unsigned id = rgb_points[order ? n - 1 - p : p];
+        f = (int)cpts[id].n_rgb >= min_views;
+        flags[p] = f ? 1 : 0;
+    }
+    const unsigned b = __ballot_sync(0xffffffffu, f);
+    if ((threadIdx.x & 31) == 0 && b) atomicAdd(count, (unsigned long long)__popc(b));
+}
+// the flagged positions of one chunk (sel relative to base) -> getPosition() as stored, r = rgb[2], g = rgb[1], b = rgb[0]: the BGR
+// state swapped, short -> double -> uint8_t as g++ compiles it on x86-64 (int32 truncation, low 8 bits)
+__global__ void k_color_export_gather(const unsigned int* __restrict__ rgb_points, const float* __restrict__ blocks, int block_pts,
+                                      const ColorPoint* __restrict__ cpts, const unsigned int* __restrict__ sel, const int* n_sel_p,
+                                      long long base, long long n, int order, float* xyz, unsigned char* rgb) {
+    const long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= *n_sel_p) return;
+    const long long p = base + sel[k];
+    const unsigned id = rgb_points[order ? n - 1 - p : p];
+    const unsigned blk = id / (unsigned)block_pts;
+    const float* b = blocks + (size_t)blk * (4 * block_pts) + 4 * (size_t)(id - blk * (unsigned)block_pts);
+    xyz[3 * k] = b[0]; xyz[3 * k + 1] = b[1]; xyz[3 * k + 2] = b[2];
+    const ColorPoint& cp = cpts[id];
+    rgb[3 * k] = (unsigned char)(cp.rgb[2] & 0xff); rgb[3 * k + 1] = (unsigned char)(cp.rgb[1] & 0xff); rgb[3 * k + 2] = (unsigned char)(cp.rgb[0] & 0xff);
+}
+
 static inline size_t align_up(size_t x, size_t a = 256) { return (x + a - 1) / a * a; }
+
+static bool is_device_ptr(const void* p) {
+    cudaPointerAttributes attr;
+    const bool dev = cudaPointerGetAttributes(&attr, p) == cudaSuccess && attr.type == cudaMemoryTypeDevice;
+    if (!dev) cudaGetLastError();
+    return dev;
+}
+// device -> host output: page-locked destinations are written by the copy engine directly, pageable ones through the ctx's
+// pinned staging buffer in chunks of at most 64 MB (no host temporary the size of the output)
+static int copy_to_host(srl_ctx* ctx, void* dst, const void* d_src, size_t bytes) {
+    if (bytes == 0) return SRL_OK;
+    cudaPointerAttributes attr;
+    const bool pinned = cudaPointerGetAttributes(&attr, dst) == cudaSuccess && attr.type == cudaMemoryTypeHost;
+    if (!pinned) cudaGetLastError();
+    if (pinned) {
+        SRL_CUDA(ctx, cudaMemcpyAsync(dst, d_src, bytes, cudaMemcpyDeviceToHost, ctx->stream));
+        SRL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        return SRL_OK;
+    }
+    const size_t chunk = std::min(bytes, size_t(64) << 20);
+    int rc = ensure_pinned(ctx, chunk);
+    if (rc != SRL_OK) return rc;
+    for (size_t off = 0; off < bytes; off += chunk) {
+        const size_t len = std::min(chunk, bytes - off);
+        SRL_CUDA(ctx, cudaMemcpyAsync(ctx->h_pinned, static_cast<const char*>(d_src) + off, len, cudaMemcpyDeviceToHost, ctx->stream));
+        SRL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        std::memcpy(static_cast<char*>(dst) + off, ctx->h_pinned, len);
+    }
+    return SRL_OK;
+}
 
 // ---- growth: arrays on CUDA VMM, slot tables rebuilt -----------------------------------------------------------------
 // The driver's VMM calls come through the runtime's entry-point query, so the library does not link libcuda.
@@ -901,8 +982,18 @@ int srl_map_download(srl_map* m, int16_t* keys, int32_t* counts, float* xyz, siz
     return SRL_OK;
 }
 
+// the registered cloud of an insert (addPointToPcl, src/lioOptimization.cpp:432,1346-1355)
+struct PublishArgs {
+    double translation_z;   // p_frame->p_state->translation.z()
+    float* d_out;           // device destination (n * 4 floats), or null: the cloud is left in scratch at *d_cloud
+    float* d_cloud = nullptr;
+    int64_t n_published = 0;
+};
+
+static size_t publish_scratch_bytes(size_t n) { return align_up(n) + align_up(n * 4) + align_up(n * 16) + 256; }
+
 static int map_insert_impl(srl_map* m, const double* d_xyz, size_t n, double min_distance_points, int32_t min_num_points,
-                           int64_t* n_added, char* scratch_after_points) {
+                           int64_t* n_added, char* scratch_after_points, PublishArgs* pa = nullptr) {
     srl_ctx* ctx = m->ctx;
     cudaStream_t st = ctx->stream;
     // scratch carve-up
@@ -926,6 +1017,19 @@ static int map_insert_impl(srl_map* m, const double* d_xyz, size_t n, double min
     cub::DeviceScan::ExclusiveSum(nullptr, tmp_scan, is_new, new_rank, (int)n, st);
     const size_t tmp_bytes = std::max(tmp_sort, std::max(tmp_sel, tmp_scan));
     void* d_tmp = take(tmp_bytes);
+    // publication (after everything the plain insert carves, so its layout is unchanged): per-point flags, the selected
+    // sweep indices, their count, and the cloud when it is not written straight to the caller's device buffer
+    unsigned char* pub = nullptr;
+    unsigned int* pub_sel = nullptr;
+    int* d_npub = nullptr;
+    if (pa) {
+        pub = reinterpret_cast<unsigned char*>(take(n));
+        pub_sel = reinterpret_cast<unsigned int*>(take(n * 4));
+        d_npub = reinterpret_cast<int*>(take(256));
+        pa->d_cloud = pa->d_out ? pa->d_out : reinterpret_cast<float*>(take(n * 16));
+        pa->n_published = 0;
+        SRL_CUDA(ctx, cudaMemsetAsync(pub, 0, n, st));
+    }
 
     const int T = 256;
     const unsigned gb = (unsigned)((n + T - 1) / T);
@@ -967,13 +1071,23 @@ static int map_insert_impl(srl_map* m, const double* d_xyz, size_t n, double min
     }
     const unsigned gw = (unsigned)(((long long)n_seg * 32 + T - 1) / T);
     k_seg_process<<<gw, T, 0, st>>>(m->d_slots, m->d_blocks, keys_b, idx_b, fxyz, seg_start, d_nseg, seg_slot, (long long)n,
-                                    m->voxel_size, m->cap, min_distance_points, min_num_points, m->d_counters);
+                                    m->voxel_size, m->cap, min_distance_points, min_num_points, m->d_counters, is_new, pub);
     ctx->launches += 1;
     SRL_CUDA(ctx, cudaGetLastError());
+    int n_pub = 0;
+    if (pa) {   // order-preserving compaction of the flagged points, then their (x, y, z, intensity)
+        tb = tmp_bytes;
+        SRL_CUDA(ctx, cub::DeviceSelect::Flagged(d_tmp, tb, thrust::counting_iterator<unsigned int>(0), pub, pub_sel, d_npub, (int)n, st));
+        k_publish_gather<<<gb, T, 0, st>>>(fxyz, pub_sel, d_npub, pa->translation_z, pa->d_cloud);
+        SRL_CUDA(ctx, cudaGetLastError());
+        SRL_CUDA(ctx, cudaMemcpyAsync(&n_pub, d_npub, sizeof(int), cudaMemcpyDeviceToHost, st));
+        ctx->launches += 2;
+    }
     SRL_CUDA(ctx, cudaMemcpyAsync(&after, m->d_counters, sizeof(long long), cudaMemcpyDeviceToHost, st));
     SRL_CUDA(ctx, cudaStreamSynchronize(st));
     m->n_voxels += total_new;
     if (n_added) *n_added = after - before;
+    if (pa) pa->n_published = n_pub;
     return SRL_OK;
 }
 
@@ -1463,6 +1577,133 @@ int srl_map_insert(srl_map* m, const double* xyz_world, size_t n, double min_dis
     char* base = static_cast<char*>(ctx->d_scratch);
     SRL_CUDA(ctx, cudaMemcpyAsync(base, xyz_world, n * 3 * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
     return map_insert_impl(m, reinterpret_cast<const double*>(base), n, min_distance_points, min_num_points, n_added, base + pts_bytes);
+}
+
+}  // extern "C"
+
+// the argument checks of the published inserts: nothing is touched before they pass
+static int check_published(srl_map* m, size_t n, const float* xyzi_out, size_t max_out, int64_t* n_added, int64_t* n_published) {
+    srl_ctx* ctx = m->ctx;
+    if (n_added) *n_added = 0;
+    if (n_published) *n_published = 0;
+    if (int rc = check_lio_map(ctx, m)) return rc;
+    if (n && !xyzi_out) return set_err(ctx, SRL_BAD_ARG, "srl_map_insert_published: xyzi_out is NULL");
+    if (max_out < n) return set_err(ctx, SRL_BAD_ARG, "srl_map_insert_published: max_out < n (up to n points can be published)");
+    if (n > 0x7fffffffULL) return set_err(ctx, SRL_BAD_ARG, "srl_map_insert: n must fit in int32");
+    return SRL_OK;
+}
+// the insert with publication, then the cloud to a host destination if it was staged in scratch
+static int insert_published(srl_map* m, const double* d_xyz, size_t n, double min_distance_points, int32_t min_num_points,
+                            double translation_z, float* xyzi_out, int64_t* n_added, int64_t* n_published, char* scratch_after_points) {
+    PublishArgs pa;
+    pa.translation_z = translation_z;
+    const bool out_dev = is_device_ptr(xyzi_out);
+    pa.d_out = out_dev ? xyzi_out : nullptr;
+    int rc = map_insert_impl(m, d_xyz, n, min_distance_points, min_num_points, n_added, scratch_after_points, &pa);
+    if (rc != SRL_OK) return rc;
+    if (!out_dev && (rc = copy_to_host(m->ctx, xyzi_out, pa.d_cloud, (size_t)pa.n_published * 16)) != SRL_OK) return rc;
+    if (n_published) *n_published = pa.n_published;
+    return SRL_OK;
+}
+
+extern "C" {
+
+int srl_map_insert_published(srl_map* m, const double* xyz_world, size_t n, double min_distance_points, int32_t min_num_points,
+                             double translation_z, float* xyzi_out, size_t max_out, int64_t* n_added, int64_t* n_published) {
+    if (!m || (n && !xyz_world)) return SRL_BAD_ARG;
+    int rc = check_published(m, n, xyzi_out, max_out, n_added, n_published);
+    if (rc != SRL_OK || n == 0) return rc;
+    srl_ctx* ctx = m->ctx;
+    SRL_CUDA(ctx, cudaSetDevice(ctx->device));
+    const bool in_dev = is_device_ptr(xyz_world);
+    const size_t pts_bytes = in_dev ? 0 : align_up(n * 3 * sizeof(double));
+    if ((rc = ensure_scratch(ctx, pts_bytes + insert_scratch_bytes(n) + publish_scratch_bytes(n))) != SRL_OK) return rc;
+    char* base = static_cast<char*>(ctx->d_scratch);
+    if (!in_dev) SRL_CUDA(ctx, cudaMemcpyAsync(base, xyz_world, n * 3 * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+    return insert_published(m, in_dev ? xyz_world : reinterpret_cast<const double*>(base), n, min_distance_points, min_num_points,
+                            translation_z, xyzi_out, n_added, n_published, base + pts_bytes);
+}
+
+int srl_map_insert_sweep_published(srl_map* m, srl_sweep* sw, const double q[4], const double t[3], const double R_il[9],
+                                   const double t_il[3], double min_distance_points, int32_t min_num_points, float* xyzi_out,
+                                   size_t max_out, int64_t* n_added, int64_t* n_published) {
+    if (!m || !sw || !q || !t || !R_il || !t_il) return SRL_BAD_ARG;
+    const size_t n = sw->n;
+    int rc = check_published(m, n, xyzi_out, max_out, n_added, n_published);
+    if (rc != SRL_OK) return rc;
+    srl_ctx* ctx = m->ctx;
+    if (sw->ctx != ctx) return set_err(ctx, SRL_BAD_ARG, "map and sweep belong to different contexts");
+    if (n == 0) return SRL_OK;
+    SRL_CUDA(ctx, cudaSetDevice(ctx->device));
+    const size_t pts_bytes = align_up(n * 3 * sizeof(double));
+    if ((rc = ensure_scratch(ctx, pts_bytes + insert_scratch_bytes(n) + publish_scratch_bytes(n))) != SRL_OK) return rc;
+    char* base = static_cast<char*>(ctx->d_scratch);
+    if ((rc = srl_sweep_transform_device(ctx, sw, q, t, R_il, t_il, reinterpret_cast<double*>(base))) != SRL_OK) return rc;
+    return insert_published(m, reinterpret_cast<const double*>(base), n, min_distance_points, min_num_points, t[2], xyzi_out, n_added,
+                            n_published, base + pts_bytes);
+}
+
+int srl_color_map_export(srl_color_map* cm, int32_t min_views, int32_t order, float* xyz, uint8_t* rgb, size_t max_points, int64_t* n_out) {
+    if (!cm || !n_out) return SRL_BAD_ARG;
+    *n_out = 0;
+    srl_ctx* ctx = cm->ctx;
+    if (order != 0 && order != 1) return set_err(ctx, SRL_BAD_ARG, "srl_color_map_export: order is 0 (publish) or 1 (save)");
+    if ((xyz == nullptr) != (rgb == nullptr)) return set_err(ctx, SRL_BAD_ARG, "srl_color_map_export: xyz and rgb are both NULL (count) or both set");
+    const long long n = cm->n_rgb_points;
+    const long long m = order ? std::max(n - 1, 0LL) : n;   // saveColorPoints stops before index 0 (:1398)
+    if (m == 0) return SRL_OK;
+    SRL_CUDA(ctx, cudaSetDevice(ctx->device));
+    cudaStream_t st = ctx->stream;
+    srl_map* vm = cm->vox;
+    const long long chunk = std::min<long long>(m, 1ll << 22);
+    const bool xyz_dev = xyz && is_device_ptr(xyz), rgb_dev = rgb && is_device_ptr(rgb);
+    size_t tmp_sel = 0;
+    cub::DeviceSelect::Flagged(nullptr, tmp_sel, thrust::counting_iterator<unsigned int>(0), (unsigned char*)nullptr, (unsigned int*)nullptr,
+                               (int*)nullptr, (int)chunk, st);
+    const size_t need = align_up((size_t)m) + 2 * 256 + align_up((size_t)chunk * 4) + align_up(tmp_sel) + align_up((size_t)chunk * 12) +
+                        align_up((size_t)chunk * 3);
+    int rc = ensure_scratch(ctx, need);
+    if (rc != SRL_OK) return rc;
+    char* p = static_cast<char*>(ctx->d_scratch);
+    auto take = [&](size_t bytes) { char* r = p; p += align_up(bytes); return r; };
+    unsigned char* flags = reinterpret_cast<unsigned char*>(take((size_t)m));
+    unsigned long long* d_count = reinterpret_cast<unsigned long long*>(take(256));
+    int* d_nsel = reinterpret_cast<int*>(take(256));
+    unsigned int* sel = reinterpret_cast<unsigned int*>(take((size_t)chunk * 4));
+    void* d_tmp = take(tmp_sel);
+    float* stage_xyz = reinterpret_cast<float*>(take((size_t)chunk * 12));
+    unsigned char* stage_rgb = reinterpret_cast<unsigned char*>(take((size_t)chunk * 3));
+    const int T = 256;
+    SRL_CUDA(ctx, cudaMemsetAsync(d_count, 0, 8, st));
+    k_color_export_flags<<<(unsigned)((m + T - 1) / T), T, 0, st>>>(cm->d_rgb_points, cm->d_cpts, m, n, order, min_views, flags, d_count);
+    SRL_CUDA(ctx, cudaGetLastError());
+    unsigned long long total = 0;
+    SRL_CUDA(ctx, cudaMemcpyAsync(&total, d_count, 8, cudaMemcpyDeviceToHost, st));
+    SRL_CUDA(ctx, cudaStreamSynchronize(st));
+    ctx->launches += 1;
+    *n_out = (int64_t)total;
+    if (!xyz || total == 0) return SRL_OK;
+    if (total > max_points) return set_err(ctx, SRL_BAD_ARG, "srl_color_map_export: max_points is smaller than the number of points (count with NULL outputs first)");
+    // one chunk of positions at a time: compact its flags (sweep of the list in output order), gather, hand over
+    size_t off = 0;
+    for (long long base = 0; base < m; base += chunk) {
+        const long long len = std::min(chunk, m - base);
+        size_t tb = tmp_sel;
+        SRL_CUDA(ctx, cub::DeviceSelect::Flagged(d_tmp, tb, thrust::counting_iterator<unsigned int>(0), flags + base, sel, d_nsel, (int)len, st));
+        float* dx = xyz_dev ? xyz + 3 * off : stage_xyz;
+        unsigned char* dr = rgb_dev ? rgb + 3 * off : stage_rgb;
+        k_color_export_gather<<<(unsigned)((len + T - 1) / T), T, 0, st>>>(cm->d_rgb_points, vm->d_blocks, vm->block_pts, cm->d_cpts, sel, d_nsel,
+                                                                          base, n, order, dx, dr);
+        SRL_CUDA(ctx, cudaGetLastError());
+        int k = 0;
+        SRL_CUDA(ctx, cudaMemcpyAsync(&k, d_nsel, sizeof(int), cudaMemcpyDeviceToHost, st));
+        SRL_CUDA(ctx, cudaStreamSynchronize(st));
+        ctx->launches += 2;
+        if (!xyz_dev && (rc = copy_to_host(ctx, xyz + 3 * off, stage_xyz, (size_t)k * 12)) != SRL_OK) return rc;
+        if (!rgb_dev && (rc = copy_to_host(ctx, rgb + 3 * off, stage_rgb, (size_t)k * 3)) != SRL_OK) return rc;
+        off += (size_t)k;
+    }
+    return SRL_OK;
 }
 
 }  // extern "C"

@@ -9,6 +9,8 @@ Names and argument meaning follow the reference so the parity tests read like it
   lioOptimization::updateIEKF           src/optimize.cpp:133-314        -> LioOptimization.updateIEKF
   lioOptimization::optimize             src/optimize.cpp:428-448        -> LioOptimization.optimize (keypoints given)
   eskfEstimator (state + observe)       src/eskfEstimator.cpp           -> EskfEstimator
+  addPointToPcl / publishCLoudWorld     src/lioOptimization.cpp:432,552 -> LioOptimization.addPointsToMapPublished
+  pubColorPoints / saveColorPoints      src/lioOptimization.cpp:1210,1386 -> ColorVoxelMap.pubColorPoints / saveColorPoints
 
 Error behaviour: optimizeSummary.success=false <-> OptimizeSummary.success False (SRL_TOO_FEW_RESIDUALS);
 the reference's `throw std::runtime_error("error")` on NaN planarity <-> RuntimeError; everything else raises
@@ -32,6 +34,48 @@ def _check(ctx, rc, ok=(capi.SRL_OK,)):
     if rc not in ok:
         raise SrlError(rc, lib().srl_last_error(ctx).decode() if ctx else "")
     return rc
+
+
+def _is_tensor(a) -> bool:
+    return type(a).__module__.split(".")[0] == "torch"
+
+
+def _addr(a, dtype, width):
+    """(address, rows) of a C-contiguous buffer of `width` elements of `dtype` per row: a numpy array (host) or a torch tensor
+    (host or CUDA; the C ABI tells host from device per pointer)."""
+    if _is_tensor(a):
+        if str(a.dtype) != "torch." + np.dtype(dtype).name or not a.is_contiguous():
+            raise TypeError(f"expected a contiguous torch.{np.dtype(dtype).name} tensor")
+        return a.data_ptr(), a.numel() // width
+    if not (isinstance(a, np.ndarray) and a.dtype == dtype and a.flags.c_contiguous):
+        raise TypeError(f"expected a C-contiguous {np.dtype(dtype).name} array")
+    return a.ctypes.data, a.size // width
+
+
+def _empty_like_input(a, rows, width, dtype):
+    if _is_tensor(a):
+        import torch
+        return torch.empty((rows, width), dtype=getattr(torch, np.dtype(dtype).name), device=a.device)
+    return np.empty((rows, width), dtype)
+
+
+def write_pcd_xyzrgb(path: str, xyz, rgb) -> None:
+    """A binary PCD v0.7 file of pcl::PointXYZRGB points as pcl::io::savePCDFileBinary writes one: fields x y z rgb, 16 bytes per
+    point, rgb the float whose bits are a << 24 | r << 16 | g << 8 | b with a = 255 (what PointXYZRGB's constructors set).
+    Header layout and alpha are taken from PCL's published sources (DESIGN.md section 2)."""
+    xyz = np.ascontiguousarray(xyz, np.float32).reshape(-1, 3)
+    rgb = np.ascontiguousarray(rgb, np.uint8).reshape(-1, 3)
+    n = xyz.shape[0]
+    assert rgb.shape[0] == n
+    rec = np.empty((n, 4), np.float32)
+    rec[:, :3] = xyz
+    c = rgb.astype(np.uint32)
+    rec.view(np.uint32)[:, 3] = (np.uint32(255) << 24) | (c[:, 0] << 16) | (c[:, 1] << 8) | c[:, 2]
+    header = ("# .PCD v0.7 - Point Cloud Data file format\nVERSION 0.7\nFIELDS x y z rgb\nSIZE 4 4 4 4\nTYPE F F F F\nCOUNT 1 1 1 1\n"
+              f"WIDTH {n}\nHEIGHT 1\nVIEWPOINT 0 0 0 1 0 0 0\nPOINTS {n}\nDATA binary\n")
+    with open(path, "wb") as f:
+        f.write(header.encode("ascii"))
+        f.write(rec.tobytes())
 
 
 class Context:
@@ -157,6 +201,20 @@ class VoxelHashMap:
                                                        min_num_points, C.byref(added)))
         return added.value
 
+    def insert_published(self, xyz_world, translation_z: float, min_distance_points: float = 0.15, min_num_points: int = 0, out=None):
+        """insert + the cloud addPointsToMap publishes (srl_map_insert_published): (points stored, xyzi) with xyzi the first
+        n_published rows of `out` (n x 4 float32: x, y, z, intensity, sweep order).  xyz_world is an (n, 3) float64 numpy array
+        or torch tensor (host or CUDA); out, when not given, is allocated like the input."""
+        if not _is_tensor(xyz_world):
+            xyz_world = f64(xyz_world).reshape(-1, 3)
+        p_in, n = _addr(xyz_world, np.float64, 3)
+        out = _empty_like_input(xyz_world, n, 4, np.float32) if out is None else out
+        p_out, max_out = _addr(out, np.float32, 4)
+        added, n_pub = C.c_int64(0), C.c_int64(0)
+        _check(self.ctx.h, lib().srl_map_insert_published(self.h, C.c_void_p(p_in), n, min_distance_points, min_num_points, float(translation_z),
+                                                          C.c_void_p(p_out), max_out, C.byref(added), C.byref(n_pub)))
+        return added.value, out[:n_pub.value]
+
 
 def r3live_map_options() -> dict:
     """`map_options` of config/r3live.yaml:71-76 (config/ntu.yaml:70-75 has the same values): the colour map's parameters."""
@@ -225,6 +283,42 @@ class ColorVoxelMap:
         n = C.c_int64(0)
         _check(self.ctx.h, lib().srl_color_map_render_recent(self.h, C.byref(camera), ptr(img), float(obs_time), C.byref(n)))
         return n.value
+
+    def exportColorPoints(self, min_views: int = 1, order: int = 0, xyz=None, rgb=None):
+        """srl_color_map_export: the rgb_points_vec entries with N_rgb >= min_views as ((n, 3) float32 positions, (n, 3) uint8 r, g, b).
+        order 0 is pubColorPoints' order, order 1 saveColorPoints'.  xyz / rgb (numpy arrays or torch tensors, host or CUDA) receive
+        the points when given (the first n rows are returned), else numpy arrays are allocated."""
+        if (xyz is None) != (rgb is None):
+            raise ValueError("give both xyz and rgb, or neither")
+        n = C.c_int64(0)
+        if xyz is None:
+            _check(self.ctx.h, lib().srl_color_map_export(self.h, int(min_views), int(order), None, None, 0, C.byref(n)))
+            xyz, rgb = np.empty((n.value, 3), np.float32), np.empty((n.value, 3), np.uint8)
+        p_xyz, cap = _addr(xyz, np.float32, 3)
+        p_rgb, cap_rgb = _addr(rgb, np.uint8, 3)
+        _check(self.ctx.h, lib().srl_color_map_export(self.h, int(min_views), int(order), C.c_void_p(p_xyz), C.c_void_p(p_rgb),
+                                                      min(cap, cap_rgb), C.byref(n)))
+        return xyz[:n.value], rgb[:n.value]
+
+    def countColorPoints(self, min_views: int = 1, order: int = 0) -> int:
+        """How many points exportColorPoints(min_views, order) hands out."""
+        n = C.c_int64(0)
+        _check(self.ctx.h, lib().srl_color_map_export(self.h, int(min_views), int(order), None, None, 0, C.byref(n)))
+        return n.value
+
+    def pubColorPoints(self, min_views: int = 1, xyz=None, rgb=None):
+        """pubColorPoints (src/lioOptimization.cpp:1210-1241): rgb_points_vec from index 0 up (one round of threadPubColorPoints'
+        topics, concatenated).  min_views is map_options.pub_point_minimum_views: 1 in r3live_map_options(), 3 in
+        r3live_compressed_map_options()."""
+        return self.exportColorPoints(min_views, 0, xyz, rgb)
+
+    def saveColorPoints(self, path: str | None = None, min_views: int = 1):
+        """saveColorPoints (src/lioOptimization.cpp:1386-1426): rgb_points_vec from the last index down to 1 (index 0 is never
+        saved); with a path, also writes the binary PCD (write_pcd_xyzrgb) the reference writes to rgb_map.pcd."""
+        xyz, rgb = self.exportColorPoints(min_views, 1)
+        if path is not None:
+            write_pcd_xyzrgb(path, xyz, rgb)
+        return xyz, rgb
 
     def download(self) -> dict:
         """voxel contents + colour state (block order) + the two lists."""
@@ -416,6 +510,25 @@ class LioOptimization:
                                                       min_distance_points, min_num_points, C.byref(added)))
         return added.value
 
+    def addPointsToMapPublished(self, points_world, translation_z: float, min_distance_points: float = 0.15, min_num_points: int = 0,
+                                out=None):
+        """addPointsToMap and the cloud it publishes (publishCLoudWorld, src/lioOptimization.cpp:552): (points stored, xyzi), xyzi
+        (n_published, 4) float32 x, y, z, intensity = 50 * (z - translation_z), in sweep order (VoxelHashMap.insert_published)."""
+        return self.voxel_map.insert_published(points_world, translation_z, min_distance_points, min_num_points, out)
+
+    def addSweepToMapPublished(self, frame_q, frame_t, min_distance_points: float = 0.15, min_num_points: int = 0, out=None):
+        """addSweepToMap and the cloud it publishes, intensity relative to frame_t[2] (srl_map_insert_sweep_published).  out: n x 4
+        float32 (numpy or torch, host or CUDA); a numpy array is allocated when not given."""
+        q, t = f64(frame_q), f64(frame_t)
+        R, ti = f64(self.R_imu_lidar).reshape(9), f64(self.t_imu_lidar)
+        out = np.empty((self.sweep.n, 4), np.float32) if out is None else out
+        p_out, max_out = _addr(out, np.float32, 4)
+        added, n_pub = C.c_int64(0), C.c_int64(0)
+        _check(self.ctx.h, lib().srl_map_insert_sweep_published(self.voxel_map.h, self.sweep.h, ptr(q), ptr(t), ptr(R), ptr(ti),
+                                                                min_distance_points, min_num_points, C.c_void_p(p_out), max_out,
+                                                                C.byref(added), C.byref(n_pub)))
+        return added.value, out[:n_pub.value]
+
     # ---- src/lioOptimization.cpp:786-893
     def buildFrame(self, raw_xyz, timestamp, imu_states, timestamp_begin: float, timestamp_offset: float, index_frame: int,
                    q_pred=None, t_pred=None, point_time_enable: bool = True, motion_compensation: int = 1, init_num_frames: int = 20,
@@ -595,4 +708,4 @@ class LioOptimization:
 
 
 __all__ = ["Context", "VoxelHashMap", "ColorVoxelMap", "Sweep", "EskfEstimator", "LioOptimization", "OptimizeSummary", "PlaneResiduals",
-           "IcpParams", "r3live_params", "r3live_map_options", "r3live_compressed_map_options", "make_frame", "SrlError"]
+           "IcpParams", "r3live_params", "r3live_map_options", "r3live_compressed_map_options", "make_frame", "SrlError", "write_pcd_xyzrgb"]
