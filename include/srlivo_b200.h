@@ -449,6 +449,42 @@ int srl_color_map_download_lists(srl_color_map* cm, int16_t* rgb_points, int16_t
 int srl_color_map_export(srl_color_map* cm, int32_t min_views, int32_t order, float* xyz, uint8_t* rgb, size_t max_points,
                          int64_t* n_out);
 
+/* rgbMapTracker::selectPointsForProjection (src/rgbMapTracker.cpp:45-152), the points the optical-flow tracker is seeded and
+ * refreshed with.  The reference's calls:
+ *   first image (src/imageProcessing.cpp:131):  minimum_dis = track_windows_size / image_scale_factor, skip_step 1, recent
+ *   refreshPointsForProjection (:159, src/rgbMapTracker.cpp:26-43): minimum_dis 10, skip_step 1, recent, from the camera that
+ *     updatePoseForProjection(p_frame, -0.4) set up, i.e. fov_margin -0.4 (points up to 40 % outside the image).  Its early
+ *     returns (image_cols == 0, the same frame_id as the last refresh) are the caller's state.
+ * Candidates, in point_index order 0, skip_step, 2 skip_step, ...: the last point of every entry of the recent-voxel list the
+ * renderer reads, in stored order (a voxel listed twice is two candidates), or rgb_points_vec when use_all_points is set or the
+ * recent list is empty.  A candidate is skipped when depth = |p - t_world_camera| (the stored float widened) is > maximum_depth
+ * or < minimum_depth, or when the renderer's projection (scale 1, the camera's own fov_margin, negative values included) refuses
+ * it.  Its cell is u = (int)(std::round(u_f / minimum_dis) * minimum_dis), the same for v; a cell goes to its first candidate,
+ * then to every later one whose depth is below the float the cell stores ((float)depth of its holder).  The winners come out in
+ * point_index order: point_ids (block * block_pts + index, the ids of rgb_points_vec), xyz (the stored floats, 3 per point),
+ * uv (the raw projection as floats, cv::Point2f(u_f, v_f), 2 per point).  Any output may be NULL, all NULL counts only; each is
+ * host or device memory (detected per pointer; host output is staged through pinned memory).  *n_out = the number of points;
+ * with outputs, max_points smaller than that returns SRL_BAD_ARG and writes nothing.  The map and both lists are not changed.
+ * SRL_BAD_ARG also for minimum_dis not finite or <= 0, skip_step < 1, cols or rows < 2 (what the renderer refuses), and a
+ * fov_margin whose window's cell coordinates do not fit an int.
+ * Point ids stay valid while the map grows (blocks never move); srl_map_remove_far refuses a colour map's voxel map. */
+typedef struct srl_projection_params {
+    double minimum_dis;                    /* cell size in pixels: 5 (default), 10 (refreshPointsForProjection),
+                                              track_windows_size / image_scale_factor (first image) */
+    int32_t skip_step;                     /* >= 1 */
+    int32_t use_all_points;
+    double minimum_depth, maximum_depth;   /* minimum/maximum_depth_for_projection: 0.1 and 200 in the reference */
+} srl_projection_params;
+int srl_color_map_select_for_projection(srl_color_map* cm, const srl_camera* cam, const srl_projection_params* prm,
+                                        uint32_t* point_ids, float* xyz, float* uv, size_t max_points, int64_t* n_out);
+/* the per-point state the tracker reads, by point id (opticalFlowTracker.cpp:25,75,226,280 read positions;
+ * imageProcessing.cpp:465-478 colour, N_rgb and covariance): xyz n*3 floats, rgb n*3 shorts (the BGR state as stored),
+ * n_rgb n shorts, cov n*3 floats (0 before the first observation), key_index n*4 shorts (voxel key x, y, z, index in block).
+ * point_ids and every output are host or device memory; any output may be NULL.  An id that names no stored point returns
+ * SRL_BAD_ARG and writes nothing. */
+int srl_color_map_gather_points(srl_color_map* cm, const uint32_t* point_ids, size_t n, float* xyz, int16_t* rgb,
+                                int16_t* n_rgb, float* cov, int16_t* key_index);
+
 /* eskfEstimator::observe (src/eskfEstimator.cpp:219-230) — host math, exported for parity tests */
 int srl_eskf_observe(srl_eskf_state* eskf, const double d_x[17]);
 

@@ -20,6 +20,7 @@
 //   rgbMapTracker::renderPointsInRecentVoxel  src/rgbMapTracker.cpp:216  srl::LioBackend::renderPointsInRecentVoxel
 //   addPointToPcl + publishCLoudWorld src/lioOptimization.cpp:432,552 srl::LioBackend::addPointsToMapPublished
 //   pubColorPoints / saveColorPoints  src/lioOptimization.cpp:1210,1386 srl::LioBackend::pubColorPoints / saveColorPoints
+//   rgbMapTracker::selectPointsForProjection src/rgbMapTracker.cpp:45 srl::LioBackend::selectPointsForProjection / gatherColorPoints
 #pragma once
 
 #include <array>
@@ -228,6 +229,31 @@ public:
     struct ColorPoints { std::vector<float> xyz; std::vector<uint8_t> rgb; };
     ColorPoints pubColorPoints(int min_views) { return exportColorPoints(min_views, 0); }
     ColorPoints saveColorPoints(int min_views) { return exportColorPoints(min_views, 1); }
+    // rgbMapTracker::selectPointsForProjection (src/rgbMapTracker.cpp:45-152): ids (point ids, block * block_pts + index) and uv
+    // (u_f, v_f per point) of the selected points in point_index order; returns their number.  refreshPointsForProjection is
+    // {10, 1, 0, 0.1, 200} from a camera with fov_margin -0.4; the first image uses minimum_dis = track_windows_size /
+    // image_scale_factor.  Refresh's early returns (image_cols == 0, the same frame_id) stay with the caller.
+    long long selectPointsForProjection(const srl_camera& cam, const srl_projection_params& prm, std::vector<uint32_t>& ids,
+                                        std::vector<float>& uv) {
+        int64_t nv = 0, np = 0, nrgb = 0, nrec = 0, nnew = 0;
+        check(srl_color_map_stats(color_, &nv, &np, &nrgb, &nrec, &nnew), "srl_color_map_stats");
+        const int64_t total = (prm.use_all_points || nrec == 0) ? nrgb : nrec;
+        const int64_t step = prm.skip_step > 0 ? prm.skip_step : 1;
+        const size_t bound = (size_t)((total + step - 1) / step);   // at most one point per candidate
+        ids.resize(bound);
+        uv.resize(bound * 2);
+        int64_t n = 0;
+        check(srl_color_map_select_for_projection(color_, &cam, &prm, ids.data(), nullptr, uv.data(), bound, &n),
+              "srl_color_map_select_for_projection");
+        ids.resize((size_t)n);
+        uv.resize((size_t)n * 2);
+        return n;
+    }
+    // the tracked points' state by id (positions: opticalFlowTracker.cpp:25,75,226,280; colour, N_rgb, covariance after each
+    // rendering: imageProcessing.cpp:465-478); any output may be nullptr, each holds n * (3, 3, 1, 3) values
+    void gatherColorPoints(const std::vector<uint32_t>& ids, float* xyz, int16_t* rgb, int16_t* n_rgb, float* cov) {
+        check(srl_color_map_gather_points(color_, ids.data(), ids.size(), xyz, rgb, n_rgb, cov, nullptr), "srl_color_map_gather_points");
+    }
     srl_color_map* colorMap() { return color_; }
 
 private:

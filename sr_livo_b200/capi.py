@@ -71,6 +71,12 @@ class Camera(C.Structure):
                 ("cols", C.c_int32), ("rows", C.c_int32)]
 
 
+class ProjectionParams(C.Structure):
+    """srl_projection_params: the arguments of rgbMapTracker::selectPointsForProjection and the tracker's depth bounds."""
+    _fields_ = [("minimum_dis", C.c_double), ("skip_step", C.c_int32), ("use_all_points", C.c_int32), ("minimum_depth", C.c_double),
+                ("maximum_depth", C.c_double)]
+
+
 class BuildFrameParams(C.Structure):
     """srl_build_frame_params: buildFrame's inputs (src/lioOptimization.cpp:821-893)."""
     _fields_ = [("timestamp_begin", C.c_double), ("timestamp_offset", C.c_double), ("point_time_enable", C.c_int32),
@@ -113,6 +119,7 @@ EXPORTS = [
     "srl_map_create_growable", "srl_map_capacity", "srl_color_map_create_growable", "srl_color_map_capacity",
     "srl_cloud_frame_create", "srl_cloud_frame_destroy", "srl_cloud_frame_size", "srl_cloud_frame_device", "srl_cloud_frame_download",
     "srl_build_frame", "srl_shuffle_replay", "srl_map_insert_published", "srl_map_insert_sweep_published", "srl_color_map_export",
+    "srl_color_map_select_for_projection", "srl_color_map_gather_points",
 ]
 
 _lib = None
@@ -206,6 +213,8 @@ def lib():
     L.srl_color_map_download_state.argtypes = [vp, sz, vp, vp, vp, vp, vp, vp]
     L.srl_color_map_download_lists.argtypes = [vp, vp, vp]
     L.srl_color_map_export.argtypes = [vp, i32, i32, vp, vp, sz, C.POINTER(i64)]
+    L.srl_color_map_select_for_projection.argtypes = [vp, C.POINTER(Camera), C.POINTER(ProjectionParams), vp, vp, vp, sz, C.POINTER(i64)]
+    L.srl_color_map_gather_points.argtypes = [vp, vp, sz, vp, vp, vp, vp, vp]
     L.srl_cloud_frame_create.argtypes = [vp, sz, C.POINTER(vp)]
     L.srl_cloud_frame_destroy.argtypes = [vp]
     L.srl_cloud_frame_destroy.restype = None

@@ -11,6 +11,7 @@
 #include <cub/cub.cuh>
 #include <thrust/iterator/counting_iterator.h>
 
+#include <limits>
 #include <mutex>
 #include <tr1/unordered_map>
 
@@ -363,23 +364,32 @@ __device__ __forceinline__ unsigned char sat_u8(double v) {       // cv::saturat
     return (unsigned char)(r < 0 ? 0 : (r > 255 ? 255 : r));
 }
 __device__ __forceinline__ unsigned char sat_add_u8(unsigned char a, unsigned char b) { const int r = (int)a + (int)b; return (unsigned char)(r > 255 ? 255 : r); }
+// cloudFrame::project3dPointInThisImage with scale 1 (src/lioOptimization.cpp:142-198) of a stored position widened to double:
+// project3dTo2d (reject pcz < 0.001), then if2dPointsAvailable with the frame's own fov_margin.  Products and sums rounded one
+// by one like the host code.  The renderer and the tracker's selection both project through it.
+__device__ __forceinline__ bool project_in_image(const CamConst& c, double px, double py, double pz, double& u, double& v) {
+    double cxm, cym, czm;
+    matvec3_exact(c.R, px, py, pz, cxm, cym, czm);
+    const double pcx = __dadd_rn(cxm, c.t_cw[0]), pcy = __dadd_rn(cym, c.t_cw[1]), pcz = __dadd_rn(czm, c.t_cw[2]);
+    if (pcz < 0.001) return false;
+    u = __dadd_rn(__ddiv_rn(__dmul_rn(pcx, c.fx), pcz), c.cx);
+    v = __dadd_rn(__ddiv_rn(__dmul_rn(pcy, c.fy), pcz), c.cy);
+    return (u >= __dadd_rn(__dmul_rn(c.fov, (double)c.cols), 1.0)) && (ceil(u) < __dmul_rn(__dsub_rn(1.0, c.fov), (double)c.cols)) &&
+           (v >= __dadd_rn(__dmul_rn(c.fov, (double)c.rows), 1.0)) && (ceil(v) < __dmul_rn(__dsub_rn(1.0, c.fov), (double)c.rows));
+}
+// (point_world - t_world_camera).norm(), the 3-term sum as c0 + (c1 + c2) (DESIGN.md section 2)
+__device__ __forceinline__ double camera_distance(const CamConst& c, double px, double py, double pz) {
+    const double dx = __dsub_rn(px, c.t_wc[0]), dy = __dsub_rn(py, c.t_wc[1]), dz = __dsub_rn(pz, c.t_wc[2]);
+    return __dsqrt_rn(__dadd_rn(__dmul_rn(dx, dx), __dadd_rn(__dmul_rn(dy, dy), __dmul_rn(dz, dz))));
+}
 // one stored point: project, sample the image, fuse `reps` times in a row (the voxel's repetitions in the recent list);
 // returns how many of those fusions updateRgb counted
 __device__ __forceinline__ unsigned render_point(const float* __restrict__ bp, ColorPoint* cpt, const CamConst& c,
                                                  const unsigned char* __restrict__ img, double obs_time, int reps) {
     const double px = (double)bp[0], py = (double)bp[1], pz = (double)bp[2];
-    // project3dTo2d (src/lioOptimization.cpp:132-152), scale 1: products and sums rounded one by one like the host code
-    double cxm, cym, czm;
-    matvec3_exact(c.R, px, py, pz, cxm, cym, czm);
-    const double pcx = __dadd_rn(cxm, c.t_cw[0]), pcy = __dadd_rn(cym, c.t_cw[1]), pcz = __dadd_rn(czm, c.t_cw[2]);
-    if (pcz < 0.001) return 0;
-    const double u = __dadd_rn(__ddiv_rn(__dmul_rn(pcx, c.fx), pcz), c.cx);
-    const double v = __dadd_rn(__ddiv_rn(__dmul_rn(pcy, c.fy), pcz), c.cy);
-    // if2dPointsAvailable (:49-60)
-    if (!((u >= __dadd_rn(__dmul_rn(c.fov, (double)c.cols), 1.0)) && (ceil(u) < __dmul_rn(__dsub_rn(1.0, c.fov), (double)c.cols)) &&
-          (v >= __dadd_rn(__dmul_rn(c.fov, (double)c.rows), 1.0)) && (ceil(v) < __dmul_rn(__dsub_rn(1.0, c.fov), (double)c.rows)))) return 0;
-    const double dx = __dsub_rn(px, c.t_wc[0]), dy = __dsub_rn(py, c.t_wc[1]), dz = __dsub_rn(pz, c.t_wc[2]);
-    const double dist = __dsqrt_rn(__dadd_rn(__dmul_rn(dx, dx), __dadd_rn(__dmul_rn(dy, dy), __dmul_rn(dz, dz))));
+    double u, v;
+    if (!project_in_image(c, px, py, pz, u, v)) return 0;
+    const double dist = camera_distance(c, px, py, pz);
     // getSubPixel<cv::Vec3b> (:71-98): four saturated products, three saturated sums per channel
     const int fr = (int)floor(v), fc = (int)floor(u);
     const double frac_r = __dsub_rn(v, (double)fr), frac_c = __dsub_rn(u, (double)fc);
@@ -476,6 +486,129 @@ __global__ void k_color_rgb_ids(const unsigned int* __restrict__ rgb_points, lon
     short x, y, z;
     unpack_key((unsigned long long)meta[kMetaKeyLo] | ((unsigned long long)meta[kMetaKeyHi] << 32), x, y, z);
     out[4 * t] = x; out[4 * t + 1] = y; out[4 * t + 2] = z; out[4 * t + 3] = (short)(id - blk * (unsigned)block_pts);
+}
+
+// ---- rgbMapTracker::selectPointsForProjection (src/rgbMapTracker.cpp:45-152) -----------------------------------------------
+// The reference walks the candidates in point_index order and keeps, per pixel cell, a winner and its depth stored as a
+// float; a later candidate takes the cell when (float)stored > depth.  That stored float is the running minimum of the
+// candidates' float depths (DESIGN.md section 4), so a cell's winner is its last candidate whose depth is below the minimum of
+// the float depths before it, or its first candidate.  Here: cell keys per candidate, a stable sort by cell, a segmented
+// exclusive min-scan of the float depths, a segmented "last flagged" reduction, and an order-preserving compaction.
+//
+// Candidate j is point_index p = j * skip of the candidate list: the last point of the voxel d_recent[p] (recent mode) or
+// rgb_points_vec[p].  One that passes the depth bounds and the projection gets the key of its cell (u, v), each offset by the
+// window's lower bound and packed as (u - u0) << bits_v | (v - v0); the others get `none`, which no cell produces.
+__global__ void k_proj_candidates(const Slot* slots, unsigned int mask, const float* __restrict__ blocks, int block_pts,
+                                  const unsigned long long* __restrict__ recent, const unsigned int* __restrict__ rgb_points, long long m,
+                                  int skip, CamConst c, double min_dis, double min_depth, double max_depth, int u0, int v0, int bits_v,
+                                  unsigned long long none, unsigned long long* key, unsigned int* ord, unsigned int* cand_id, double* depth,
+                                  float2* uv) {
+    const long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= m) return;
+    const long long p = j * skip;
+    unsigned id = kNoIndex;
+    if (recent) {                                                    // map[voxel].points.back() (:76-82)
+        const unsigned long long vk = recent[p];
+        short kx, ky, kz;
+        unpack_key(vk, kx, ky, kz);
+        const int slot = slot_find_rw(slots, mask, vk, kx, ky, kz);
+        if (slot >= 0 && slots[slot].count > 0) id = slots[slot].block * (unsigned)block_pts + slots[slot].count - 1u;
+    } else {
+        id = rgb_points[p];
+    }
+    unsigned long long k = none;
+    double d = 0.0;
+    if (id != kNoIndex) {
+        const unsigned blk = id / (unsigned)block_pts;
+        const float* bp = blocks + (size_t)blk * (4 * block_pts) + 4 * (size_t)(id - blk * (unsigned)block_pts);
+        const double px = (double)bp[0], py = (double)bp[1], pz = (double)bp[2];
+        d = camera_distance(c, px, py, pz);                         // :97
+        double u, v;
+        if (!(d > max_depth) && !(d < min_depth) && project_in_image(c, px, py, pz, u, v)) {   // :99-114
+            // :116-117: std::round (half away from zero), times minimum_dis, the double truncated to int
+            const int cu = (int)__dmul_rn(round(__ddiv_rn(u, min_dis)), min_dis);
+            const int cv = (int)__dmul_rn(round(__ddiv_rn(v, min_dis)), min_dis);
+            k = ((unsigned long long)(unsigned)(cu - u0) << bits_v) | (unsigned long long)(unsigned)(cv - v0);
+            uv[j] = make_float2(__double2float_rn(u), __double2float_rn(v));   // cv::Point2f(u_f, v_f)
+        }
+    }
+    key[j] = k;
+    ord[j] = (unsigned)j;
+    cand_id[j] = id;
+    depth[j] = d;
+}
+// the float depths in cell order: mask_depth holds (float)depth (:134)
+__global__ void k_proj_float_depths(const unsigned int* __restrict__ ord_sorted, const double* __restrict__ depth, long long m, float* fd) {
+    const long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (k < m) fd[k] = __double2float_rn(depth[ord_sorted[k]]);
+}
+// sorted position k takes its cell when its depth is below the minimum of the float depths before it in the cell (the float
+// widened, as `mask_depth[u][v] > depth` compares at :119); the first of a cell sees +inf.  Value: k if it takes the cell, else -1.
+__global__ void k_proj_takers(const unsigned long long* __restrict__ key_sorted, const unsigned int* __restrict__ ord_sorted,
+                              const double* __restrict__ depth, const float* __restrict__ prefix_min, long long m, unsigned long long none,
+                              int* taker) {
+    const long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= m) return;
+    taker[k] = (key_sorted[k] != none && depth[ord_sorted[k]] < (double)prefix_min[k]) ? (int)k : -1;
+}
+// the last taker of each cell is its winner: flag it in candidate order
+__global__ void k_proj_mark_winners(const int* __restrict__ last_taker, const int* n_cells_p, const unsigned int* __restrict__ ord_sorted,
+                                    unsigned char* win) {
+    const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= *n_cells_p) return;
+    const int k = last_taker[r];
+    if (k >= 0) win[ord_sorted[k]] = 1;
+}
+// the winners in point_index order (std::map order, :141-151): point id, the stored position, the float uv
+__global__ void k_proj_gather(const unsigned int* __restrict__ sel, long long n, const unsigned int* __restrict__ cand_id,
+                              const float2* __restrict__ cand_uv, const float* __restrict__ blocks, int block_pts, unsigned int* ids,
+                              float* xyz, float* uv) {
+    const long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= n) return;
+    const unsigned j = sel[k];
+    const unsigned id = cand_id[j];
+    if (ids) ids[k] = id;
+    if (xyz) {
+        const unsigned blk = id / (unsigned)block_pts;
+        const float* bp = blocks + (size_t)blk * (4 * block_pts) + 4 * (size_t)(id - blk * (unsigned)block_pts);
+        xyz[3 * k] = bp[0]; xyz[3 * k + 1] = bp[1]; xyz[3 * k + 2] = bp[2];
+    }
+    if (uv) { const float2 w = cand_uv[j]; uv[2 * k] = w.x; uv[2 * k + 1] = w.y; }
+}
+struct ProjMinF { __device__ __forceinline__ float operator()(float a, float b) const { return b < a ? b : a; } };
+struct ProjMaxI { __device__ __forceinline__ int operator()(int a, int b) const { return b > a ? b : a; } };
+struct ProjKeyEq { __device__ __forceinline__ bool operator()(unsigned long long a, unsigned long long b) const { return a == b; } };
+
+// ---- the tracker's per-point reads: gather by point id -------------------------------------------------------------------
+// an id is known when its block is one of the map's voxels and its index is below that voxel's count
+__global__ void k_color_check_ids(const unsigned int* __restrict__ ids, long long n, const float* __restrict__ blocks, int block_pts,
+                                  long long n_voxels, unsigned long long* n_bad) {
+    const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    bool bad = false;
+    if (t < n) {
+        const unsigned id = ids[t];
+        const unsigned blk = id / (unsigned)block_pts;
+        bad = (long long)blk >= n_voxels ||
+              id - blk * (unsigned)block_pts >= reinterpret_cast<const unsigned int*>(blocks + (size_t)blk * (4 * block_pts))[kMetaCount];
+    }
+    const unsigned b = __ballot_sync(0xffffffffu, bad);
+    if ((threadIdx.x & 31) == 0 && b) atomicAdd(n_bad, (unsigned long long)__popc(b));
+}
+// position, BGR state, N_rgb and covariance of each id (cov 0 before the first observation, like srl_color_map_download_state)
+__global__ void k_color_gather(const unsigned int* __restrict__ ids, long long n, const float* __restrict__ blocks, int block_pts,
+                               const ColorPoint* __restrict__ cpts, float* xyz, short* rgb, short* n_rgb, float* cov) {
+    const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= n) return;
+    const unsigned id = ids[t];
+    const unsigned blk = id / (unsigned)block_pts;
+    if (xyz) {
+        const float* bp = blocks + (size_t)blk * (4 * block_pts) + 4 * (size_t)(id - blk * (unsigned)block_pts);
+        xyz[3 * t] = bp[0]; xyz[3 * t + 1] = bp[1]; xyz[3 * t + 2] = bp[2];
+    }
+    const ColorPoint cp = cpts[id];
+    if (rgb) { rgb[3 * t] = cp.rgb[0]; rgb[3 * t + 1] = cp.rgb[1]; rgb[3 * t + 2] = cp.rgb[2]; }
+    if (n_rgb) n_rgb[t] = cp.n_rgb;
+    if (cov) for (int a = 0; a < 3; ++a) cov[3 * t + a] = cp.n_rgb > 0 ? cp.cov[a] : 0.f;
 }
 
 __global__ void k_gather_points(const double* __restrict__ xyz, const unsigned int* __restrict__ sel, int m, double* out) {
@@ -859,6 +992,8 @@ int srl_map_remove_far(srl_map* m, const double location[3], double distance, in
     if (!m || !location) return SRL_BAD_ARG;
     srl_ctx* ctx = m->ctx;
     if (int rc = check_lio_map(ctx, m)) return rc;
+    // the compaction moves blocks, which a colour map's per-point state, rgb list and point ids are indexed by
+    if (m->owner) return set_err(ctx, SRL_BAD_ARG, "srl_map_remove_far: the map is a colour map's voxel map (eviction would move its point ids)");
     SRL_CUDA(ctx, cudaSetDevice(ctx->device));
     if (n_removed) *n_removed = 0;
     const long long nv = (long long)m->n_voxels;
@@ -1703,6 +1838,198 @@ int srl_color_map_export(srl_color_map* cm, int32_t min_views, int32_t order, fl
         if (!rgb_dev && (rc = copy_to_host(ctx, rgb + 3 * off, stage_rgb, (size_t)k * 3)) != SRL_OK) return rc;
         off += (size_t)k;
     }
+    return SRL_OK;
+}
+
+}  // extern "C"
+
+// ---- selectPointsForProjection / the tracker's gather ------------------------------------------------------------------
+static CamConst camera_constants(const srl_camera* cam) {
+    CamConst c;
+    quat_to_rot(cam->q_camera_world, c.R);
+    for (int i = 0; i < 3; ++i) { c.t_cw[i] = cam->t_camera_world[i]; c.t_wc[i] = cam->t_world_camera[i]; }
+    c.fx = cam->fx; c.fy = cam->fy; c.cx = cam->cx; c.cy = cam->cy; c.fov = cam->fov_margin; c.cols = cam->cols; c.rows = cam->rows;
+    return c;
+}
+
+// The cell coordinates of one image axis: if2dPointsAvailable accepts fov * size + 1 <= x and ceil(x) < (1 - fov) * size, so
+// |x| <= a = max(|lo|, |hi|), and the cell std::round(x / d) * d lies within 2a + 1 of zero (it is 0, or |x / d| >= 1/2 and
+// |round(x / d)| <= 2 |x / d|).  The axis is offset by -b (b = ceil(2a) + 2) and takes `bits` bits, with 2^bits > 2b + 1 so that
+// an all-ones field never comes from a cell.  False when b does not fit an int or x / d can overflow.
+static bool cell_axis(double fov, int size, double min_dis, int& offset, int& bits) {
+    const double lo = fov * (double)size + 1.0, hi = (1.0 - fov) * (double)size;
+    const double a = std::max(std::fabs(lo), std::fabs(hi));
+    if (!(a < 1e9) || !(a / min_dis < 1e300)) return false;
+    const double b = std::ceil(2.0 * a) + 2.0;
+    if (!(b <= 2147483647.0)) return false;
+    offset = -(int)b;
+    const unsigned long long span = 2ull * (unsigned long long)b + 2ull;
+    bits = 0;
+    while ((1ull << bits) < span) ++bits;
+    return true;
+}
+
+extern "C" {
+
+int srl_color_map_select_for_projection(srl_color_map* cm, const srl_camera* cam, const srl_projection_params* prm, uint32_t* point_ids,
+                                        float* xyz, float* uv, size_t max_points, int64_t* n_out) {
+    if (!cm || !n_out) return SRL_BAD_ARG;
+    *n_out = 0;
+    srl_ctx* ctx = cm->ctx;
+    if (!cam || !prm) return set_err(ctx, SRL_BAD_ARG, "srl_color_map_select_for_projection: camera and parameters are required");
+    if (cam->cols < 2 || cam->rows < 2) return set_err(ctx, SRL_BAD_ARG, "srl_color_map_select_for_projection: the image needs cols >= 2 and rows >= 2");
+    if (!(std::isfinite(prm->minimum_dis) && prm->minimum_dis > 0))
+        return set_err(ctx, SRL_BAD_ARG, "srl_color_map_select_for_projection: minimum_dis must be finite and > 0");
+    if (prm->skip_step < 1) return set_err(ctx, SRL_BAD_ARG, "srl_color_map_select_for_projection: skip_step must be >= 1");
+    int u0 = 0, v0 = 0, bits_u = 0, bits_v = 0;
+    if (!std::isfinite(cam->fov_margin) || !cell_axis(cam->fov_margin, cam->cols, prm->minimum_dis, u0, bits_u) ||
+        !cell_axis(cam->fov_margin, cam->rows, prm->minimum_dis, v0, bits_v))
+        return set_err(ctx, SRL_BAD_ARG, "srl_color_map_select_for_projection: the cell coordinates of the FoV window do not fit an int");
+    const int end_bit = bits_u + bits_v;
+    const unsigned long long none = end_bit >= 64 ? ~0ull : (1ull << end_bit) - 1ull;
+    // :74-89: the last point of every recent voxel, or rgb_points_vec when use_all_points is set or the recent list is empty
+    const bool recent = !prm->use_all_points && cm->n_recent > 0;
+    const long long total = recent ? cm->n_recent : cm->n_rgb_points;
+    const long long m = (total + prm->skip_step - 1) / prm->skip_step;
+    if (m == 0) return SRL_OK;
+    if (m > 0x7fffffffLL) return set_err(ctx, SRL_BAD_ARG, "srl_color_map_select_for_projection: more than 2^31 - 1 candidates");
+    SRL_CUDA(ctx, cudaSetDevice(ctx->device));
+    cudaStream_t st = ctx->stream;
+    srl_map* vm = cm->vox;
+    const bool ids_dev = point_ids && is_device_ptr(point_ids), xyz_dev = xyz && is_device_ptr(xyz), uv_dev = uv && is_device_ptr(uv);
+    const int n = (int)m;
+    size_t tmp_sort = 0, tmp_scan = 0, tmp_red = 0, tmp_sel = 0;
+    cub::DeviceRadixSort::SortPairs(nullptr, tmp_sort, (unsigned long long*)nullptr, (unsigned long long*)nullptr, (unsigned int*)nullptr,
+                                    (unsigned int*)nullptr, n, 0, std::max(end_bit, 1), st);
+    cub::DeviceScan::ExclusiveScanByKey(nullptr, tmp_scan, (unsigned long long*)nullptr, (float*)nullptr, (float*)nullptr, ProjMinF(),
+                                        std::numeric_limits<float>::infinity(), n, ProjKeyEq(), st);
+    cub::DeviceReduce::ReduceByKey(nullptr, tmp_red, (unsigned long long*)nullptr, (unsigned long long*)nullptr, (int*)nullptr, (int*)nullptr,
+                                   (int*)nullptr, ProjMaxI(), n, st);
+    cub::DeviceSelect::Flagged(nullptr, tmp_sel, thrust::counting_iterator<unsigned int>(0), (unsigned char*)nullptr, (unsigned int*)nullptr,
+                               (int*)nullptr, n, st);
+    const size_t tmp_bytes = std::max(std::max(tmp_sort, tmp_scan), std::max(tmp_red, tmp_sel));
+    const size_t M = (size_t)m;
+    const size_t stage = (point_ids && !ids_dev ? align_up(M * 4) : 0) + (xyz && !xyz_dev ? align_up(M * 12) : 0) + (uv && !uv_dev ? align_up(M * 8) : 0);
+    const size_t need = 3 * align_up(M * 8) + 2 * align_up(M * 4) + align_up(M * 8) + align_up(M * 4) + align_up(M * 8) +
+                        3 * align_up(M * 4) + align_up(M * 4) + align_up(M) + align_up(M * 4) + 2 * 256 + align_up(tmp_bytes) + stage;
+    int rc = ensure_scratch(ctx, need);
+    if (rc != SRL_OK) return rc;
+    char* p = static_cast<char*>(ctx->d_scratch);
+    auto take = [&](size_t bytes) { char* r = p; p += align_up(bytes); return r; };
+    unsigned long long* key_a = reinterpret_cast<unsigned long long*>(take(M * 8));
+    unsigned long long* key_b = reinterpret_cast<unsigned long long*>(take(M * 8));
+    unsigned long long* cells = reinterpret_cast<unsigned long long*>(take(M * 8));
+    unsigned int* ord_a = reinterpret_cast<unsigned int*>(take(M * 4));
+    unsigned int* ord_b = reinterpret_cast<unsigned int*>(take(M * 4));
+    double* depth = reinterpret_cast<double*>(take(M * 8));
+    unsigned int* cand_id = reinterpret_cast<unsigned int*>(take(M * 4));
+    float2* cand_uv = reinterpret_cast<float2*>(take(M * 8));
+    float* fd = reinterpret_cast<float*>(take(M * 4));
+    float* pre = reinterpret_cast<float*>(take(M * 4));
+    int* taker = reinterpret_cast<int*>(take(M * 4));
+    int* last_taker = reinterpret_cast<int*>(take(M * 4));
+    unsigned char* win = reinterpret_cast<unsigned char*>(take(M));
+    unsigned int* sel = reinterpret_cast<unsigned int*>(take(M * 4));
+    int* d_ncells = reinterpret_cast<int*>(take(256));
+    int* d_nsel = reinterpret_cast<int*>(take(256));
+    void* d_tmp = take(tmp_bytes);
+    const int T = 256;
+    const unsigned gb = (unsigned)((m + T - 1) / T);
+    SRL_CUDA(ctx, cudaMemsetAsync(win, 0, M, st));
+    k_proj_candidates<<<gb, T, 0, st>>>(vm->d_slots, (unsigned)(vm->capacity - 1), vm->d_blocks, vm->block_pts, recent ? cm->d_recent : nullptr,
+                                        cm->d_rgb_points, m, prm->skip_step, camera_constants(cam), prm->minimum_dis, prm->minimum_depth,
+                                        prm->maximum_depth, u0, v0, bits_v, none, key_a, ord_a, cand_id, depth, cand_uv);
+    SRL_CUDA(ctx, cudaGetLastError());
+    size_t tb = tmp_bytes;
+    SRL_CUDA(ctx, cub::DeviceRadixSort::SortPairs(d_tmp, tb, key_a, key_b, ord_a, ord_b, n, 0, std::max(end_bit, 1), st));   // stable
+    k_proj_float_depths<<<gb, T, 0, st>>>(ord_b, depth, m, fd);
+    SRL_CUDA(ctx, cudaGetLastError());
+    tb = tmp_bytes;
+    SRL_CUDA(ctx, cub::DeviceScan::ExclusiveScanByKey(d_tmp, tb, key_b, fd, pre, ProjMinF(), std::numeric_limits<float>::infinity(), n, ProjKeyEq(), st));
+    k_proj_takers<<<gb, T, 0, st>>>(key_b, ord_b, depth, pre, m, none, taker);
+    SRL_CUDA(ctx, cudaGetLastError());
+    tb = tmp_bytes;
+    SRL_CUDA(ctx, cub::DeviceReduce::ReduceByKey(d_tmp, tb, key_b, cells, taker, last_taker, d_ncells, ProjMaxI(), n, st));
+    k_proj_mark_winners<<<gb, T, 0, st>>>(last_taker, d_ncells, ord_b, win);
+    SRL_CUDA(ctx, cudaGetLastError());
+    tb = tmp_bytes;
+    SRL_CUDA(ctx, cub::DeviceSelect::Flagged(d_tmp, tb, thrust::counting_iterator<unsigned int>(0), win, sel, d_nsel, n, st));
+    int k = 0;
+    SRL_CUDA(ctx, cudaMemcpyAsync(&k, d_nsel, sizeof(int), cudaMemcpyDeviceToHost, st));
+    SRL_CUDA(ctx, cudaStreamSynchronize(st));
+    ctx->launches += 8;
+    *n_out = k;
+    if ((!point_ids && !xyz && !uv) || k == 0) return SRL_OK;
+    if ((size_t)k > max_points) return set_err(ctx, SRL_BAD_ARG, "srl_color_map_select_for_projection: max_points is smaller than the number of points (count with NULL outputs first)");
+    unsigned int* o_ids = point_ids ? (ids_dev ? point_ids : reinterpret_cast<unsigned int*>(take(M * 4))) : nullptr;
+    float* o_xyz = xyz ? (xyz_dev ? xyz : reinterpret_cast<float*>(take(M * 12))) : nullptr;
+    float* o_uv = uv ? (uv_dev ? uv : reinterpret_cast<float*>(take(M * 8))) : nullptr;
+    k_proj_gather<<<(unsigned)((k + T - 1) / T), T, 0, st>>>(sel, k, cand_id, cand_uv, vm->d_blocks, vm->block_pts, o_ids, o_xyz, o_uv);
+    SRL_CUDA(ctx, cudaGetLastError());
+    ctx->launches += 1;
+    if (point_ids && !ids_dev && (rc = copy_to_host(ctx, point_ids, o_ids, (size_t)k * 4)) != SRL_OK) return rc;
+    if (xyz && !xyz_dev && (rc = copy_to_host(ctx, xyz, o_xyz, (size_t)k * 12)) != SRL_OK) return rc;
+    if (uv && !uv_dev && (rc = copy_to_host(ctx, uv, o_uv, (size_t)k * 8)) != SRL_OK) return rc;
+    SRL_CUDA(ctx, cudaStreamSynchronize(st));
+    return SRL_OK;
+}
+
+int srl_color_map_gather_points(srl_color_map* cm, const uint32_t* point_ids, size_t n, float* xyz, int16_t* rgb, int16_t* n_rgb, float* cov,
+                                int16_t* key_index) {
+    if (!cm) return SRL_BAD_ARG;
+    srl_ctx* ctx = cm->ctx;
+    if (n && !point_ids) return set_err(ctx, SRL_BAD_ARG, "srl_color_map_gather_points: point_ids is NULL");
+    if (n == 0) return SRL_OK;
+    if (n > 0x7fffffffULL) return set_err(ctx, SRL_BAD_ARG, "srl_color_map_gather_points: n must fit in int32");
+    SRL_CUDA(ctx, cudaSetDevice(ctx->device));
+    cudaStream_t st = ctx->stream;
+    srl_map* vm = cm->vox;
+    const bool in_dev = is_device_ptr(point_ids);
+    const bool xyz_dev = xyz && is_device_ptr(xyz), rgb_dev = rgb && is_device_ptr(rgb), nr_dev = n_rgb && is_device_ptr(n_rgb);
+    const bool cov_dev = cov && is_device_ptr(cov), ki_dev = key_index && is_device_ptr(key_index);
+    const size_t need = (in_dev ? 0 : align_up(n * 4)) + 256 + align_up(n * 12) + align_up(n * 6) + align_up(n * 2) + align_up(n * 12) + align_up(n * 8);
+    int rc = ensure_scratch(ctx, need);
+    if (rc != SRL_OK) return rc;
+    char* p = static_cast<char*>(ctx->d_scratch);
+    auto take = [&](size_t bytes) { char* r = p; p += align_up(bytes); return r; };
+    const unsigned int* ids = point_ids;
+    if (!in_dev) {
+        unsigned int* buf = reinterpret_cast<unsigned int*>(take(n * 4));
+        SRL_CUDA(ctx, cudaMemcpyAsync(buf, point_ids, n * 4, cudaMemcpyHostToDevice, st));
+        ids = buf;
+    }
+    unsigned long long* d_bad = reinterpret_cast<unsigned long long*>(take(256));
+    const int T = 256;
+    const unsigned gb = (unsigned)((n + T - 1) / T);
+    SRL_CUDA(ctx, cudaMemsetAsync(d_bad, 0, 8, st));
+    k_color_check_ids<<<gb, T, 0, st>>>(ids, (long long)n, vm->d_blocks, vm->block_pts, (long long)vm->n_voxels, d_bad);
+    SRL_CUDA(ctx, cudaGetLastError());
+    unsigned long long bad = 0;
+    SRL_CUDA(ctx, cudaMemcpyAsync(&bad, d_bad, 8, cudaMemcpyDeviceToHost, st));
+    SRL_CUDA(ctx, cudaStreamSynchronize(st));
+    ctx->launches += 1;
+    if (bad) return set_err(ctx, SRL_BAD_ARG, "srl_color_map_gather_points: " + std::to_string(bad) + " point id(s) name no stored point");
+    float* o_xyz = xyz ? (xyz_dev ? xyz : reinterpret_cast<float*>(take(n * 12))) : nullptr;
+    short* o_rgb = rgb ? (rgb_dev ? rgb : reinterpret_cast<short*>(take(n * 6))) : nullptr;
+    short* o_nr = n_rgb ? (nr_dev ? n_rgb : reinterpret_cast<short*>(take(n * 2))) : nullptr;
+    float* o_cov = cov ? (cov_dev ? cov : reinterpret_cast<float*>(take(n * 12))) : nullptr;
+    short* o_ki = key_index ? (ki_dev ? key_index : reinterpret_cast<short*>(take(n * 8))) : nullptr;
+    if (o_xyz || o_rgb || o_nr || o_cov) {
+        k_color_gather<<<gb, T, 0, st>>>(ids, (long long)n, vm->d_blocks, vm->block_pts, cm->d_cpts, o_xyz, o_rgb, o_nr, o_cov);
+        SRL_CUDA(ctx, cudaGetLastError());
+        ctx->launches += 1;
+    }
+    if (o_ki) {
+        k_color_rgb_ids<<<gb, T, 0, st>>>(ids, (long long)n, vm->d_blocks, vm->block_pts, o_ki);
+        SRL_CUDA(ctx, cudaGetLastError());
+        ctx->launches += 1;
+    }
+    if (xyz && !xyz_dev && (rc = copy_to_host(ctx, xyz, o_xyz, n * 12)) != SRL_OK) return rc;
+    if (rgb && !rgb_dev && (rc = copy_to_host(ctx, rgb, o_rgb, n * 6)) != SRL_OK) return rc;
+    if (n_rgb && !nr_dev && (rc = copy_to_host(ctx, n_rgb, o_nr, n * 2)) != SRL_OK) return rc;
+    if (cov && !cov_dev && (rc = copy_to_host(ctx, cov, o_cov, n * 12)) != SRL_OK) return rc;
+    if (key_index && !ki_dev && (rc = copy_to_host(ctx, key_index, o_ki, n * 8)) != SRL_OK) return rc;
+    SRL_CUDA(ctx, cudaStreamSynchronize(st));
     return SRL_OK;
 }
 

@@ -11,6 +11,7 @@ Names and argument meaning follow the reference so the parity tests read like it
   eskfEstimator (state + observe)       src/eskfEstimator.cpp           -> EskfEstimator
   addPointToPcl / publishCLoudWorld     src/lioOptimization.cpp:432,552 -> LioOptimization.addPointsToMapPublished
   pubColorPoints / saveColorPoints      src/lioOptimization.cpp:1210,1386 -> ColorVoxelMap.pubColorPoints / saveColorPoints
+  rgbMapTracker::selectPointsForProjection src/rgbMapTracker.cpp:45     -> ColorVoxelMap.selectPointsForProjection / gatherPoints
 
 Error behaviour: optimizeSummary.success=false <-> OptimizeSummary.success False (SRL_TOO_FEW_RESIDUALS);
 the reference's `throw std::runtime_error("error")` on NaN planarity <-> RuntimeError; everything else raises
@@ -319,6 +320,62 @@ class ColorVoxelMap:
         if path is not None:
             write_pcd_xyzrgb(path, xyz, rgb)
         return xyz, rgb
+
+    def selectPointsForProjection(self, camera: "capi.Camera", minimum_dis: float = 5.0, skip_step: int = 1, use_all_points: bool = False,
+                                  minimum_depth: float = 0.1, maximum_depth: float = 200.0, out=None):
+        """rgbMapTracker::selectPointsForProjection (src/rgbMapTracker.cpp:45-152, srl_color_map_select_for_projection):
+        (ids, xyz, uv) of the selected points in point_index order — uint32 point ids, (n, 3) float32 positions, (n, 2) float32
+        cv::Point2f(u_f, v_f).  refreshPointsForProjection is minimum_dis=10 from a camera with fov_margin -0.4; the first image
+        uses minimum_dis = track_windows_size / image_scale_factor.  out = (ids, xyz, uv) buffers (numpy arrays or torch tensors,
+        host or CUDA; any may be None) receive the points and their first n rows are returned; without it numpy arrays are made."""
+        prm = capi.ProjectionParams(float(minimum_dis), int(skip_step), 1 if use_all_points else 0, float(minimum_depth), float(maximum_depth))
+        n = C.c_int64(0)
+        if out is None:
+            st = self.stats()
+            total = st["rgb_points"] if use_all_points or st["recent"] == 0 else st["recent"]
+            bound = (total + max(int(skip_step), 1) - 1) // max(int(skip_step), 1)
+            out = (np.empty(bound, np.uint32), np.empty((bound, 3), np.float32), np.empty((bound, 2), np.float32))
+        ids, xyz, uv = out
+        addrs, caps = [], []
+        for a, dt, w in ((ids, np.uint32, 1), (xyz, np.float32, 3), (uv, np.float32, 2)):
+            if a is None:
+                addrs.append(None)
+                continue
+            if _is_tensor(a) and str(a.dtype) == "torch.int32" and dt == np.uint32:
+                p, rows = a.data_ptr(), a.numel()          # torch has no uint32 of its own: int32 holds the ids' bits
+            else:
+                p, rows = _addr(a, dt, w)
+            addrs.append(C.c_void_p(p))
+            caps.append(rows)
+        _check(self.ctx.h, lib().srl_color_map_select_for_projection(self.h, C.byref(camera), C.byref(prm), addrs[0], addrs[1], addrs[2],
+                                                                      min(caps) if caps else 0, C.byref(n)))
+        k = n.value
+        return tuple(None if a is None else a[:k] for a in (ids, xyz, uv))
+
+    def countPointsForProjection(self, camera: "capi.Camera", minimum_dis: float = 5.0, skip_step: int = 1, use_all_points: bool = False,
+                                 minimum_depth: float = 0.1, maximum_depth: float = 200.0) -> int:
+        """How many points selectPointsForProjection with the same arguments returns."""
+        prm = capi.ProjectionParams(float(minimum_dis), int(skip_step), 1 if use_all_points else 0, float(minimum_depth), float(maximum_depth))
+        n = C.c_int64(0)
+        _check(self.ctx.h, lib().srl_color_map_select_for_projection(self.h, C.byref(camera), C.byref(prm), None, None, None, 0, C.byref(n)))
+        return n.value
+
+    def gatherPoints(self, ids) -> dict:
+        """srl_color_map_gather_points: the state of each point id as numpy arrays — xyz (n, 3) float32, rgb (n, 3) int16 (the BGR
+        state), n_rgb (n,) int16, cov (n, 3) float32, key_index (n, 4) int16 (voxel key, index in block).  ids: a uint32 numpy array
+        or a torch tensor (host or CUDA; int32 holds the ids' bits).  An id that names no stored point raises SrlError."""
+        if _is_tensor(ids):
+            p, n = ids.data_ptr(), ids.numel()
+            if ids.element_size() != 4 or not ids.is_contiguous():
+                raise TypeError("expected a contiguous 32-bit tensor of point ids")
+        else:
+            ids = np.ascontiguousarray(ids, np.uint32).reshape(-1)
+            p, n = ids.ctypes.data, ids.size
+        out = dict(xyz=np.empty((n, 3), np.float32), rgb=np.empty((n, 3), np.int16), n_rgb=np.empty(n, np.int16),
+                   cov=np.empty((n, 3), np.float32), key_index=np.empty((n, 4), np.int16))
+        _check(self.ctx.h, lib().srl_color_map_gather_points(self.h, C.c_void_p(p), n, *[ptr(out[k]) for k in ("xyz", "rgb", "n_rgb", "cov",
+                                                                                                                "key_index")]))
+        return out
 
     def download(self) -> dict:
         """voxel contents + colour state (block order) + the two lists."""
