@@ -16,6 +16,8 @@
  *   - every function returns an srl_status; srl_last_error(ctx) gives the text.
  *   - there is NO CPU fallback: without a CUDA device every compute entry point returns
  *     SRL_CUDA_ERROR.
+ *   - "host or device, detected per pointer": device and managed (cudaMallocManaged) memory
+ *     is used in place; page-locked and pageable host memory is staged through device scratch.
  */
 #ifndef SRLIVO_B200_H
 #define SRLIVO_B200_H
@@ -179,7 +181,8 @@ int srl_map_remove_far(srl_map* map, const double location[3], double distance, 
 /* mirror of a host voxelHashMap: keys n*3, counts n, xyz n*cap*3 (block order = voxelBlock::points order) */
 int srl_map_upload(srl_map* map, const int16_t* keys, const int32_t* counts, const float* xyz, size_t n_voxels);
 int srl_map_download(srl_map* map, int16_t* keys, int32_t* counts, float* xyz, size_t max_voxels, int64_t* n_voxels);
-/* addPointsToMap, sweep order preserved per voxel. xyz_world: host (or device if *_device) n*3 doubles */
+/* addPointsToMap, sweep order preserved per voxel. xyz_world: n*3 doubles, host or device, detected per pointer (both
+ * names run the same code) */
 int srl_map_insert(srl_map* map, const double* xyz_world, size_t n, double min_distance_points,
                    int32_t min_num_points, int64_t* n_added);
 int srl_map_insert_device(srl_map* map, const double* d_xyz_world, size_t n, double min_distance_points,

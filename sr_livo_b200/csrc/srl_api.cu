@@ -37,6 +37,30 @@ int ensure_pinned(srl_ctx* ctx, size_t bytes) {
     ctx->pinned_bytes = want;
     return SRL_OK;
 }
+MemKind mem_kind(const void* p) {
+    cudaPointerAttributes attr;
+    if (cudaPointerGetAttributes(&attr, p) != cudaSuccess) { cudaGetLastError(); return MemKind::Pageable; }
+    if (attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged) return MemKind::Device;
+    return attr.type == cudaMemoryTypeHost ? MemKind::Pinned : MemKind::Pageable;
+}
+int copy_to_host(srl_ctx* ctx, void* dst, const void* d_src, size_t bytes) {
+    if (bytes == 0) return SRL_OK;
+    if (mem_kind(dst) == MemKind::Pinned) {
+        SRL_CUDA(ctx, cudaMemcpyAsync(dst, d_src, bytes, cudaMemcpyDeviceToHost, ctx->stream));
+        SRL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        return SRL_OK;
+    }
+    const size_t chunk = std::min(bytes, size_t(64) << 20);   // no host temporary the size of the output
+    int rc = ensure_pinned(ctx, chunk);
+    if (rc != SRL_OK) return rc;
+    for (size_t off = 0; off < bytes; off += chunk) {
+        const size_t len = std::min(chunk, bytes - off);
+        SRL_CUDA(ctx, cudaMemcpyAsync(ctx->h_pinned, static_cast<const char*>(d_src) + off, len, cudaMemcpyDeviceToHost, ctx->stream));
+        SRL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        std::memcpy(static_cast<char*>(dst) + off, ctx->h_pinned, len);
+    }
+    return SRL_OK;
+}
 
 // fold a finished event pair into the running totals.  Pairs alternate between passes and the pair of the PREVIOUS pass is
 // collected when the next one starts: its last kernel (the fallback launch, which on one GPU is off the host's critical
@@ -497,10 +521,8 @@ int srl_sweep_upload(srl_sweep* s, const double* raw_xyz, size_t n) {
     SRL_CUDA(ctx, cudaSetDevice(ctx->device));
     if (n) {
         // pinned caller memory goes straight to the DMA engine; pageable memory is staged through a pinned buffer
-        cudaPointerAttributes attr;
-        const bool pinned = cudaPointerGetAttributes(&attr, raw_xyz) == cudaSuccess && attr.type == cudaMemoryTypeHost;
+        const bool pinned = mem_kind(raw_xyz) == MemKind::Pinned;
         if (!pinned) {
-            cudaGetLastError();
             int rc = ensure_pinned(ctx, n * 3 * sizeof(double));
             if (rc != SRL_OK) return rc;
             std::memcpy(ctx->h_pinned, raw_xyz, n * 3 * sizeof(double));

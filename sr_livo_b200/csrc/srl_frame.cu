@@ -178,13 +178,6 @@ __global__ void k_frame_gather(const unsigned int* __restrict__ c, long long m, 
 }
 
 inline unsigned grid_of(long long n, int T = 256) { return (unsigned)((n + T - 1) / T); }
-inline size_t al256(size_t x) { return (x + 255) / 256 * 256; }
-
-bool is_device_ptr(const void* p) {
-    cudaPointerAttributes a;
-    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
-    return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
-}
 
 }  // namespace
 
@@ -328,21 +321,14 @@ static int shuffle_indices(srl_ctx* ctx, WordStream& ws, ShuffleWork& w, const u
     return SRL_OK;
 }
 
-static size_t shuffle_cub_bytes(size_t cap) {
-    size_t b = 0;
-    cub::DeviceRadixSort::SortKeys(nullptr, b, (unsigned long long*)nullptr, (unsigned long long*)nullptr, (int)std::max<size_t>(cap, 1), 0, 64);
-    return b;
+// the work buffers of one shuffle over up to `cap` elements (w.cub_bytes set by the caller)
+static void shuffle_work_layout(ShuffleWork& w, Carve& c, size_t cap) {
+    w.j = c.take<unsigned int>(cap + 1);
+    w.keys = c.take<unsigned long long>(cap + 1);
+    w.keys_sorted = c.take<unsigned long long>(cap + 1);
+    w.first_rej = c.take<unsigned long long>(1);
+    w.cub_tmp = c.take<char>(w.cub_bytes);
 }
-static void shuffle_work_take(ShuffleWork& w, char*& p, size_t cap) {
-    auto take = [&](size_t bytes) { char* r = p; p += al256(bytes); return r; };
-    w.j = reinterpret_cast<unsigned int*>(take(cap * 4 + 4));
-    w.keys = reinterpret_cast<unsigned long long*>(take(cap * 8 + 8));
-    w.keys_sorted = reinterpret_cast<unsigned long long*>(take(cap * 8 + 8));
-    w.first_rej = reinterpret_cast<unsigned long long*>(take(8));
-    w.cub_bytes = shuffle_cub_bytes(cap);
-    w.cub_tmp = take(w.cub_bytes);
-}
-static size_t shuffle_work_bytes(size_t cap) { return al256(cap * 4 + 4) + 2 * al256(cap * 8 + 8) + al256(8) + al256(shuffle_cub_bytes(cap)); }
 
 }  // namespace srl
 
@@ -369,39 +355,42 @@ struct srl_cloud_frame {
     ShuffleWork sw;
 };
 
+// the frame's arrays, its selection's and its shuffles' work buffers for up to `cap` points (sel_bytes and sw.cub_bytes set)
+static void frame_layout(srl_cloud_frame& f, Carve& c, size_t cap) {
+    f.raw = c.take<double>(cap * 3); f.point = c.take<double>(cap * 3); f.imu = c.take<double>(cap * 3);
+    f.rel = c.take<double>(cap); f.alpha = c.take<double>(cap); f.ts = c.take<double>(cap);
+    f.src = c.take<int>(cap);
+    f.raw1 = c.take<double>(cap * 3); f.imu1 = c.take<double>(cap * 3);
+    f.ts1 = c.take<double>(cap); f.rel1 = c.take<double>(cap); f.alpha1 = c.take<double>(cap);
+    f.src1 = c.take<unsigned int>(cap);
+    f.in_raw = c.take<double>(cap * 3); f.pt = c.take<double>(cap * 3);
+    f.in_ts = c.take<double>(cap);
+    f.keep = c.take<unsigned char>(cap);
+    f.ca = c.take<unsigned int>(cap); f.cb = c.take<unsigned int>(cap); f.sel = c.take<unsigned int>(cap);
+    f.d_count = c.take<int>(1);
+    f.sel_tmp = c.take<char>(f.sel_bytes);
+    shuffle_work_layout(f.sw, c, cap);
+}
+
 static int frame_reserve(srl_cloud_frame* f, size_t cap) {
     srl_ctx* ctx = f->ctx;
     if (cap <= f->capacity && f->mem) return SRL_OK;
     cap = std::max(cap, f->capacity * 2);
     cap = std::max<size_t>(cap, 1024);
-    size_t sel = 0;
-    cub::DeviceSelect::Flagged(nullptr, sel, (unsigned int*)nullptr, (unsigned char*)nullptr, (unsigned int*)nullptr, (int*)nullptr, (int)cap);
-    const size_t v3 = al256(cap * 24), v1 = al256(cap * 8), u1 = al256(cap * 4);
-    const size_t bytes = 3 * v3 + 3 * v1 + u1 + 2 * v3 + 3 * v1 + u1 + 2 * v3 + v1 + al256(cap) + 3 * u1 + 256 + al256(sel) +
-                         shuffle_work_bytes(cap);
-    void* mem = nullptr;
+    srl_cloud_frame g;   // the grown frame, laid out first to measure it
+    g.ctx = ctx;
+    g.capacity = cap;
+    cub::DeviceSelect::Flagged(nullptr, g.sel_bytes, (unsigned int*)nullptr, (unsigned char*)nullptr, (unsigned int*)nullptr, (int*)nullptr, (int)cap);
+    cub::DeviceRadixSort::SortKeys(nullptr, g.sw.cub_bytes, (unsigned long long*)nullptr, (unsigned long long*)nullptr, (int)cap, 0, 64);
+    Carve probe;
+    frame_layout(g, probe, cap);
     SRL_CUDA(ctx, cudaSetDevice(ctx->device));
     SRL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    SRL_CUDA(ctx, cudaMalloc(&mem, bytes));
+    SRL_CUDA(ctx, cudaMalloc(&g.mem, probe.used));
     if (f->mem) cudaFree(f->mem);
-    f->mem = mem;
-    f->capacity = cap;
-    f->n = 0;
-    char* p = static_cast<char*>(mem);
-    auto take = [&](size_t b) { char* r = p; p += al256(b); return r; };
-    f->raw = (double*)take(cap * 24); f->point = (double*)take(cap * 24); f->imu = (double*)take(cap * 24);
-    f->rel = (double*)take(cap * 8); f->alpha = (double*)take(cap * 8); f->ts = (double*)take(cap * 8);
-    f->src = (int*)take(cap * 4);
-    f->raw1 = (double*)take(cap * 24); f->imu1 = (double*)take(cap * 24);
-    f->ts1 = (double*)take(cap * 8); f->rel1 = (double*)take(cap * 8); f->alpha1 = (double*)take(cap * 8);
-    f->src1 = (unsigned int*)take(cap * 4);
-    f->in_raw = (double*)take(cap * 24); f->pt = (double*)take(cap * 24);
-    f->in_ts = (double*)take(cap * 8);
-    f->keep = (unsigned char*)take(cap);
-    f->ca = (unsigned int*)take(cap * 4); f->cb = (unsigned int*)take(cap * 4); f->sel = (unsigned int*)take(cap * 4);
-    f->d_count = (int*)take(256);
-    f->sel_bytes = sel; f->sel_tmp = take(sel);
-    shuffle_work_take(f->sw, p, cap);
+    Carve c{static_cast<char*>(g.mem), 0};
+    frame_layout(g, c, cap);
+    *f = g;
     return SRL_OK;
 }
 
@@ -492,8 +481,8 @@ int srl_build_frame(srl_ctx* ctx, const double* raw_xyz, const double* timestamp
 
     // 1. makePointTimestamp (:786-819)
     const double* raw = raw_xyz; const double* ts = timestamp;
-    if (n && !is_device_ptr(raw_xyz)) { SRL_CUDA(ctx, cudaMemcpyAsync(f->in_raw, raw_xyz, n * 24, cudaMemcpyHostToDevice, st)); raw = f->in_raw; }
-    if (n && !is_device_ptr(timestamp)) { SRL_CUDA(ctx, cudaMemcpyAsync(f->in_ts, timestamp, n * 8, cudaMemcpyHostToDevice, st)); ts = f->in_ts; }
+    if (n && mem_kind(raw_xyz) != MemKind::Device) { SRL_CUDA(ctx, cudaMemcpyAsync(f->in_raw, raw_xyz, n * 24, cudaMemcpyHostToDevice, st)); raw = f->in_raw; }
+    if (n && mem_kind(timestamp) != MemKind::Device) { SRL_CUDA(ctx, cudaMemcpyAsync(f->in_ts, timestamp, n * 8, cudaMemcpyHostToDevice, st)); ts = f->in_ts; }
     const double delta_t = time_end - time_frame_begin;
     long long n1 = (long long)n;
     if (n && prm->point_time_enable) {

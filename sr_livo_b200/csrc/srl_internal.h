@@ -468,6 +468,54 @@ int ensure_pinned(srl_ctx* ctx, size_t bytes);
 void timing_collect(srl_ctx* ctx);
 // SRL_OK for a map laid out with kBlockCap points per block (the layout every LIO kernel addresses), else SRL_BAD_ARG
 int check_lio_map(srl_ctx* ctx, const srl_map* m);
+
+// Where a caller's buffer lives.  Device covers device and managed memory: a kernel can use it in place.  Pinned is
+// page-locked host memory, which the copy engine reads and writes directly.
+enum class MemKind { Pageable, Pinned, Device };
+MemKind mem_kind(const void* p);
+// device -> host: a pinned destination is written by the copy engine directly, any other through the ctx's pinned staging
+// buffer in chunks of at most 64 MB.  Returns when the bytes are in dst.
+int copy_to_host(srl_ctx* ctx, void* dst, const void* d_src, size_t bytes);
+
+inline size_t align_up(size_t x, size_t a = 256) { return (x + a - 1) / a * a; }
+
+// Bump allocation of 256-byte-aligned arrays from one region; with base == nullptr it only measures (take returns null).
+struct Carve {
+    char* base = nullptr;
+    size_t used = 0;
+    template <class T> T* take(size_t count) {
+        T* p = base ? reinterpret_cast<T*>(base + used) : nullptr;
+        used += align_up(count * sizeof(T));
+        return p;
+    }
+};
+// An entry point's scratch: layout(Carve&) runs once to measure, the ctx scratch grows to that size, and layout runs again
+// over it.  The layout must take the same arrays both times.
+template <class Layout> int carve_scratch(srl_ctx* ctx, Layout&& layout) {
+    Carve probe;
+    layout(probe);
+    const int rc = ensure_scratch(ctx, probe.used);
+    if (rc != SRL_OK) return rc;
+    Carve c{static_cast<char*>(ctx->d_scratch), 0};
+    layout(c);
+    return SRL_OK;
+}
+
+// A caller's buffer of T, host or device (detected per pointer), as the kernels see it: the buffer itself when it is on the
+// device, else scratch placed by place().  upload() fills the scratch from an input; hand_back() returns an output.  A null
+// buffer stays null.
+template <class T> struct Staged {
+    T* user;
+    bool dev;
+    T* d = nullptr;
+    explicit Staged(T* p) : user(p), dev(p && mem_kind(p) == MemKind::Device) {}
+    void place(Carve& c, size_t count) { d = (dev || !user) ? user : c.take<T>(count); }
+    int upload(srl_ctx* ctx, size_t count) const;
+    // elements [0, count) of the scratch into the caller's buffer at element `offset`
+    int hand_back(srl_ctx* ctx, size_t count, size_t offset = 0) const {
+        return (dev || !user) ? SRL_OK : copy_to_host(ctx, user + offset, d, count * sizeof(T));
+    }
+};
 }  // namespace srl
 
 #define SRL_CUDA(ctx, call)                                             \
@@ -475,3 +523,9 @@ int check_lio_map(srl_ctx* ctx, const srl_map* m);
         cudaError_t e__ = (call);                                       \
         if (e__ != cudaSuccess) return srl::cuda_fail((ctx), e__, #call); \
     } while (0)
+
+template <class T> int srl::Staged<T>::upload(srl_ctx* ctx, size_t count) const {
+    if (!dev && user && count)
+        SRL_CUDA(ctx, cudaMemcpyAsync(const_cast<void*>(static_cast<const void*>(d)), user, count * sizeof(T), cudaMemcpyHostToDevice, ctx->stream));
+    return SRL_OK;
+}

@@ -660,38 +660,6 @@ __global__ void k_color_export_gather(const unsigned int* __restrict__ rgb_point
     rgb[3 * k] = (unsigned char)(cp.rgb[2] & 0xff); rgb[3 * k + 1] = (unsigned char)(cp.rgb[1] & 0xff); rgb[3 * k + 2] = (unsigned char)(cp.rgb[0] & 0xff);
 }
 
-static inline size_t align_up(size_t x, size_t a = 256) { return (x + a - 1) / a * a; }
-
-static bool is_device_ptr(const void* p) {
-    cudaPointerAttributes attr;
-    const bool dev = cudaPointerGetAttributes(&attr, p) == cudaSuccess && attr.type == cudaMemoryTypeDevice;
-    if (!dev) cudaGetLastError();
-    return dev;
-}
-// device -> host output: page-locked destinations are written by the copy engine directly, pageable ones through the ctx's
-// pinned staging buffer in chunks of at most 64 MB (no host temporary the size of the output)
-static int copy_to_host(srl_ctx* ctx, void* dst, const void* d_src, size_t bytes) {
-    if (bytes == 0) return SRL_OK;
-    cudaPointerAttributes attr;
-    const bool pinned = cudaPointerGetAttributes(&attr, dst) == cudaSuccess && attr.type == cudaMemoryTypeHost;
-    if (!pinned) cudaGetLastError();
-    if (pinned) {
-        SRL_CUDA(ctx, cudaMemcpyAsync(dst, d_src, bytes, cudaMemcpyDeviceToHost, ctx->stream));
-        SRL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        return SRL_OK;
-    }
-    const size_t chunk = std::min(bytes, size_t(64) << 20);
-    int rc = ensure_pinned(ctx, chunk);
-    if (rc != SRL_OK) return rc;
-    for (size_t off = 0; off < bytes; off += chunk) {
-        const size_t len = std::min(chunk, bytes - off);
-        SRL_CUDA(ctx, cudaMemcpyAsync(ctx->h_pinned, static_cast<const char*>(d_src) + off, len, cudaMemcpyDeviceToHost, ctx->stream));
-        SRL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        std::memcpy(static_cast<char*>(dst) + off, ctx->h_pinned, len);
-    }
-    return SRL_OK;
-}
-
 // ---- growth: arrays on CUDA VMM, slot tables rebuilt -----------------------------------------------------------------
 // The driver's VMM calls come through the runtime's entry-point query, so the library does not link libcuda.
 struct VmmApi {
@@ -816,6 +784,14 @@ int srl::check_lio_map(srl_ctx* ctx, const srl_map* m) {
 }
 
 // ---- N4: colour map host side ---------------------------------------------------------------------------------------
+// the renderer's and the selection's projection constants of a camera
+static CamConst camera_constants(const srl_camera* cam) {
+    CamConst c;
+    quat_to_rot(cam->q_camera_world, c.R);
+    for (int i = 0; i < 3; ++i) { c.t_cw[i] = cam->t_camera_world[i]; c.t_wc[i] = cam->t_world_camera[i]; }
+    c.fx = cam->fx; c.fy = cam->fy; c.cx = cam->cx; c.cy = cam->cy; c.fov = cam->fov_margin; c.cols = cam->cols; c.rows = cam->rows;
+    return c;
+}
 struct srl_color_map {
     srl_ctx* ctx = nullptr;
     srl_map* vox = nullptr;                 // color_voxel_map (include/lioOptimization.h:275)
@@ -881,6 +857,79 @@ static int map_grow(srl_map* m, size_t need) {
     if ((rc = vm_grow(m->ctx, m->blocks_mem, nv * 4 * (size_t)m->block_pts * sizeof(float))) != SRL_OK) return rc;
     if ((rc = table_grow(m->ctx, m->d_slots, m->capacity, nv)) != SRL_OK) return rc;
     m->committed_voxels = nv;
+    return SRL_OK;
+}
+
+// the total of an exclusive scan over n > 0 flags: its last rank plus the last flag
+static int scan_total(srl_ctx* ctx, const unsigned* flags, const unsigned* rank, long long n, long long* total) {
+    unsigned last_rank = 0, last_flag = 0;
+    SRL_CUDA(ctx, cudaMemcpyAsync(&last_rank, rank + (n - 1), sizeof(unsigned), cudaMemcpyDeviceToHost, ctx->stream));
+    SRL_CUDA(ctx, cudaMemcpyAsync(&last_flag, flags + (n - 1), sizeof(unsigned), cudaMemcpyDeviceToHost, ctx->stream));
+    SRL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    *total = (long long)last_rank + last_flag;
+    return SRL_OK;
+}
+
+// The voxel segments of a batch of points: their keys sorted stably (sweep order inside a voxel) with the points' indices,
+// the start of every run of one valid key, and per run its slot and whether its voxel is new, with the rank of the new ones.
+struct Segments {
+    unsigned long long *keys, *keys_sorted;
+    unsigned *idx, *idx_sorted;
+    unsigned char* flags;
+    unsigned *start, *is_new, *new_rank;
+    int* slot;
+    int* d_count;
+    void* tmp;          // CUB temporary storage of segment_tmp_bytes (or more)
+    size_t tmp_bytes;
+    void place(Carve& c, size_t n, size_t tmp_size) {
+        keys = c.take<unsigned long long>(n); keys_sorted = c.take<unsigned long long>(n);
+        idx = c.take<unsigned>(n); idx_sorted = c.take<unsigned>(n);
+        flags = c.take<unsigned char>(n);
+        start = c.take<unsigned>(n); slot = c.take<int>(n); is_new = c.take<unsigned>(n); new_rank = c.take<unsigned>(n);
+        d_count = c.take<int>(1);
+        tmp = c.take<char>(tmp_size); tmp_bytes = tmp_size;
+    }
+};
+// CUB temporary storage for the sort, the selection and the scan of n keys (also every other selection or scan over n)
+static size_t segment_tmp_bytes(int n, cudaStream_t st) {
+    size_t tmp_sort = 0, tmp_sel = 0, tmp_scan = 0;
+    cub::DeviceRadixSort::SortPairs(nullptr, tmp_sort, (unsigned long long*)nullptr, (unsigned long long*)nullptr, (unsigned*)nullptr,
+                                    (unsigned*)nullptr, n, 0, 50, st);
+    cub::DeviceSelect::Flagged(nullptr, tmp_sel, thrust::counting_iterator<unsigned int>(0), (unsigned char*)nullptr, (unsigned*)nullptr,
+                               (int*)nullptr, n, st);
+    cub::DeviceScan::ExclusiveSum(nullptr, tmp_scan, (unsigned*)nullptr, (unsigned*)nullptr, n, st);
+    return std::max(tmp_sort, std::max(tmp_sel, tmp_scan));
+}
+// sort the n keys in s.keys (with s.idx) and find the starts of their runs; *n_seg = the number of runs
+static int segment_keys(srl_ctx* ctx, const Segments& s, int n, int* n_seg) {
+    cudaStream_t st = ctx->stream;
+    const int T = 256;
+    size_t tb = s.tmp_bytes;
+    cub::DeviceRadixSort::SortPairs(s.tmp, tb, s.keys, s.keys_sorted, s.idx, s.idx_sorted, n, 0, 50, st);
+    k_seg_flags<<<(unsigned)((n + T - 1) / T), T, 0, st>>>(s.keys_sorted, (long long)n, s.flags);
+    tb = s.tmp_bytes;
+    cub::DeviceSelect::Flagged(s.tmp, tb, thrust::counting_iterator<unsigned int>(0), s.flags, s.start, s.d_count, n, st);
+    *n_seg = 0;
+    SRL_CUDA(ctx, cudaMemcpyAsync(n_seg, s.d_count, sizeof(int), cudaMemcpyDeviceToHost, st));
+    SRL_CUDA(ctx, cudaStreamSynchronize(st));
+    ctx->launches += 3;
+    return SRL_OK;
+}
+// the voxels of n_seg > 0 runs: the map grows for up to n_seg new ones (before the lookup, which stores slot indices), each
+// run finds its slot (allow_new: an absent voxel is new), the new ones are ranked and counted.  SRL_MAP_FULL past max_voxels.
+static int count_new_voxels(srl_map* m, const Segments& s, int n_seg, bool allow_new, const char* who, long long* total_new) {
+    srl_ctx* ctx = m->ctx;
+    int rc = map_grow(m, (size_t)m->n_voxels + (size_t)n_seg);
+    if (rc != SRL_OK) return rc;
+    const int T = 256;
+    k_seg_lookup<<<(unsigned)((n_seg + T - 1) / T), T, 0, ctx->stream>>>(m->d_slots, (unsigned)(m->capacity - 1), s.keys_sorted, s.start,
+                                                                       s.d_count, allow_new ? 1 : 0, s.slot, s.is_new);
+    size_t tb = s.tmp_bytes;
+    cub::DeviceScan::ExclusiveSum(s.tmp, tb, s.is_new, s.new_rank, n_seg, ctx->stream);
+    if ((rc = scan_total(ctx, s.is_new, s.new_rank, n_seg, total_new)) != SRL_OK) return rc;
+    ctx->launches += 2;
+    if ((size_t)(m->n_voxels + *total_new) > m->max_voxels)
+        return set_err(ctx, SRL_MAP_FULL, std::string(who) + ": voxel pool exhausted (raise max_voxels)");
     return SRL_OK;
 }
 
@@ -998,27 +1047,23 @@ int srl_map_remove_far(srl_map* m, const double location[3], double distance, in
     if (n_removed) *n_removed = 0;
     const long long nv = (long long)m->n_voxels;
     if (nv == 0) return SRL_OK;
-    auto al = [](size_t x) { return (x + 255) / 256 * 256; };
     size_t tmp = 0;
     cub::DeviceScan::ExclusiveSum(nullptr, tmp, (unsigned*)nullptr, (unsigned*)nullptr, (int)nv, ctx->stream);
-    // worst case every block survives: the compacted copy needs a pool-sized scratch
-    const size_t need = 2 * al((size_t)nv * 4) + al(tmp) + al((size_t)nv * kBlockFloats * sizeof(float)) + 256;
-    int rc = ensure_scratch(ctx, need);
+    unsigned *keep = nullptr, *nidx = nullptr;
+    void* cub_tmp = nullptr;
+    float* pool = nullptr;   // worst case every block survives: the compacted copy needs a pool-sized scratch
+    int rc = carve_scratch(ctx, [&](Carve& c) {
+        keep = c.take<unsigned>(nv); nidx = c.take<unsigned>(nv);
+        cub_tmp = c.take<char>(tmp);
+        pool = c.take<float>((size_t)nv * kBlockFloats);
+    });
     if (rc != SRL_OK) return rc;
-    char* p = static_cast<char*>(ctx->d_scratch);
-    unsigned* keep = reinterpret_cast<unsigned*>(p); p += al((size_t)nv * 4);
-    unsigned* nidx = reinterpret_cast<unsigned*>(p); p += al((size_t)nv * 4);
-    void* cub_tmp = p; p += al(tmp);
-    float* pool = reinterpret_cast<float*>(p);
     const int T = 256;
     k_far_flags<<<(unsigned)((nv + T - 1) / T), T, 0, ctx->stream>>>(m->d_blocks, nv, location[0], location[1], location[2], distance * distance, keep);
     SRL_CUDA(ctx, cudaGetLastError());
     SRL_CUDA(ctx, cub::DeviceScan::ExclusiveSum(cub_tmp, tmp, keep, nidx, (int)nv, ctx->stream));
-    unsigned last_keep = 0, last_idx = 0;
-    SRL_CUDA(ctx, cudaMemcpyAsync(&last_keep, keep + (nv - 1), 4, cudaMemcpyDeviceToHost, ctx->stream));
-    SRL_CUDA(ctx, cudaMemcpyAsync(&last_idx, nidx + (nv - 1), 4, cudaMemcpyDeviceToHost, ctx->stream));
-    SRL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    const long long n_keep = (long long)last_idx + last_keep;
+    long long n_keep = 0;
+    if ((rc = scan_total(ctx, keep, nidx, nv, &n_keep)) != SRL_OK) return rc;
     ctx->launches += 2;
     if (n_keep == nv) return SRL_OK;   // nothing to evict
     const long long n_quads = nv * (kBlockFloats / 4);
@@ -1064,14 +1109,13 @@ int srl_map_upload(srl_map* m, const int16_t* keys, const int32_t* counts, const
         if (counts[v] < 0 || counts[v] > cap) return set_err(ctx, SRL_BAD_ARG, "srl_map_upload: count outside [0, cap]");
         total_pts += counts[v];
     }
-    const size_t b_keys = align_up(n_voxels * 3 * sizeof(short)), b_cnt = align_up(n_voxels * sizeof(int)),
-                 b_xyz = align_up(n_voxels * cap * 3 * sizeof(float));
-    if ((rc = ensure_scratch(ctx, b_keys + b_cnt + b_xyz + 256)) != SRL_OK) return rc;
-    char* base = static_cast<char*>(ctx->d_scratch);
-    short* d_keys = reinterpret_cast<short*>(base);
-    int* d_cnt = reinterpret_cast<int*>(base + b_keys);
-    float* d_xyz = reinterpret_cast<float*>(base + b_keys + b_cnt);
-    int* d_dup = reinterpret_cast<int*>(base + b_keys + b_cnt + b_xyz);
+    short* d_keys = nullptr;
+    int *d_cnt = nullptr, *d_dup = nullptr;
+    float* d_xyz = nullptr;
+    rc = carve_scratch(ctx, [&](Carve& c) {
+        d_keys = c.take<short>(n_voxels * 3); d_cnt = c.take<int>(n_voxels); d_xyz = c.take<float>(n_voxels * cap * 3); d_dup = c.take<int>(1);
+    });
+    if (rc != SRL_OK) return rc;
     SRL_CUDA(ctx, cudaMemcpyAsync(d_keys, keys, n_voxels * 3 * sizeof(short), cudaMemcpyHostToDevice, ctx->stream));
     SRL_CUDA(ctx, cudaMemcpyAsync(d_cnt, counts, n_voxels * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
     SRL_CUDA(ctx, cudaMemcpyAsync(d_xyz, xyz, n_voxels * cap * 3 * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
@@ -1099,13 +1143,11 @@ int srl_map_download(srl_map* m, int16_t* keys, int32_t* counts, float* xyz, siz
     if (nv == 0) return SRL_OK;
     if (nv > max_voxels || !keys || !counts || !xyz) return set_err(ctx, SRL_BAD_ARG, "srl_map_download: output too small");
     const int cap = m->cap;
-    const size_t b_keys = align_up(nv * 3 * sizeof(short)), b_cnt = align_up(nv * sizeof(int)), b_xyz = align_up(nv * cap * 3 * sizeof(float));
-    int rc;
-    if ((rc = ensure_scratch(ctx, b_keys + b_cnt + b_xyz)) != SRL_OK) return rc;
-    char* base = static_cast<char*>(ctx->d_scratch);
-    short* d_keys = reinterpret_cast<short*>(base);
-    int* d_cnt = reinterpret_cast<int*>(base + b_keys);
-    float* d_xyz = reinterpret_cast<float*>(base + b_keys + b_cnt);
+    short* d_keys = nullptr;
+    int* d_cnt = nullptr;
+    float* d_xyz = nullptr;
+    int rc = carve_scratch(ctx, [&](Carve& c) { d_keys = c.take<short>(nv * 3); d_cnt = c.take<int>(nv); d_xyz = c.take<float>(nv * cap * 3); });
+    if (rc != SRL_OK) return rc;
     const int T = 256;
     k_download<<<(unsigned)((nv * cap + T - 1) / T), T, 0, ctx->stream>>>(m->d_blocks, m->block_pts, (long long)nv, cap, d_keys, d_cnt, d_xyz);
     ctx->launches += 1;
@@ -1117,103 +1159,87 @@ int srl_map_download(srl_map* m, int16_t* keys, int32_t* counts, float* xyz, siz
     return SRL_OK;
 }
 
+// where an insert's points come from: n world points in a caller's buffer (host or device, detected per pointer), or the
+// resident sweep under the pose (q, t) when sweep is set
+struct InsertSource {
+    const double* xyz;
+    size_t n;
+    srl_sweep* sweep;
+    const double *q, *t, *R_il, *t_il;
+};
 // the registered cloud of an insert (addPointToPcl, src/lioOptimization.cpp:432,1346-1355)
 struct PublishArgs {
     double translation_z;   // p_frame->p_state->translation.z()
-    float* d_out;           // device destination (n * 4 floats), or null: the cloud is left in scratch at *d_cloud
-    float* d_cloud = nullptr;
-    int64_t n_published = 0;
+    float* xyzi_out;        // host or device, max_out * 4 floats
+    size_t max_out;
+    int64_t* n_published;
 };
 
-static size_t publish_scratch_bytes(size_t n) { return align_up(n) + align_up(n * 4) + align_up(n * 16) + 256; }
-
-static int map_insert_impl(srl_map* m, const double* d_xyz, size_t n, double min_distance_points, int32_t min_num_points,
-                           int64_t* n_added, char* scratch_after_points, PublishArgs* pa = nullptr) {
+// addPointsToMap (and with pa its published cloud) for every srl_map_insert* entry point; nothing is touched before the
+// argument checks pass
+static int insert_entry(srl_map* m, const InsertSource& src, double min_distance_points, int32_t min_num_points, int64_t* n_added,
+                        const PublishArgs* pa) {
     srl_ctx* ctx = m->ctx;
+    const size_t n = src.n;
+    if (n_added) *n_added = 0;
+    if (pa && pa->n_published) *pa->n_published = 0;
+    if (int rc = check_lio_map(ctx, m)) return rc;
+    if (pa && n && !pa->xyzi_out) return set_err(ctx, SRL_BAD_ARG, "srl_map_insert_published: xyzi_out is NULL");
+    if (pa && pa->max_out < n) return set_err(ctx, SRL_BAD_ARG, "srl_map_insert_published: max_out < n (up to n points can be published)");
+    if (n > 0x7fffffffULL) return set_err(ctx, SRL_BAD_ARG, "srl_map_insert: n must fit in int32");
+    if (src.sweep && src.sweep->ctx != ctx) return set_err(ctx, SRL_BAD_ARG, "map and sweep belong to different contexts");
+    if (n == 0) return SRL_OK;
+    SRL_CUDA(ctx, cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->stream;
-    // scratch carve-up
-    char* p = scratch_after_points;
-    auto take = [&](size_t bytes) { char* r = p; p += align_up(bytes); return r; };
-    unsigned long long* keys_a = reinterpret_cast<unsigned long long*>(take(n * 8));
-    unsigned long long* keys_b = reinterpret_cast<unsigned long long*>(take(n * 8));
-    unsigned int* idx_a = reinterpret_cast<unsigned int*>(take(n * 4));
-    unsigned int* idx_b = reinterpret_cast<unsigned int*>(take(n * 4));
-    float* fxyz = reinterpret_cast<float*>(take(n * 12));
-    unsigned char* flags = reinterpret_cast<unsigned char*>(take(n));
-    unsigned int* seg_start = reinterpret_cast<unsigned int*>(take(n * 4));
-    int* seg_slot = reinterpret_cast<int*>(take(n * 4));
-    unsigned int* is_new = reinterpret_cast<unsigned int*>(take(n * 4));
-    unsigned int* new_rank = reinterpret_cast<unsigned int*>(take(n * 4));
-    int* d_nseg = reinterpret_cast<int*>(take(256));
-    unsigned int* d_total_new = reinterpret_cast<unsigned int*>(take(256));
-    size_t tmp_sort = 0, tmp_sel = 0, tmp_scan = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, tmp_sort, keys_a, keys_b, idx_a, idx_b, (int)n, 0, 50, st);
-    cub::DeviceSelect::Flagged(nullptr, tmp_sel, thrust::counting_iterator<unsigned int>(0), flags, seg_start, d_nseg, (int)n, st);
-    cub::DeviceScan::ExclusiveSum(nullptr, tmp_scan, is_new, new_rank, (int)n, st);
-    const size_t tmp_bytes = std::max(tmp_sort, std::max(tmp_sel, tmp_scan));
-    void* d_tmp = take(tmp_bytes);
-    // publication (after everything the plain insert carves, so its layout is unchanged): per-point flags, the selected
-    // sweep indices, their count, and the cloud when it is not written straight to the caller's device buffer
-    unsigned char* pub = nullptr;
+    const int N = (int)n;
+    const size_t tmp_bytes = segment_tmp_bytes(N, st);
+    Staged<const double> in(src.sweep ? nullptr : src.xyz);
+    Staged<float> cloud(pa ? pa->xyzi_out : nullptr);
+    double* d_registered = nullptr;   // the sweep's points under the pose
+    Segments s;
+    float* fxyz = nullptr;
+    unsigned char* pub = nullptr;     // publication: per-point flags, the selected sweep indices and their count
     unsigned int* pub_sel = nullptr;
     int* d_npub = nullptr;
-    if (pa) {
-        pub = reinterpret_cast<unsigned char*>(take(n));
-        pub_sel = reinterpret_cast<unsigned int*>(take(n * 4));
-        d_npub = reinterpret_cast<int*>(take(256));
-        pa->d_cloud = pa->d_out ? pa->d_out : reinterpret_cast<float*>(take(n * 16));
-        pa->n_published = 0;
-        SRL_CUDA(ctx, cudaMemsetAsync(pub, 0, n, st));
-    }
+    int rc = carve_scratch(ctx, [&](Carve& c) {
+        if (src.sweep) d_registered = c.take<double>(n * 3);
+        in.place(c, n * 3);
+        s.place(c, n, tmp_bytes);
+        fxyz = c.take<float>(n * 3);
+        if (pa) { pub = c.take<unsigned char>(n); pub_sel = c.take<unsigned int>(n); d_npub = c.take<int>(1); cloud.place(c, n * 4); }
+    });
+    if (rc != SRL_OK) return rc;
+    if (src.sweep) rc = srl_sweep_transform_device(ctx, src.sweep, src.q, src.t, src.R_il, src.t_il, d_registered);
+    else rc = in.upload(ctx, n * 3);
+    if (rc != SRL_OK) return rc;
+    if (pa) SRL_CUDA(ctx, cudaMemsetAsync(pub, 0, n, st));
 
     const int T = 256;
     const unsigned gb = (unsigned)((n + T - 1) / T);
-    k_insert_keys<<<gb, T, 0, st>>>(d_xyz, (long long)n, m->voxel_size, keys_a, idx_a, fxyz);
-    size_t tb = tmp_bytes;
-    cub::DeviceRadixSort::SortPairs(d_tmp, tb, keys_a, keys_b, idx_a, idx_b, (int)n, 0, 50, st);
-    k_seg_flags<<<gb, T, 0, st>>>(keys_b, (long long)n, flags);
-    tb = tmp_bytes;
-    cub::DeviceSelect::Flagged(d_tmp, tb, thrust::counting_iterator<unsigned int>(0), flags, seg_start, d_nseg, (int)n, st);
+    k_insert_keys<<<gb, T, 0, st>>>(src.sweep ? d_registered : in.d, (long long)n, m->voxel_size, s.keys, s.idx, fxyz);
+    ctx->launches += 1;
     int n_seg = 0;
-    SRL_CUDA(ctx, cudaMemcpyAsync(&n_seg, d_nseg, sizeof(int), cudaMemcpyDeviceToHost, st));
-    SRL_CUDA(ctx, cudaStreamSynchronize(st));
-    ctx->launches += 4;
-    if (n_seg == 0) { if (n_added) *n_added = 0; return SRL_OK; }
-    // at most n_seg new voxels; seg_slot holds slot indices, so the table is rebuilt (if at all) before the lookup
-    int rc = map_grow(m, (size_t)m->n_voxels + (size_t)n_seg);
-    if (rc != SRL_OK) return rc;
-    const unsigned mask = (unsigned)(m->capacity - 1);
-    const unsigned gs = (unsigned)((n_seg + T - 1) / T);
-    k_seg_lookup<<<gs, T, 0, st>>>(m->d_slots, mask, keys_b, seg_start, d_nseg, min_num_points <= 0 ? 1 : 0, seg_slot, is_new);
-    tb = tmp_bytes;
-    cub::DeviceScan::ExclusiveSum(d_tmp, tb, is_new, new_rank, n_seg, st);
-    // total new voxels = new_rank[last] + is_new[last]
-    unsigned int last_rank = 0, last_new = 0;
-    SRL_CUDA(ctx, cudaMemcpyAsync(&last_rank, new_rank + (n_seg - 1), sizeof(unsigned int), cudaMemcpyDeviceToHost, st));
-    SRL_CUDA(ctx, cudaMemcpyAsync(&last_new, is_new + (n_seg - 1), sizeof(unsigned int), cudaMemcpyDeviceToHost, st));
-    SRL_CUDA(ctx, cudaStreamSynchronize(st));
-    ctx->launches += 2;
-    const long long total_new = (long long)last_rank + last_new;
-    (void)d_total_new;
-    if ((size_t)(m->n_voxels + total_new) > m->max_voxels)
-        return set_err(ctx, SRL_MAP_FULL, "srl_map_insert: voxel pool exhausted (raise max_voxels)");
+    if ((rc = segment_keys(ctx, s, N, &n_seg)) != SRL_OK) return rc;
+    if (n_seg == 0) return SRL_OK;
+    long long total_new = 0;
+    if ((rc = count_new_voxels(m, s, n_seg, min_num_points <= 0, "srl_map_insert", &total_new)) != SRL_OK) return rc;
     long long before = 0, after = 0;
     SRL_CUDA(ctx, cudaMemcpyAsync(&before, m->d_counters, sizeof(long long), cudaMemcpyDeviceToHost, st));
     if (total_new > 0) {
-        k_seg_claim<<<gs, T, 0, st>>>(m->d_slots, mask, m->d_blocks, keys_b, seg_start, d_nseg, is_new, new_rank,
-                                      (long long)m->n_voxels, seg_slot);
+        k_seg_claim<<<(unsigned)((n_seg + T - 1) / T), T, 0, st>>>(m->d_slots, (unsigned)(m->capacity - 1), m->d_blocks, s.keys_sorted, s.start,
+                                                                   s.d_count, s.is_new, s.new_rank, (long long)m->n_voxels, s.slot);
         ctx->launches += 1;
     }
     const unsigned gw = (unsigned)(((long long)n_seg * 32 + T - 1) / T);
-    k_seg_process<<<gw, T, 0, st>>>(m->d_slots, m->d_blocks, keys_b, idx_b, fxyz, seg_start, d_nseg, seg_slot, (long long)n,
-                                    m->voxel_size, m->cap, min_distance_points, min_num_points, m->d_counters, is_new, pub);
+    k_seg_process<<<gw, T, 0, st>>>(m->d_slots, m->d_blocks, s.keys_sorted, s.idx_sorted, fxyz, s.start, s.d_count, s.slot, (long long)n,
+                                    m->voxel_size, m->cap, min_distance_points, min_num_points, m->d_counters, s.is_new, pub);
     ctx->launches += 1;
     SRL_CUDA(ctx, cudaGetLastError());
     int n_pub = 0;
     if (pa) {   // order-preserving compaction of the flagged points, then their (x, y, z, intensity)
-        tb = tmp_bytes;
-        SRL_CUDA(ctx, cub::DeviceSelect::Flagged(d_tmp, tb, thrust::counting_iterator<unsigned int>(0), pub, pub_sel, d_npub, (int)n, st));
-        k_publish_gather<<<gb, T, 0, st>>>(fxyz, pub_sel, d_npub, pa->translation_z, pa->d_cloud);
+        size_t tb = tmp_bytes;
+        SRL_CUDA(ctx, cub::DeviceSelect::Flagged(s.tmp, tb, thrust::counting_iterator<unsigned int>(0), pub, pub_sel, d_npub, N, st));
+        k_publish_gather<<<gb, T, 0, st>>>(fxyz, pub_sel, d_npub, pa->translation_z, cloud.d);
         SRL_CUDA(ctx, cudaGetLastError());
         SRL_CUDA(ctx, cudaMemcpyAsync(&n_pub, d_npub, sizeof(int), cudaMemcpyDeviceToHost, st));
         ctx->launches += 2;
@@ -1222,13 +1248,10 @@ static int map_insert_impl(srl_map* m, const double* d_xyz, size_t n, double min
     SRL_CUDA(ctx, cudaStreamSynchronize(st));
     m->n_voxels += total_new;
     if (n_added) *n_added = after - before;
-    if (pa) pa->n_published = n_pub;
+    if (!pa) return SRL_OK;
+    if ((rc = cloud.hand_back(ctx, (size_t)n_pub * 4)) != SRL_OK) return rc;
+    if (pa->n_published) *pa->n_published = n_pub;
     return SRL_OK;
-}
-
-static size_t insert_scratch_bytes(size_t n) {
-    // generous upper bound: arrays + CUB temp (radix sort of 64-bit keys needs ~ (8+4)*n + small)
-    return n * (8 + 8 + 4 + 4 + 12 + 1 + 4 + 4 + 4 + 4) + n * 16 + (1u << 20) + 16 * 256;
 }
 
 namespace {
@@ -1254,26 +1277,26 @@ int srl_grid_sampling(srl_ctx* ctx, const double* xyz_world, size_t n, double si
     cub::DeviceSelect::Flagged(nullptr, tmp_sel, thrust::counting_iterator<unsigned int>(0), (unsigned char*)nullptr,
                                (unsigned int*)nullptr, (int*)nullptr, (int)n, st);
     const size_t tmp_bytes = std::max(tmp_sort, tmp_sel);
-    const size_t need = align_up(n * 24) + 2 * align_up(n * 8) + 3 * align_up(n * 4) + align_up(n) + 256 + align_up(tmp_bytes);
-    int rc = ensure_scratch(ctx, need);
-    if (rc != SRL_OK) return rc;
-    char* p = static_cast<char*>(ctx->d_scratch);
-    auto take = [&](size_t bytes) { char* r = p; p += align_up(bytes); return r; };
-    // the frame may already be in HBM (e.g. the output of srl_distort_frame_* / srl_sweep_transform_device): no H2D then
-    cudaPointerAttributes attr;
-    const bool on_device = cudaPointerGetAttributes(&attr, xyz_world) == cudaSuccess && attr.type == cudaMemoryTypeDevice;
-    if (!on_device) cudaGetLastError();
-    double* d_stage = reinterpret_cast<double*>(take(n * 24));
-    const double* d_xyz = on_device ? xyz_world : d_stage;
-    unsigned long long* ka = reinterpret_cast<unsigned long long*>(take(n * 8));
-    unsigned long long* kb = reinterpret_cast<unsigned long long*>(take(n * 8));
-    unsigned int* ia = reinterpret_cast<unsigned int*>(take(n * 4));
-    unsigned int* ib = reinterpret_cast<unsigned int*>(take(n * 4));
-    unsigned int* sel = reinterpret_cast<unsigned int*>(take(n * 4));
-    unsigned char* is_first = reinterpret_cast<unsigned char*>(take(n));
-    int* d_count = reinterpret_cast<int*>(take(256));
-    void* d_tmp = take(tmp_bytes);
-    if (!on_device) SRL_CUDA(ctx, cudaMemcpyAsync(d_stage, xyz_world, n * 24, cudaMemcpyHostToDevice, st));
+    // the frame may already be in HBM (e.g. the output of srl_distort_frame_* / srl_sweep_transform_device): no H2D then, and
+    // the coordinates of the kept points are gathered for the replay below
+    Staged<const double> in(xyz_world);
+    double* first_dev = nullptr;
+    unsigned long long *ka = nullptr, *kb = nullptr;
+    unsigned int *ia = nullptr, *ib = nullptr, *sel = nullptr;
+    unsigned char* is_first = nullptr;
+    int* d_count = nullptr;
+    void* d_tmp = nullptr;
+    int rc = carve_scratch(ctx, [&](Carve& c) {
+        in.place(c, n * 3);
+        if (in.dev) first_dev = c.take<double>(n * 3);
+        ka = c.take<unsigned long long>(n); kb = c.take<unsigned long long>(n);
+        ia = c.take<unsigned int>(n); ib = c.take<unsigned int>(n); sel = c.take<unsigned int>(n);
+        is_first = c.take<unsigned char>(n);
+        d_count = c.take<int>(1);
+        d_tmp = c.take<char>(tmp_bytes);
+    });
+    if (rc != SRL_OK || (rc = in.upload(ctx, n * 3)) != SRL_OK) return rc;
+    const double* d_xyz = in.d;
     const int T = 256;
     const unsigned gb = (unsigned)((n + T - 1) / T);
     k_cell_keys<<<gb, T, 0, st>>>(d_xyz, (long long)n, size, ka, ia);
@@ -1290,11 +1313,11 @@ int srl_grid_sampling(srl_ctx* ctx, const double* xyz_world, size_t n, double si
     std::vector<unsigned int> first((size_t)m);
     if (m) SRL_CUDA(ctx, cudaMemcpy(first.data(), sel, (size_t)m * sizeof(unsigned int), cudaMemcpyDeviceToHost));
     std::vector<double> first_xyz;                       // device input: the coordinates of those points come back, not the frame
-    if (on_device && m) {
-        k_gather_points<<<(unsigned)((m + T - 1) / T), T, 0, st>>>(d_xyz, sel, m, d_stage);
+    if (in.dev && m) {
+        k_gather_points<<<(unsigned)((m + T - 1) / T), T, 0, st>>>(d_xyz, sel, m, first_dev);
         SRL_CUDA(ctx, cudaGetLastError());
         first_xyz.resize((size_t)m * 3);
-        SRL_CUDA(ctx, cudaMemcpyAsync(first_xyz.data(), d_stage, (size_t)m * 24, cudaMemcpyDeviceToHost, st));
+        SRL_CUDA(ctx, cudaMemcpyAsync(first_xyz.data(), first_dev, (size_t)m * 24, cudaMemcpyDeviceToHost, st));
         SRL_CUDA(ctx, cudaStreamSynchronize(st));
     }
     // `first` = the frame indices that open a new cell, in frame order: exactly the sequence of node insertions the
@@ -1303,7 +1326,7 @@ int srl_grid_sampling(srl_ctx* ctx, const double* xyz_world, size_t n, double si
     std::tr1::unordered_map<CellKey, unsigned int, CellHash> grid;
     for (int j = 0; j < m; ++j) {
         const unsigned int i = first[(size_t)j];
-        const double* pt = on_device ? &first_xyz[3 * (size_t)j] : &xyz_world[3 * (size_t)i];
+        const double* pt = in.dev ? &first_xyz[3 * (size_t)j] : &xyz_world[3 * (size_t)i];
         CellKey k;
         k.x = static_cast<short>(pt[0] / size);
         k.y = static_cast<short>(pt[1] / size);
@@ -1417,92 +1440,52 @@ int srl_color_map_add_points(srl_color_map* cm, const double* xyz_world, size_t 
     const size_t msel = (n + (size_t)add_point_step - 1) / (size_t)add_point_step;   // points with idx % step == 0
     if (msel > 0x7fffffffULL) return set_err(ctx, SRL_BAD_ARG, "srl_color_map_add_points: too many points");
     if (msel) {
-        cudaPointerAttributes attr;
-        const bool on_device = cudaPointerGetAttributes(&attr, xyz_world) == cudaSuccess && attr.type == cudaMemoryTypeDevice;
-        if (!on_device) cudaGetLastError();
-        size_t tmp_sort = 0, tmp_sort32 = 0, tmp_sel = 0, tmp_scan = 0;
-        cub::DeviceRadixSort::SortPairs(nullptr, tmp_sort, (unsigned long long*)nullptr, (unsigned long long*)nullptr, (unsigned int*)nullptr,
-                                        (unsigned int*)nullptr, (int)msel, 0, 50, st);
+        const int M = (int)msel;
+        size_t tmp_sort32 = 0;
         cub::DeviceRadixSort::SortPairs(nullptr, tmp_sort32, (unsigned int*)nullptr, (unsigned int*)nullptr, (unsigned long long*)nullptr,
-                                        (unsigned long long*)nullptr, (int)msel, 0, 32, st);
-        cub::DeviceSelect::Flagged(nullptr, tmp_sel, thrust::counting_iterator<unsigned int>(0), (unsigned char*)nullptr,
-                                   (unsigned int*)nullptr, (int*)nullptr, (int)msel, st);
-        cub::DeviceScan::ExclusiveSum(nullptr, tmp_scan, (unsigned int*)nullptr, (unsigned int*)nullptr, (int)msel, st);
-        const size_t tmp_bytes = std::max(std::max(tmp_sort, tmp_sort32), std::max(tmp_sel, tmp_scan));
-        const size_t need = (on_device ? 0 : align_up(n * 24)) + 5 * align_up(msel * 8) + 12 * align_up(msel * 4) + align_up(msel * 12) +
-                            align_up(msel) + 4 * 256 + align_up(tmp_bytes);
-        int rc = ensure_scratch(ctx, need);
-        if (rc != SRL_OK) return rc;
-        char* p = static_cast<char*>(ctx->d_scratch);
-        auto take = [&](size_t bytes) { char* r = p; p += align_up(bytes); return r; };
-        const double* d_xyz = xyz_world;
-        if (!on_device) {
-            double* buf = reinterpret_cast<double*>(take(n * 24));
-            SRL_CUDA(ctx, cudaMemcpyAsync(buf, xyz_world, n * 24, cudaMemcpyHostToDevice, st));
-            d_xyz = buf;
-        }
-        unsigned long long* vk_a = reinterpret_cast<unsigned long long*>(take(msel * 8));
-        unsigned long long* vk_b = reinterpret_cast<unsigned long long*>(take(msel * 8));
-        unsigned long long* fk_a = reinterpret_cast<unsigned long long*>(take(msel * 8));
-        unsigned long long* fk_b = reinterpret_cast<unsigned long long*>(take(msel * 8));
-        unsigned long long* seg_key = reinterpret_cast<unsigned long long*>(take(msel * 8));
-        unsigned int* idx_a = reinterpret_cast<unsigned int*>(take(msel * 4));
-        unsigned int* idx_b = reinterpret_cast<unsigned int*>(take(msel * 4));
-        unsigned int* idx_c = reinterpret_cast<unsigned int*>(take(msel * 4));
-        unsigned int* seg_start = reinterpret_cast<unsigned int*>(take(msel * 4));
-        int* seg_slot = reinterpret_cast<int*>(take(msel * 4));
-        unsigned int* is_new = reinterpret_cast<unsigned int*>(take(msel * 4));
-        unsigned int* new_rank = reinterpret_cast<unsigned int*>(take(msel * 4));
-        unsigned int* accept_id = reinterpret_cast<unsigned int*>(take(msel * 4));
-        unsigned int* seg_first = reinterpret_cast<unsigned int*>(take(msel * 4));
-        unsigned int* seg_first_sorted = reinterpret_cast<unsigned int*>(take(msel * 4));
-        unsigned int* winner = reinterpret_cast<unsigned int*>(take(msel * 4));
-        unsigned int* wrank = reinterpret_cast<unsigned int*>(take(msel * 4));
-        float* fxyz = reinterpret_cast<float*>(take(msel * 12));
-        unsigned char* flags = reinterpret_cast<unsigned char*>(take(msel));
-        int* d_nseg = reinterpret_cast<int*>(take(256));
-        void* d_tmp = take(tmp_bytes);
+                                        (unsigned long long*)nullptr, M, 0, 32, st);
+        const size_t tmp_bytes = std::max(segment_tmp_bytes(M, st), tmp_sort32);
+        Staged<const double> in(xyz_world);
+        Segments s;
+        unsigned long long *fk_a = nullptr, *fk_b = nullptr, *seg_key = nullptr;
+        unsigned int *idx_c = nullptr, *accept_id = nullptr, *seg_first = nullptr, *seg_first_sorted = nullptr, *winner = nullptr, *wrank = nullptr;
+        float* fxyz = nullptr;
+        int rc = carve_scratch(ctx, [&](Carve& c) {
+            in.place(c, n * 3);
+            s.place(c, msel, tmp_bytes);
+            fk_a = c.take<unsigned long long>(msel); fk_b = c.take<unsigned long long>(msel); seg_key = c.take<unsigned long long>(msel);
+            idx_c = c.take<unsigned int>(msel); accept_id = c.take<unsigned int>(msel);
+            seg_first = c.take<unsigned int>(msel); seg_first_sorted = c.take<unsigned int>(msel);
+            winner = c.take<unsigned int>(msel); wrank = c.take<unsigned int>(msel);
+            fxyz = c.take<float>(msel * 3);
+        });
+        if (rc != SRL_OK || (rc = in.upload(ctx, n * 3)) != SRL_OK) return rc;
         const int T = 256;
         const unsigned gb = (unsigned)((msel + T - 1) / T);
-        k_color_keys<<<gb, T, 0, st>>>(d_xyz, (long long)msel, add_point_step, m->voxel_size, cm->min_dist, vk_a, fk_a, idx_a, fxyz);
+        k_color_keys<<<gb, T, 0, st>>>(in.d, (long long)msel, add_point_step, m->voxel_size, cm->min_dist, s.keys, fk_a, s.idx, fxyz);
         SRL_CUDA(ctx, cudaMemsetAsync(accept_id, 0xff, msel * 4, st));
         SRL_CUDA(ctx, cudaMemsetAsync(winner, 0, msel * 4, st));
-        size_t tb = tmp_bytes;
-        cub::DeviceRadixSort::SortPairs(d_tmp, tb, vk_a, vk_b, idx_a, idx_b, (int)msel, 0, 50, st);
-        k_seg_flags<<<gb, T, 0, st>>>(vk_b, (long long)msel, flags);
-        tb = tmp_bytes;
-        cub::DeviceSelect::Flagged(d_tmp, tb, thrust::counting_iterator<unsigned int>(0), flags, seg_start, d_nseg, (int)msel, st);
+        ctx->launches += 1;
         int n_seg = 0;
-        SRL_CUDA(ctx, cudaMemcpyAsync(&n_seg, d_nseg, sizeof(int), cudaMemcpyDeviceToHost, st));
-        SRL_CUDA(ctx, cudaStreamSynchronize(st));
-        ctx->launches += 4;
+        if ((rc = segment_keys(ctx, s, M, &n_seg)) != SRL_OK) return rc;
         if (n_seg > 0) {
-            if ((rc = map_grow(m, (size_t)m->n_voxels + (size_t)n_seg)) != SRL_OK) return rc;   // before the lookup: slot indices
+            long long total_new = 0;   // min_num_points = 0 (:539): an absent voxel is new
+            if ((rc = count_new_voxels(m, s, n_seg, true, "srl_color_map_add_points", &total_new)) != SRL_OK) return rc;
             const unsigned vmask = (unsigned)(m->capacity - 1);
             const unsigned gs = (unsigned)((n_seg + T - 1) / T);
-            k_seg_lookup<<<gs, T, 0, st>>>(m->d_slots, vmask, vk_b, seg_start, d_nseg, 1, seg_slot, is_new);   // min_num_points = 0 (:539)
-            tb = tmp_bytes;
-            cub::DeviceScan::ExclusiveSum(d_tmp, tb, is_new, new_rank, n_seg, st);
-            unsigned int last_rank = 0, last_new = 0;
-            SRL_CUDA(ctx, cudaMemcpyAsync(&last_rank, new_rank + (n_seg - 1), 4, cudaMemcpyDeviceToHost, st));
-            SRL_CUDA(ctx, cudaMemcpyAsync(&last_new, is_new + (n_seg - 1), 4, cudaMemcpyDeviceToHost, st));
-            SRL_CUDA(ctx, cudaStreamSynchronize(st));
-            const long long total_new = (long long)last_rank + last_new;
-            if ((size_t)(m->n_voxels + total_new) > m->max_voxels)
-                return set_err(ctx, SRL_MAP_FULL, "srl_color_map_add_points: voxel pool exhausted (raise max_voxels)");
             long long before = 0, after = 0;
             SRL_CUDA(ctx, cudaMemcpyAsync(&before, m->d_counters, sizeof(long long), cudaMemcpyDeviceToHost, st));
             if (total_new > 0)
-                k_color_seg_claim<<<gs, T, 0, st>>>(m->d_slots, vmask, m->d_blocks, m->block_pts, vk_b, seg_start, d_nseg, is_new, new_rank,
-                                                    (long long)m->n_voxels, seg_slot);
-            k_color_seg_process<<<gs, T, 0, st>>>(m->d_slots, m->d_blocks, cm->d_cpts, cm->d_last_visited, vk_b, idx_b, fxyz, seg_start, d_nseg,
-                                                  seg_slot, is_new, (long long)msel, m->cap, m->block_pts, time_sweep_end, time_last_process,
-                                                  accept_id, seg_first, m->d_counters);
+                k_color_seg_claim<<<gs, T, 0, st>>>(m->d_slots, vmask, m->d_blocks, m->block_pts, s.keys_sorted, s.start, s.d_count, s.is_new,
+                                                    s.new_rank, (long long)m->n_voxels, s.slot);
+            k_color_seg_process<<<gs, T, 0, st>>>(m->d_slots, m->d_blocks, cm->d_cpts, cm->d_last_visited, s.keys_sorted, s.idx_sorted, fxyz,
+                                                  s.start, s.d_count, s.slot, s.is_new, (long long)msel, m->cap, m->block_pts, time_sweep_end,
+                                                  time_last_process, accept_id, seg_first, m->d_counters);
             m->n_voxels += total_new;
             // ---- recent list: the voxels this sweep visited for the first time, in the order of their first point
-            k_color_seg_keys<<<gs, T, 0, st>>>(vk_b, seg_start, d_nseg, seg_key);
-            tb = tmp_bytes;
-            cub::DeviceRadixSort::SortPairs(d_tmp, tb, seg_first, seg_first_sorted, seg_key, fk_b /* reused as sorted keys */, n_seg, 0, 32, st);
+            k_color_seg_keys<<<gs, T, 0, st>>>(s.keys_sorted, s.start, s.d_count, seg_key);
+            size_t tb = tmp_bytes;
+            cub::DeviceRadixSort::SortPairs(s.tmp, tb, seg_first, seg_first_sorted, seg_key, fk_b /* reused as sorted keys */, n_seg, 0, 32, st);
             const long long host_cnt[4] = {cm->n_rgb_points, cm->n_recent_temp, 0, 0};
             SRL_CUDA(ctx, cudaMemcpyAsync(cm->d_counters, host_cnt, sizeof(host_cnt), cudaMemcpyHostToDevice, st));
             // at most n_seg entries are appended; below the limit the committed list holds all of them, so only the limit
@@ -1523,15 +1506,12 @@ int srl_color_map_add_points(srl_color_map* cm, const double* xyz_world, size_t 
             const unsigned fmask = (unsigned)(cm->fine_capacity - 1);
             k_color_mask_fine<<<gb, T, 0, st>>>(fk_a, accept_id, (long long)msel);
             tb = tmp_bytes;
-            cub::DeviceRadixSort::SortPairs(d_tmp, tb, fk_a, fk_b, idx_a, idx_c, (int)msel, 0, 50, st);
+            cub::DeviceRadixSort::SortPairs(s.tmp, tb, fk_a, fk_b, s.idx, idx_c, M, 0, 50, st);
             k_color_fine_winners<<<gb, T, 0, st>>>(cm->d_fine, fmask, fk_b, idx_c, (long long)msel, winner);
             tb = tmp_bytes;
-            cub::DeviceScan::ExclusiveSum(d_tmp, tb, winner, wrank, (int)msel, st);
-            unsigned int lr = 0, lw = 0;
-            SRL_CUDA(ctx, cudaMemcpyAsync(&lr, wrank + (msel - 1), 4, cudaMemcpyDeviceToHost, st));
-            SRL_CUDA(ctx, cudaMemcpyAsync(&lw, winner + (msel - 1), 4, cudaMemcpyDeviceToHost, st));
-            SRL_CUDA(ctx, cudaStreamSynchronize(st));
-            const long long n_win = (long long)lr + lw;
+            cub::DeviceScan::ExclusiveSum(s.tmp, tb, winner, wrank, M, st);
+            long long n_win = 0;
+            if ((rc = scan_total(ctx, winner, wrank, M, &n_win)) != SRL_OK) return rc;
             if ((size_t)(cm->n_rgb_points + n_win) > cm->max_rgb_points)
                 return set_err(ctx, SRL_MAP_FULL, "srl_color_map_add_points: rgb point list exhausted");
             if (n_win > 0)
@@ -1539,7 +1519,7 @@ int srl_color_map_add_points(srl_color_map* cm, const double* xyz_world, size_t 
                                                    (long long)cm->committed_rgb_points);
             SRL_CUDA(ctx, cudaGetLastError());
             cm->n_rgb_points += n_win;
-            ctx->launches += 12;
+            ctx->launches += 10;
         }
     }
     if (to_rendering) {                                                         // :544-550
@@ -1560,43 +1540,30 @@ int srl_color_map_render_recent(srl_color_map* cm, const srl_camera* cam, const 
     if (n_rendered) *n_rendered = 0;
     const size_t nr = (size_t)cm->n_recent;
     if (nr == 0) return SRL_OK;
-    cudaPointerAttributes attr;
-    const bool on_device = cudaPointerGetAttributes(&attr, image_bgr) == cudaSuccess && attr.type == cudaMemoryTypeDevice;
-    if (!on_device) cudaGetLastError();
     const size_t img_bytes = (size_t)cam->rows * cam->cols * 3;
     size_t tmp_sort = 0, tmp_rle = 0;
     cub::DeviceRadixSort::SortKeys(nullptr, tmp_sort, (unsigned long long*)nullptr, (unsigned long long*)nullptr, (int)nr, 0, 50, st);
     cub::DeviceRunLengthEncode::Encode(nullptr, tmp_rle, (unsigned long long*)nullptr, (unsigned long long*)nullptr, (int*)nullptr, (int*)nullptr, (int)nr, st);
     const size_t tmp_bytes = std::max(tmp_sort, tmp_rle);
-    const size_t need = (on_device ? 0 : align_up(img_bytes)) + 2 * align_up(nr * 8) + align_up(nr * 4) + 2 * 256 + align_up(tmp_bytes);
-    int rc = ensure_scratch(ctx, need);
-    if (rc != SRL_OK) return rc;
-    char* p = static_cast<char*>(ctx->d_scratch);
-    auto take = [&](size_t bytes) { char* r = p; p += align_up(bytes); return r; };
-    const unsigned char* d_img = image_bgr;
-    if (!on_device) {
-        unsigned char* buf = reinterpret_cast<unsigned char*>(take(img_bytes));
-        SRL_CUDA(ctx, cudaMemcpyAsync(buf, image_bgr, img_bytes, cudaMemcpyHostToDevice, st));
-        d_img = buf;
-    }
-    unsigned long long* sorted = reinterpret_cast<unsigned long long*>(take(nr * 8));
-    unsigned long long* uniq = reinterpret_cast<unsigned long long*>(take(nr * 8));
-    int* mult = reinterpret_cast<int*>(take(nr * 4));
-    int* d_nuniq = reinterpret_cast<int*>(take(256));
-    unsigned long long* d_count = reinterpret_cast<unsigned long long*>(take(256));
-    void* d_tmp = take(tmp_bytes);
+    Staged<const uint8_t> img(image_bgr);
+    unsigned long long *sorted = nullptr, *uniq = nullptr, *d_count = nullptr;
+    int *mult = nullptr, *d_nuniq = nullptr;
+    void* d_tmp = nullptr;
+    int rc = carve_scratch(ctx, [&](Carve& c) {
+        img.place(c, img_bytes);
+        sorted = c.take<unsigned long long>(nr); uniq = c.take<unsigned long long>(nr);
+        mult = c.take<int>(nr); d_nuniq = c.take<int>(1); d_count = c.take<unsigned long long>(1);
+        d_tmp = c.take<char>(tmp_bytes);
+    });
+    if (rc != SRL_OK || (rc = img.upload(ctx, img_bytes)) != SRL_OK) return rc;
     SRL_CUDA(ctx, cudaMemsetAsync(d_count, 0, 8, st));
     size_t tb = tmp_bytes;
     cub::DeviceRadixSort::SortKeys(d_tmp, tb, cm->d_recent, sorted, (int)nr, 0, 50, st);
     tb = tmp_bytes;
     cub::DeviceRunLengthEncode::Encode(d_tmp, tb, sorted, uniq, mult, d_nuniq, (int)nr, st);
-    CamConst c;
-    quat_to_rot(cam->q_camera_world, c.R);
-    for (int i = 0; i < 3; ++i) { c.t_cw[i] = cam->t_camera_world[i]; c.t_wc[i] = cam->t_world_camera[i]; }
-    c.fx = cam->fx; c.fy = cam->fy; c.cx = cam->cx; c.cy = cam->cy; c.fov = cam->fov_margin; c.cols = cam->cols; c.rows = cam->rows;
     const int T = 256;
     k_color_render<<<(unsigned)((nr * 32 + T - 1) / T), T, 0, st>>>(m->d_slots, (unsigned)(m->capacity - 1), m->d_blocks, m->block_pts, cm->d_cpts, uniq, mult,
-                                                               d_nuniq, c, d_img, obs_time, d_count);
+                                                               d_nuniq, camera_constants(cam), img.d, obs_time, d_count);
     SRL_CUDA(ctx, cudaGetLastError());
     unsigned long long cnt = 0;
     SRL_CUDA(ctx, cudaMemcpyAsync(&cnt, d_count, 8, cudaMemcpyDeviceToHost, st));
@@ -1616,17 +1583,14 @@ int srl_color_map_download_state(srl_color_map* cm, size_t max_voxels, int16_t* 
     if (nv > max_voxels || !rgb || !n_rgb || !cov || !obs_dist || !last_obs || !last_visited) return set_err(ctx, SRL_BAD_ARG, "srl_color_map_download_state: output too small");
     const int cap = m->cap;
     const size_t e = nv * (size_t)cap;
-    const size_t need = align_up(e * 6) + align_up(e * 2) + align_up(e * 12) + 2 * align_up(e * 8) + align_up(nv * 8);
-    int rc = ensure_scratch(ctx, need);
+    short *d_rgb = nullptr, *d_n = nullptr;
+    float* d_cov = nullptr;
+    double *d_od = nullptr, *d_lo = nullptr, *d_lv = nullptr;
+    int rc = carve_scratch(ctx, [&](Carve& c) {
+        d_rgb = c.take<short>(e * 3); d_n = c.take<short>(e); d_cov = c.take<float>(e * 3);
+        d_od = c.take<double>(e); d_lo = c.take<double>(e); d_lv = c.take<double>(nv);
+    });
     if (rc != SRL_OK) return rc;
-    char* p = static_cast<char*>(ctx->d_scratch);
-    auto take = [&](size_t bytes) { char* r = p; p += align_up(bytes); return r; };
-    short* d_rgb = reinterpret_cast<short*>(take(e * 6));
-    short* d_n = reinterpret_cast<short*>(take(e * 2));
-    float* d_cov = reinterpret_cast<float*>(take(e * 12));
-    double* d_od = reinterpret_cast<double*>(take(e * 8));
-    double* d_lo = reinterpret_cast<double*>(take(e * 8));
-    double* d_lv = reinterpret_cast<double*>(take(nv * 8));
     const int T = 256;
     k_color_download<<<(unsigned)((e + T - 1) / T), T, 0, ctx->stream>>>(cm->d_cpts, m->d_blocks, cm->d_last_visited, m->block_pts, (long long)nv, cap, d_rgb, d_n, d_cov,
                                                                          d_od, d_lo, d_lv);
@@ -1645,137 +1609,53 @@ int srl_color_map_download_lists(srl_color_map* cm, int16_t* rgb_points /* n_rgb
     if (!cm) return SRL_BAD_ARG;
     srl_ctx* ctx = cm->ctx;
     srl_map* m = cm->vox;
+    std::vector<unsigned long long> keys(recent ? (size_t)cm->n_recent : 0);
     if (cm->n_rgb_points && rgb_points) {
         const size_t n = (size_t)cm->n_rgb_points;
-        int rc = ensure_scratch(ctx, n * 8);
+        short* d_out = nullptr;
+        int rc = carve_scratch(ctx, [&](Carve& c) { d_out = c.take<short>(n * 4); });
         if (rc != SRL_OK) return rc;
-        short* d_out = static_cast<short*>(ctx->d_scratch);
         const int T = 256;
         k_color_rgb_ids<<<(unsigned)((n + T - 1) / T), T, 0, ctx->stream>>>(cm->d_rgb_points, (long long)n, m->d_blocks, m->block_pts, d_out);
         SRL_CUDA(ctx, cudaGetLastError());
         SRL_CUDA(ctx, cudaMemcpyAsync(rgb_points, d_out, n * 8, cudaMemcpyDeviceToHost, ctx->stream));
     }
-    if (cm->n_recent && recent) {
-        std::vector<unsigned long long> keys((size_t)cm->n_recent);
-        SRL_CUDA(ctx, cudaMemcpyAsync(keys.data(), cm->d_recent, keys.size() * 8, cudaMemcpyDeviceToHost, ctx->stream));
-        SRL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        for (size_t i = 0; i < keys.size(); ++i) { short x, y, z; unpack_key(keys[i], x, y, z); recent[3 * i] = x; recent[3 * i + 1] = y; recent[3 * i + 2] = z; }
-    }
+    if (!keys.empty()) SRL_CUDA(ctx, cudaMemcpyAsync(keys.data(), cm->d_recent, keys.size() * 8, cudaMemcpyDeviceToHost, ctx->stream));
     SRL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    for (size_t i = 0; i < keys.size(); ++i) { short x, y, z; unpack_key(keys[i], x, y, z); recent[3 * i] = x; recent[3 * i + 1] = y; recent[3 * i + 2] = z; }
     return SRL_OK;
-}
-
-int srl_map_insert_device(srl_map* m, const double* d_xyz_world, size_t n, double min_distance_points, int32_t min_num_points,
-                          int64_t* n_added) {
-    if (!m || (n && !d_xyz_world)) return SRL_BAD_ARG;
-    if (n_added) *n_added = 0;
-    srl_ctx* ctx = m->ctx;
-    if (int rc = check_lio_map(ctx, m)) return rc;
-    if (n == 0) return SRL_OK;
-    if (n > 0x7fffffffULL) return set_err(ctx, SRL_BAD_ARG, "srl_map_insert: n must fit in int32");
-    SRL_CUDA(ctx, cudaSetDevice(ctx->device));
-    int rc;
-    if ((rc = ensure_scratch(ctx, insert_scratch_bytes(n))) != SRL_OK) return rc;
-    return map_insert_impl(m, d_xyz_world, n, min_distance_points, min_num_points, n_added, static_cast<char*>(ctx->d_scratch));
-}
-
-int srl_map_insert_sweep(srl_map* m, srl_sweep* sw, const double q[4], const double t[3], const double R_il[9], const double t_il[3],
-                         double min_distance_points, int32_t min_num_points, int64_t* n_added) {
-    if (!m || !sw || !q || !t || !R_il || !t_il) return SRL_BAD_ARG;
-    if (n_added) *n_added = 0;
-    srl_ctx* ctx = m->ctx;
-    if (int rc = check_lio_map(ctx, m)) return rc;
-    if (sw->ctx != ctx) return set_err(ctx, SRL_BAD_ARG, "map and sweep belong to different contexts");
-    const size_t n = sw->n;
-    if (n == 0) return SRL_OK;
-    SRL_CUDA(ctx, cudaSetDevice(ctx->device));
-    const size_t pts_bytes = align_up(n * 3 * sizeof(double));
-    int rc;
-    if ((rc = ensure_scratch(ctx, pts_bytes + insert_scratch_bytes(n))) != SRL_OK) return rc;
-    char* base = static_cast<char*>(ctx->d_scratch);
-    if ((rc = srl_sweep_transform_device(ctx, sw, q, t, R_il, t_il, reinterpret_cast<double*>(base))) != SRL_OK) return rc;
-    return map_insert_impl(m, reinterpret_cast<const double*>(base), n, min_distance_points, min_num_points, n_added, base + pts_bytes);
 }
 
 int srl_map_insert(srl_map* m, const double* xyz_world, size_t n, double min_distance_points, int32_t min_num_points,
                    int64_t* n_added) {
     if (!m || (n && !xyz_world)) return SRL_BAD_ARG;
-    if (n_added) *n_added = 0;
-    srl_ctx* ctx = m->ctx;
-    if (int rc = check_lio_map(ctx, m)) return rc;
-    if (n == 0) return SRL_OK;
-    if (n > 0x7fffffffULL) return set_err(ctx, SRL_BAD_ARG, "srl_map_insert: n must fit in int32");
-    SRL_CUDA(ctx, cudaSetDevice(ctx->device));
-    const size_t pts_bytes = align_up(n * 3 * sizeof(double));
-    int rc;
-    if ((rc = ensure_scratch(ctx, pts_bytes + insert_scratch_bytes(n))) != SRL_OK) return rc;
-    char* base = static_cast<char*>(ctx->d_scratch);
-    SRL_CUDA(ctx, cudaMemcpyAsync(base, xyz_world, n * 3 * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
-    return map_insert_impl(m, reinterpret_cast<const double*>(base), n, min_distance_points, min_num_points, n_added, base + pts_bytes);
+    return insert_entry(m, InsertSource{xyz_world, n, nullptr}, min_distance_points, min_num_points, n_added, nullptr);
 }
 
-}  // extern "C"
-
-// the argument checks of the published inserts: nothing is touched before they pass
-static int check_published(srl_map* m, size_t n, const float* xyzi_out, size_t max_out, int64_t* n_added, int64_t* n_published) {
-    srl_ctx* ctx = m->ctx;
-    if (n_added) *n_added = 0;
-    if (n_published) *n_published = 0;
-    if (int rc = check_lio_map(ctx, m)) return rc;
-    if (n && !xyzi_out) return set_err(ctx, SRL_BAD_ARG, "srl_map_insert_published: xyzi_out is NULL");
-    if (max_out < n) return set_err(ctx, SRL_BAD_ARG, "srl_map_insert_published: max_out < n (up to n points can be published)");
-    if (n > 0x7fffffffULL) return set_err(ctx, SRL_BAD_ARG, "srl_map_insert: n must fit in int32");
-    return SRL_OK;
-}
-// the insert with publication, then the cloud to a host destination if it was staged in scratch
-static int insert_published(srl_map* m, const double* d_xyz, size_t n, double min_distance_points, int32_t min_num_points,
-                            double translation_z, float* xyzi_out, int64_t* n_added, int64_t* n_published, char* scratch_after_points) {
-    PublishArgs pa;
-    pa.translation_z = translation_z;
-    const bool out_dev = is_device_ptr(xyzi_out);
-    pa.d_out = out_dev ? xyzi_out : nullptr;
-    int rc = map_insert_impl(m, d_xyz, n, min_distance_points, min_num_points, n_added, scratch_after_points, &pa);
-    if (rc != SRL_OK) return rc;
-    if (!out_dev && (rc = copy_to_host(m->ctx, xyzi_out, pa.d_cloud, (size_t)pa.n_published * 16)) != SRL_OK) return rc;
-    if (n_published) *n_published = pa.n_published;
-    return SRL_OK;
+int srl_map_insert_device(srl_map* m, const double* d_xyz_world, size_t n, double min_distance_points, int32_t min_num_points,
+                          int64_t* n_added) {
+    return srl_map_insert(m, d_xyz_world, n, min_distance_points, min_num_points, n_added);
 }
 
-extern "C" {
+int srl_map_insert_sweep(srl_map* m, srl_sweep* sw, const double q[4], const double t[3], const double R_il[9], const double t_il[3],
+                         double min_distance_points, int32_t min_num_points, int64_t* n_added) {
+    if (!m || !sw || !q || !t || !R_il || !t_il) return SRL_BAD_ARG;
+    return insert_entry(m, InsertSource{nullptr, sw->n, sw, q, t, R_il, t_il}, min_distance_points, min_num_points, n_added, nullptr);
+}
 
 int srl_map_insert_published(srl_map* m, const double* xyz_world, size_t n, double min_distance_points, int32_t min_num_points,
                              double translation_z, float* xyzi_out, size_t max_out, int64_t* n_added, int64_t* n_published) {
     if (!m || (n && !xyz_world)) return SRL_BAD_ARG;
-    int rc = check_published(m, n, xyzi_out, max_out, n_added, n_published);
-    if (rc != SRL_OK || n == 0) return rc;
-    srl_ctx* ctx = m->ctx;
-    SRL_CUDA(ctx, cudaSetDevice(ctx->device));
-    const bool in_dev = is_device_ptr(xyz_world);
-    const size_t pts_bytes = in_dev ? 0 : align_up(n * 3 * sizeof(double));
-    if ((rc = ensure_scratch(ctx, pts_bytes + insert_scratch_bytes(n) + publish_scratch_bytes(n))) != SRL_OK) return rc;
-    char* base = static_cast<char*>(ctx->d_scratch);
-    if (!in_dev) SRL_CUDA(ctx, cudaMemcpyAsync(base, xyz_world, n * 3 * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
-    return insert_published(m, in_dev ? xyz_world : reinterpret_cast<const double*>(base), n, min_distance_points, min_num_points,
-                            translation_z, xyzi_out, n_added, n_published, base + pts_bytes);
+    const PublishArgs pa{translation_z, xyzi_out, max_out, n_published};
+    return insert_entry(m, InsertSource{xyz_world, n, nullptr}, min_distance_points, min_num_points, n_added, &pa);
 }
 
 int srl_map_insert_sweep_published(srl_map* m, srl_sweep* sw, const double q[4], const double t[3], const double R_il[9],
                                    const double t_il[3], double min_distance_points, int32_t min_num_points, float* xyzi_out,
                                    size_t max_out, int64_t* n_added, int64_t* n_published) {
     if (!m || !sw || !q || !t || !R_il || !t_il) return SRL_BAD_ARG;
-    const size_t n = sw->n;
-    int rc = check_published(m, n, xyzi_out, max_out, n_added, n_published);
-    if (rc != SRL_OK) return rc;
-    srl_ctx* ctx = m->ctx;
-    if (sw->ctx != ctx) return set_err(ctx, SRL_BAD_ARG, "map and sweep belong to different contexts");
-    if (n == 0) return SRL_OK;
-    SRL_CUDA(ctx, cudaSetDevice(ctx->device));
-    const size_t pts_bytes = align_up(n * 3 * sizeof(double));
-    if ((rc = ensure_scratch(ctx, pts_bytes + insert_scratch_bytes(n) + publish_scratch_bytes(n))) != SRL_OK) return rc;
-    char* base = static_cast<char*>(ctx->d_scratch);
-    if ((rc = srl_sweep_transform_device(ctx, sw, q, t, R_il, t_il, reinterpret_cast<double*>(base))) != SRL_OK) return rc;
-    return insert_published(m, reinterpret_cast<const double*>(base), n, min_distance_points, min_num_points, t[2], xyzi_out, n_added,
-                            n_published, base + pts_bytes);
+    const PublishArgs pa{t[2], xyzi_out, max_out, n_published};
+    return insert_entry(m, InsertSource{nullptr, sw->n, sw, q, t, R_il, t_il}, min_distance_points, min_num_points, n_added, &pa);
 }
 
 int srl_color_map_export(srl_color_map* cm, int32_t min_views, int32_t order, float* xyz, uint8_t* rgb, size_t max_points, int64_t* n_out) {
@@ -1791,23 +1671,24 @@ int srl_color_map_export(srl_color_map* cm, int32_t min_views, int32_t order, fl
     cudaStream_t st = ctx->stream;
     srl_map* vm = cm->vox;
     const long long chunk = std::min<long long>(m, 1ll << 22);
-    const bool xyz_dev = xyz && is_device_ptr(xyz), rgb_dev = rgb && is_device_ptr(rgb);
     size_t tmp_sel = 0;
     cub::DeviceSelect::Flagged(nullptr, tmp_sel, thrust::counting_iterator<unsigned int>(0), (unsigned char*)nullptr, (unsigned int*)nullptr,
                                (int*)nullptr, (int)chunk, st);
-    const size_t need = align_up((size_t)m) + 2 * 256 + align_up((size_t)chunk * 4) + align_up(tmp_sel) + align_up((size_t)chunk * 12) +
-                        align_up((size_t)chunk * 3);
-    int rc = ensure_scratch(ctx, need);
+    Staged<float> out_xyz(xyz);
+    Staged<uint8_t> out_rgb(rgb);
+    unsigned char* flags = nullptr;
+    unsigned long long* d_count = nullptr;
+    int* d_nsel = nullptr;
+    unsigned int* sel = nullptr;
+    void* d_tmp = nullptr;
+    int rc = carve_scratch(ctx, [&](Carve& c) {
+        flags = c.take<unsigned char>((size_t)m);
+        d_count = c.take<unsigned long long>(1); d_nsel = c.take<int>(1);
+        sel = c.take<unsigned int>((size_t)chunk);
+        d_tmp = c.take<char>(tmp_sel);
+        out_xyz.place(c, (size_t)chunk * 3); out_rgb.place(c, (size_t)chunk * 3);   // one chunk of a host output at a time
+    });
     if (rc != SRL_OK) return rc;
-    char* p = static_cast<char*>(ctx->d_scratch);
-    auto take = [&](size_t bytes) { char* r = p; p += align_up(bytes); return r; };
-    unsigned char* flags = reinterpret_cast<unsigned char*>(take((size_t)m));
-    unsigned long long* d_count = reinterpret_cast<unsigned long long*>(take(256));
-    int* d_nsel = reinterpret_cast<int*>(take(256));
-    unsigned int* sel = reinterpret_cast<unsigned int*>(take((size_t)chunk * 4));
-    void* d_tmp = take(tmp_sel);
-    float* stage_xyz = reinterpret_cast<float*>(take((size_t)chunk * 12));
-    unsigned char* stage_rgb = reinterpret_cast<unsigned char*>(take((size_t)chunk * 3));
     const int T = 256;
     SRL_CUDA(ctx, cudaMemsetAsync(d_count, 0, 8, st));
     k_color_export_flags<<<(unsigned)((m + T - 1) / T), T, 0, st>>>(cm->d_rgb_points, cm->d_cpts, m, n, order, min_views, flags, d_count);
@@ -1825,8 +1706,8 @@ int srl_color_map_export(srl_color_map* cm, int32_t min_views, int32_t order, fl
         const long long len = std::min(chunk, m - base);
         size_t tb = tmp_sel;
         SRL_CUDA(ctx, cub::DeviceSelect::Flagged(d_tmp, tb, thrust::counting_iterator<unsigned int>(0), flags + base, sel, d_nsel, (int)len, st));
-        float* dx = xyz_dev ? xyz + 3 * off : stage_xyz;
-        unsigned char* dr = rgb_dev ? rgb + 3 * off : stage_rgb;
+        float* dx = out_xyz.dev ? xyz + 3 * off : out_xyz.d;
+        unsigned char* dr = out_rgb.dev ? rgb + 3 * off : out_rgb.d;
         k_color_export_gather<<<(unsigned)((len + T - 1) / T), T, 0, st>>>(cm->d_rgb_points, vm->d_blocks, vm->block_pts, cm->d_cpts, sel, d_nsel,
                                                                           base, n, order, dx, dr);
         SRL_CUDA(ctx, cudaGetLastError());
@@ -1834,8 +1715,8 @@ int srl_color_map_export(srl_color_map* cm, int32_t min_views, int32_t order, fl
         SRL_CUDA(ctx, cudaMemcpyAsync(&k, d_nsel, sizeof(int), cudaMemcpyDeviceToHost, st));
         SRL_CUDA(ctx, cudaStreamSynchronize(st));
         ctx->launches += 2;
-        if (!xyz_dev && (rc = copy_to_host(ctx, xyz + 3 * off, stage_xyz, (size_t)k * 12)) != SRL_OK) return rc;
-        if (!rgb_dev && (rc = copy_to_host(ctx, rgb + 3 * off, stage_rgb, (size_t)k * 3)) != SRL_OK) return rc;
+        if ((rc = out_xyz.hand_back(ctx, (size_t)k * 3, 3 * off)) != SRL_OK || (rc = out_rgb.hand_back(ctx, (size_t)k * 3, 3 * off)) != SRL_OK)
+            return rc;
         off += (size_t)k;
     }
     return SRL_OK;
@@ -1844,14 +1725,6 @@ int srl_color_map_export(srl_color_map* cm, int32_t min_views, int32_t order, fl
 }  // extern "C"
 
 // ---- selectPointsForProjection / the tracker's gather ------------------------------------------------------------------
-static CamConst camera_constants(const srl_camera* cam) {
-    CamConst c;
-    quat_to_rot(cam->q_camera_world, c.R);
-    for (int i = 0; i < 3; ++i) { c.t_cw[i] = cam->t_camera_world[i]; c.t_wc[i] = cam->t_world_camera[i]; }
-    c.fx = cam->fx; c.fy = cam->fy; c.cx = cam->cx; c.cy = cam->cy; c.fov = cam->fov_margin; c.cols = cam->cols; c.rows = cam->rows;
-    return c;
-}
-
 // The cell coordinates of one image axis: if2dPointsAvailable accepts fov * size + 1 <= x and ceil(x) < (1 - fov) * size, so
 // |x| <= a = max(|lo|, |hi|), and the cell std::round(x / d) * d lies within 2a + 1 of zero (it is 0, or |x / d| >= 1/2 and
 // |round(x / d)| <= 2 |x / d|).  The axis is offset by -b (b = ceil(2a) + 2) and takes `bits` bits, with 2^bits > 2b + 1 so that
@@ -1896,7 +1769,6 @@ int srl_color_map_select_for_projection(srl_color_map* cm, const srl_camera* cam
     SRL_CUDA(ctx, cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->stream;
     srl_map* vm = cm->vox;
-    const bool ids_dev = point_ids && is_device_ptr(point_ids), xyz_dev = xyz && is_device_ptr(xyz), uv_dev = uv && is_device_ptr(uv);
     const int n = (int)m;
     size_t tmp_sort = 0, tmp_scan = 0, tmp_red = 0, tmp_sel = 0;
     cub::DeviceRadixSort::SortPairs(nullptr, tmp_sort, (unsigned long long*)nullptr, (unsigned long long*)nullptr, (unsigned int*)nullptr,
@@ -1909,30 +1781,28 @@ int srl_color_map_select_for_projection(srl_color_map* cm, const srl_camera* cam
                                (int*)nullptr, n, st);
     const size_t tmp_bytes = std::max(std::max(tmp_sort, tmp_scan), std::max(tmp_red, tmp_sel));
     const size_t M = (size_t)m;
-    const size_t stage = (point_ids && !ids_dev ? align_up(M * 4) : 0) + (xyz && !xyz_dev ? align_up(M * 12) : 0) + (uv && !uv_dev ? align_up(M * 8) : 0);
-    const size_t need = 3 * align_up(M * 8) + 2 * align_up(M * 4) + align_up(M * 8) + align_up(M * 4) + align_up(M * 8) +
-                        3 * align_up(M * 4) + align_up(M * 4) + align_up(M) + align_up(M * 4) + 2 * 256 + align_up(tmp_bytes) + stage;
-    int rc = ensure_scratch(ctx, need);
+    Staged<unsigned int> o_ids(point_ids);
+    Staged<float> o_xyz(xyz), o_uv(uv);
+    unsigned long long *key_a = nullptr, *key_b = nullptr, *cells = nullptr;
+    unsigned int *ord_a = nullptr, *ord_b = nullptr, *cand_id = nullptr, *sel = nullptr;
+    double* depth = nullptr;
+    float2* cand_uv = nullptr;
+    float *fd = nullptr, *pre = nullptr;
+    int *taker = nullptr, *last_taker = nullptr, *d_ncells = nullptr, *d_nsel = nullptr;
+    unsigned char* win = nullptr;
+    void* d_tmp = nullptr;
+    int rc = carve_scratch(ctx, [&](Carve& c) {
+        key_a = c.take<unsigned long long>(M); key_b = c.take<unsigned long long>(M); cells = c.take<unsigned long long>(M);
+        ord_a = c.take<unsigned int>(M); ord_b = c.take<unsigned int>(M);
+        depth = c.take<double>(M); cand_id = c.take<unsigned int>(M); cand_uv = c.take<float2>(M);
+        fd = c.take<float>(M); pre = c.take<float>(M);
+        taker = c.take<int>(M); last_taker = c.take<int>(M);
+        win = c.take<unsigned char>(M); sel = c.take<unsigned int>(M);
+        d_ncells = c.take<int>(1); d_nsel = c.take<int>(1);
+        d_tmp = c.take<char>(tmp_bytes);
+        o_ids.place(c, M); o_xyz.place(c, M * 3); o_uv.place(c, M * 2);
+    });
     if (rc != SRL_OK) return rc;
-    char* p = static_cast<char*>(ctx->d_scratch);
-    auto take = [&](size_t bytes) { char* r = p; p += align_up(bytes); return r; };
-    unsigned long long* key_a = reinterpret_cast<unsigned long long*>(take(M * 8));
-    unsigned long long* key_b = reinterpret_cast<unsigned long long*>(take(M * 8));
-    unsigned long long* cells = reinterpret_cast<unsigned long long*>(take(M * 8));
-    unsigned int* ord_a = reinterpret_cast<unsigned int*>(take(M * 4));
-    unsigned int* ord_b = reinterpret_cast<unsigned int*>(take(M * 4));
-    double* depth = reinterpret_cast<double*>(take(M * 8));
-    unsigned int* cand_id = reinterpret_cast<unsigned int*>(take(M * 4));
-    float2* cand_uv = reinterpret_cast<float2*>(take(M * 8));
-    float* fd = reinterpret_cast<float*>(take(M * 4));
-    float* pre = reinterpret_cast<float*>(take(M * 4));
-    int* taker = reinterpret_cast<int*>(take(M * 4));
-    int* last_taker = reinterpret_cast<int*>(take(M * 4));
-    unsigned char* win = reinterpret_cast<unsigned char*>(take(M));
-    unsigned int* sel = reinterpret_cast<unsigned int*>(take(M * 4));
-    int* d_ncells = reinterpret_cast<int*>(take(256));
-    int* d_nsel = reinterpret_cast<int*>(take(256));
-    void* d_tmp = take(tmp_bytes);
     const int T = 256;
     const unsigned gb = (unsigned)((m + T - 1) / T);
     SRL_CUDA(ctx, cudaMemsetAsync(win, 0, M, st));
@@ -1961,15 +1831,12 @@ int srl_color_map_select_for_projection(srl_color_map* cm, const srl_camera* cam
     *n_out = k;
     if ((!point_ids && !xyz && !uv) || k == 0) return SRL_OK;
     if ((size_t)k > max_points) return set_err(ctx, SRL_BAD_ARG, "srl_color_map_select_for_projection: max_points is smaller than the number of points (count with NULL outputs first)");
-    unsigned int* o_ids = point_ids ? (ids_dev ? point_ids : reinterpret_cast<unsigned int*>(take(M * 4))) : nullptr;
-    float* o_xyz = xyz ? (xyz_dev ? xyz : reinterpret_cast<float*>(take(M * 12))) : nullptr;
-    float* o_uv = uv ? (uv_dev ? uv : reinterpret_cast<float*>(take(M * 8))) : nullptr;
-    k_proj_gather<<<(unsigned)((k + T - 1) / T), T, 0, st>>>(sel, k, cand_id, cand_uv, vm->d_blocks, vm->block_pts, o_ids, o_xyz, o_uv);
+    k_proj_gather<<<(unsigned)((k + T - 1) / T), T, 0, st>>>(sel, k, cand_id, cand_uv, vm->d_blocks, vm->block_pts, o_ids.d, o_xyz.d, o_uv.d);
     SRL_CUDA(ctx, cudaGetLastError());
     ctx->launches += 1;
-    if (point_ids && !ids_dev && (rc = copy_to_host(ctx, point_ids, o_ids, (size_t)k * 4)) != SRL_OK) return rc;
-    if (xyz && !xyz_dev && (rc = copy_to_host(ctx, xyz, o_xyz, (size_t)k * 12)) != SRL_OK) return rc;
-    if (uv && !uv_dev && (rc = copy_to_host(ctx, uv, o_uv, (size_t)k * 8)) != SRL_OK) return rc;
+    if ((rc = o_ids.hand_back(ctx, (size_t)k)) != SRL_OK || (rc = o_xyz.hand_back(ctx, (size_t)k * 3)) != SRL_OK ||
+        (rc = o_uv.hand_back(ctx, (size_t)k * 2)) != SRL_OK)
+        return rc;
     SRL_CUDA(ctx, cudaStreamSynchronize(st));
     return SRL_OK;
 }
@@ -1984,51 +1851,39 @@ int srl_color_map_gather_points(srl_color_map* cm, const uint32_t* point_ids, si
     SRL_CUDA(ctx, cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->stream;
     srl_map* vm = cm->vox;
-    const bool in_dev = is_device_ptr(point_ids);
-    const bool xyz_dev = xyz && is_device_ptr(xyz), rgb_dev = rgb && is_device_ptr(rgb), nr_dev = n_rgb && is_device_ptr(n_rgb);
-    const bool cov_dev = cov && is_device_ptr(cov), ki_dev = key_index && is_device_ptr(key_index);
-    const size_t need = (in_dev ? 0 : align_up(n * 4)) + 256 + align_up(n * 12) + align_up(n * 6) + align_up(n * 2) + align_up(n * 12) + align_up(n * 8);
-    int rc = ensure_scratch(ctx, need);
-    if (rc != SRL_OK) return rc;
-    char* p = static_cast<char*>(ctx->d_scratch);
-    auto take = [&](size_t bytes) { char* r = p; p += align_up(bytes); return r; };
-    const unsigned int* ids = point_ids;
-    if (!in_dev) {
-        unsigned int* buf = reinterpret_cast<unsigned int*>(take(n * 4));
-        SRL_CUDA(ctx, cudaMemcpyAsync(buf, point_ids, n * 4, cudaMemcpyHostToDevice, st));
-        ids = buf;
-    }
-    unsigned long long* d_bad = reinterpret_cast<unsigned long long*>(take(256));
+    Staged<const unsigned int> ids(point_ids);
+    Staged<float> o_xyz(xyz), o_cov(cov);
+    Staged<short> o_rgb(rgb), o_nr(n_rgb), o_ki(key_index);
+    unsigned long long* d_bad = nullptr;
+    int rc = carve_scratch(ctx, [&](Carve& c) {
+        ids.place(c, n);
+        d_bad = c.take<unsigned long long>(1);
+        o_xyz.place(c, n * 3); o_rgb.place(c, n * 3); o_nr.place(c, n); o_cov.place(c, n * 3); o_ki.place(c, n * 4);
+    });
+    if (rc != SRL_OK || (rc = ids.upload(ctx, n)) != SRL_OK) return rc;
     const int T = 256;
     const unsigned gb = (unsigned)((n + T - 1) / T);
     SRL_CUDA(ctx, cudaMemsetAsync(d_bad, 0, 8, st));
-    k_color_check_ids<<<gb, T, 0, st>>>(ids, (long long)n, vm->d_blocks, vm->block_pts, (long long)vm->n_voxels, d_bad);
+    k_color_check_ids<<<gb, T, 0, st>>>(ids.d, (long long)n, vm->d_blocks, vm->block_pts, (long long)vm->n_voxels, d_bad);
     SRL_CUDA(ctx, cudaGetLastError());
     unsigned long long bad = 0;
     SRL_CUDA(ctx, cudaMemcpyAsync(&bad, d_bad, 8, cudaMemcpyDeviceToHost, st));
     SRL_CUDA(ctx, cudaStreamSynchronize(st));
     ctx->launches += 1;
     if (bad) return set_err(ctx, SRL_BAD_ARG, "srl_color_map_gather_points: " + std::to_string(bad) + " point id(s) name no stored point");
-    float* o_xyz = xyz ? (xyz_dev ? xyz : reinterpret_cast<float*>(take(n * 12))) : nullptr;
-    short* o_rgb = rgb ? (rgb_dev ? rgb : reinterpret_cast<short*>(take(n * 6))) : nullptr;
-    short* o_nr = n_rgb ? (nr_dev ? n_rgb : reinterpret_cast<short*>(take(n * 2))) : nullptr;
-    float* o_cov = cov ? (cov_dev ? cov : reinterpret_cast<float*>(take(n * 12))) : nullptr;
-    short* o_ki = key_index ? (ki_dev ? key_index : reinterpret_cast<short*>(take(n * 8))) : nullptr;
-    if (o_xyz || o_rgb || o_nr || o_cov) {
-        k_color_gather<<<gb, T, 0, st>>>(ids, (long long)n, vm->d_blocks, vm->block_pts, cm->d_cpts, o_xyz, o_rgb, o_nr, o_cov);
+    if (xyz || rgb || n_rgb || cov) {
+        k_color_gather<<<gb, T, 0, st>>>(ids.d, (long long)n, vm->d_blocks, vm->block_pts, cm->d_cpts, o_xyz.d, o_rgb.d, o_nr.d, o_cov.d);
         SRL_CUDA(ctx, cudaGetLastError());
         ctx->launches += 1;
     }
-    if (o_ki) {
-        k_color_rgb_ids<<<gb, T, 0, st>>>(ids, (long long)n, vm->d_blocks, vm->block_pts, o_ki);
+    if (key_index) {
+        k_color_rgb_ids<<<gb, T, 0, st>>>(ids.d, (long long)n, vm->d_blocks, vm->block_pts, o_ki.d);
         SRL_CUDA(ctx, cudaGetLastError());
         ctx->launches += 1;
     }
-    if (xyz && !xyz_dev && (rc = copy_to_host(ctx, xyz, o_xyz, n * 12)) != SRL_OK) return rc;
-    if (rgb && !rgb_dev && (rc = copy_to_host(ctx, rgb, o_rgb, n * 6)) != SRL_OK) return rc;
-    if (n_rgb && !nr_dev && (rc = copy_to_host(ctx, n_rgb, o_nr, n * 2)) != SRL_OK) return rc;
-    if (cov && !cov_dev && (rc = copy_to_host(ctx, cov, o_cov, n * 12)) != SRL_OK) return rc;
-    if (key_index && !ki_dev && (rc = copy_to_host(ctx, key_index, o_ki, n * 8)) != SRL_OK) return rc;
+    if ((rc = o_xyz.hand_back(ctx, n * 3)) != SRL_OK || (rc = o_rgb.hand_back(ctx, n * 3)) != SRL_OK || (rc = o_nr.hand_back(ctx, n)) != SRL_OK ||
+        (rc = o_cov.hand_back(ctx, n * 3)) != SRL_OK || (rc = o_ki.hand_back(ctx, n * 4)) != SRL_OK)
+        return rc;
     SRL_CUDA(ctx, cudaStreamSynchronize(st));
     return SRL_OK;
 }

@@ -160,21 +160,6 @@ __global__ void k_imu_to_lidar_end(const double* __restrict__ imu, long long n, 
     out[3 * i] = bx - c.off[0]; out[3 * i + 1] = by - c.off[1]; out[3 * i + 2] = bz - c.off[2];
 }
 
-static bool on_device(const void* p) {
-    cudaPointerAttributes a;
-    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
-    return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
-}
-static size_t al256(size_t x) { return (x + 255) / 256 * 256; }
-
-// stages host inputs into the ctx scratch; outputs computed in scratch are copied back by finish()
-struct Stage {
-    srl_ctx* ctx;
-    char* base = nullptr;
-    size_t used = 0;
-    template <typename T> T* take(size_t count) { T* p = reinterpret_cast<T*>(base + used); used += al256(count * sizeof(T)); return p; }
-};
-
 }  // namespace srl
 
 using namespace srl;
@@ -196,24 +181,21 @@ int srl_distort_frame_by_constant(srl_ctx* ctx, const double* raw_xyz, const dou
     if (rc != SRL_OK) return rc;
     if (n == 0) return SRL_OK;
     SRL_CUDA(ctx, cudaSetDevice(ctx->device));
-    const bool d_raw = on_device(raw_xyz), d_rel = on_device(relative_time_ms), d_out = on_device(imu_xyz);
-    const size_t need = al256(n_states * sizeof(ImuDev)) + (d_raw ? 0 : al256(n * 24)) + (d_rel ? 0 : al256(n * 8)) + (d_out ? 0 : al256(n * 24));
-    if ((rc = ensure_scratch(ctx, need)) != SRL_OK) return rc;
-    Stage s{ctx, static_cast<char*>(ctx->d_scratch)};
-    ImuDev* st = s.take<ImuDev>(n_states);
+    Staged<const double> raw(raw_xyz), rel(relative_time_ms);
+    Staged<double> out(imu_xyz);
+    ImuDev* st = nullptr;
+    rc = carve_scratch(ctx, [&](Carve& c) { st = c.take<ImuDev>(n_states); raw.place(c, n * 3); rel.place(c, n); out.place(c, n * 3); });
+    if (rc != SRL_OK) return rc;
     SRL_CUDA(ctx, cudaMemcpyAsync(st, states, n_states * sizeof(ImuDev), cudaMemcpyHostToDevice, ctx->stream));
-    const double* raw = raw_xyz; const double* rel = relative_time_ms; double* out = imu_xyz;
-    if (!d_raw) { double* p = s.take<double>(n * 3); SRL_CUDA(ctx, cudaMemcpyAsync(p, raw_xyz, n * 24, cudaMemcpyHostToDevice, ctx->stream)); raw = p; }
-    if (!d_rel) { double* p = s.take<double>(n); SRL_CUDA(ctx, cudaMemcpyAsync(p, relative_time_ms, n * 8, cudaMemcpyHostToDevice, ctx->stream)); rel = p; }
-    if (!d_out) out = s.take<double>(n * 3);
+    if ((rc = raw.upload(ctx, n * 3)) != SRL_OK || (rc = rel.upload(ctx, n)) != SRL_OK) return rc;
     PointsConst c;
     std::memcpy(c.R_il, R_il, sizeof(c.R_il)); std::memcpy(c.t_il, t_il, sizeof(c.t_il));
     c.time_frame_begin = time_frame_begin; c.n_states = (int)n_states;
     const int T = 256;
-    k_distort_constant<<<(unsigned)((n + T - 1) / T), T, 0, ctx->stream>>>(raw, rel, (long long)n, st, c, out);
+    k_distort_constant<<<(unsigned)((n + T - 1) / T), T, 0, ctx->stream>>>(raw.d, rel.d, (long long)n, st, c, out.d);
     SRL_CUDA(ctx, cudaGetLastError());
     ctx->launches += 1;
-    if (!d_out) SRL_CUDA(ctx, cudaMemcpyAsync(imu_xyz, out, n * 24, cudaMemcpyDeviceToHost, ctx->stream));
+    if ((rc = out.hand_back(ctx, n * 3)) != SRL_OK) return rc;
     SRL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     return SRL_OK;
 }
@@ -229,25 +211,24 @@ int srl_distort_frame_by_imu(srl_ctx* ctx, const double* raw_xyz, const double* 
         if (!(states[k].timestamp <= states[k + 1].timestamp)) return set_err(ctx, SRL_BAD_ARG, "IMU timestamps must be non-decreasing");
     if (n_states > 4096) return set_err(ctx, SRL_BAD_ARG, "at most 4096 IMU states per sweep");
     SRL_CUDA(ctx, cudaSetDevice(ctx->device));
-    const bool d_raw = on_device(raw_xyz), d_rel = on_device(relative_time_ms), d_out = on_device(imu_xyz);
     size_t tmp = 0;
     cub::DeviceScan::InclusiveScan(nullptr, tmp, (int*)nullptr, (int*)nullptr, MaxOp(), (int)n, ctx->stream);
-    const size_t need = al256(n_states * sizeof(ImuDev)) + (d_raw ? 0 : al256(n * 24)) + (d_rel ? 0 : al256(n * 8)) + (d_out ? 0 : al256(n * 24)) +
-                        3 * al256(n * 4) + al256(16) + al256(tmp);
-    if ((rc = ensure_scratch(ctx, need)) != SRL_OK) return rc;
-    Stage s{ctx, static_cast<char*>(ctx->d_scratch)};
-    ImuDev* st = s.take<ImuDev>(n_states);
+    Staged<const double> raw(raw_xyz), rel(relative_time_ms);
+    Staged<double> out(imu_xyz);   // in/out: points the iterator never reaches keep what the caller had
+    ImuDev* st = nullptr;
+    int *f = nullptr, *l = nullptr, *m = nullptr;
+    long long* v = nullptr;   // [0] first violating point, [1] contiguity check
+    void* cub_tmp = nullptr;
+    rc = carve_scratch(ctx, [&](Carve& c) {
+        st = c.take<ImuDev>(n_states);
+        raw.place(c, n * 3); rel.place(c, n); out.place(c, n * 3);
+        f = c.take<int>(n); l = c.take<int>(n); m = c.take<int>(n);
+        v = c.take<long long>(2);
+        cub_tmp = c.take<char>(tmp);
+    });
+    if (rc != SRL_OK) return rc;
     SRL_CUDA(ctx, cudaMemcpyAsync(st, states, n_states * sizeof(ImuDev), cudaMemcpyHostToDevice, ctx->stream));
-    const double* raw = raw_xyz; const double* rel = relative_time_ms; double* out = imu_xyz;
-    if (!d_raw) { double* p = s.take<double>(n * 3); SRL_CUDA(ctx, cudaMemcpyAsync(p, raw_xyz, n * 24, cudaMemcpyHostToDevice, ctx->stream)); raw = p; }
-    if (!d_rel) { double* p = s.take<double>(n); SRL_CUDA(ctx, cudaMemcpyAsync(p, relative_time_ms, n * 8, cudaMemcpyHostToDevice, ctx->stream)); rel = p; }
-    if (!d_out) {   // in/out: points the iterator never reaches keep what the caller had
-        out = s.take<double>(n * 3);
-        SRL_CUDA(ctx, cudaMemcpyAsync(out, imu_xyz, n * 24, cudaMemcpyHostToDevice, ctx->stream));
-    }
-    int* f = s.take<int>(n); int* l = s.take<int>(n); int* m = s.take<int>(n);
-    long long* v = s.take<long long>(2);   // [0] first violating point, [1] contiguity check
-    void* cub_tmp = s.take<char>(tmp);
+    if ((rc = raw.upload(ctx, n * 3)) != SRL_OK || (rc = rel.upload(ctx, n)) != SRL_OK || (rc = out.upload(ctx, n * 3)) != SRL_OK) return rc;
     PointsConst c;
     std::memcpy(c.R_il, R_il, sizeof(c.R_il)); std::memcpy(c.t_il, t_il, sizeof(c.t_il));
     c.time_frame_begin = time_frame_begin; c.n_states = (int)n_states;
@@ -255,16 +236,16 @@ int srl_distort_frame_by_imu(srl_ctx* ctx, const double* raw_xyz, const double* 
     SRL_CUDA(ctx, cudaMemcpyAsync(v, init, sizeof(init), cudaMemcpyHostToDevice, ctx->stream));
     const int T = 256;
     const unsigned G = (unsigned)((n + T - 1) / T);
-    k_imu_intervals<<<G, T, n_states * sizeof(double), ctx->stream>>>(rel, (long long)n, st, c, f, l, reinterpret_cast<int*>(v + 1));
+    k_imu_intervals<<<G, T, n_states * sizeof(double), ctx->stream>>>(rel.d, (long long)n, st, c, f, l, reinterpret_cast<int*>(v + 1));
     SRL_CUDA(ctx, cudaGetLastError());
     SRL_CUDA(ctx, cub::DeviceScan::InclusiveScan(cub_tmp, tmp, f, m, MaxOp(), (int)n, ctx->stream));
     k_imu_first_violation<<<G, T, 0, ctx->stream>>>(m, l, (long long)n, (int)n_states, v);
-    k_distort_imu<<<G, T, 0, ctx->stream>>>(raw, rel, (long long)n, st, c, m, v, out);
+    k_distort_imu<<<G, T, 0, ctx->stream>>>(raw.d, rel.d, (long long)n, st, c, m, v, out.d);
     SRL_CUDA(ctx, cudaGetLastError());
     ctx->launches += 4;
     long long hv[2] = {0, 0};
     SRL_CUDA(ctx, cudaMemcpyAsync(hv, v, sizeof(hv), cudaMemcpyDeviceToHost, ctx->stream));
-    if (!d_out) SRL_CUDA(ctx, cudaMemcpyAsync(imu_xyz, out, n * 24, cudaMemcpyDeviceToHost, ctx->stream));
+    if ((rc = out.hand_back(ctx, n * 3)) != SRL_OK) return rc;
     SRL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     if ((int)hv[1] != 0) return set_err(ctx, SRL_BAD_ARG, "IMU intervals holding a point are not contiguous");
     if (n_written) *n_written = hv[0];
@@ -288,18 +269,15 @@ int srl_transform_all_imu_point(srl_ctx* ctx, const double* imu_xyz, size_t n, c
         c.tinv[r] = -(c.Rinv[3 * r] * last->trans[0] + (c.Rinv[3 * r + 1] * last->trans[1] + c.Rinv[3 * r + 2] * last->trans[2]));
     for (int r = 0; r < 3; ++r) for (int k = 0; k < 3; ++k) c.Rt[3 * r + k] = R_il[3 * k + r];
     for (int r = 0; r < 3; ++r) c.off[r] = c.Rt[3 * r] * t_il[0] + (c.Rt[3 * r + 1] * t_il[1] + c.Rt[3 * r + 2] * t_il[2]);
-    const bool d_in = on_device(imu_xyz), d_out = on_device(raw_out);
-    int rc;
-    if ((rc = ensure_scratch(ctx, (d_in ? 0 : al256(n * 24)) + (d_out ? 0 : al256(n * 24)) + 256)) != SRL_OK) return rc;
-    Stage s{ctx, static_cast<char*>(ctx->d_scratch)};
-    const double* in = imu_xyz; double* out = raw_out;
-    if (!d_in) { double* p = s.take<double>(n * 3); SRL_CUDA(ctx, cudaMemcpyAsync(p, imu_xyz, n * 24, cudaMemcpyHostToDevice, ctx->stream)); in = p; }
-    if (!d_out) out = s.take<double>(n * 3);
+    Staged<const double> in(imu_xyz);
+    Staged<double> out(raw_out);
+    int rc = carve_scratch(ctx, [&](Carve& s) { in.place(s, n * 3); out.place(s, n * 3); });
+    if (rc != SRL_OK || (rc = in.upload(ctx, n * 3)) != SRL_OK) return rc;
     const int T = 256;
-    k_imu_to_lidar_end<<<(unsigned)((n + T - 1) / T), T, 0, ctx->stream>>>(in, (long long)n, c, out);
+    k_imu_to_lidar_end<<<(unsigned)((n + T - 1) / T), T, 0, ctx->stream>>>(in.d, (long long)n, c, out.d);
     SRL_CUDA(ctx, cudaGetLastError());
     ctx->launches += 1;
-    if (!d_out) SRL_CUDA(ctx, cudaMemcpyAsync(raw_out, out, n * 24, cudaMemcpyDeviceToHost, ctx->stream));
+    if ((rc = out.hand_back(ctx, n * 3)) != SRL_OK) return rc;
     SRL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     return SRL_OK;
 }
