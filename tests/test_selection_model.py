@@ -31,34 +31,44 @@ def key_value(k):
     return v
 
 
-def select_model(d2_exact, d2f, size=1.0, chunks=None, lbs=None):
-    """Returns (flagged, chosen candidate indices (set), nearest candidate index).  d2_exact: float64 exact squared
-    distances; d2f: float32 values the kernel would have computed; chunks: list of index arrays visited in order
-    ("voxels") with lower bounds lbs (float32) used for the skip rule; default: one chunk, no skipping."""
-    n = d2_exact.shape[0]
+def scan_verdict(d2f, size=1.0, chunks=None, lbs=None, lpk=LPK, nls=NLS, fast=False, ids=None):
+    """The FP32 stage of one keypoint: lane lists, voxel skip, merge and verdict.  fast=False models k1_scan<lpk, nls>
+    (skip bound = the largest of the lanes' ceil(K/lpk)-th keys, lane certificate, j0 / b1 rules); fast=True models
+    k1_fast with lpk lanes of NL keys (skip bound = the smallest of the lanes' K-th keys, certifier only).  ids: the
+    10-bit candidate id packed into each key (default: the candidate's index).  Returns a dict with flagged, m, j0, b1,
+    the merged keys and, per slot, the candidate index it holds."""
+    n = d2f.shape[0]
     eps_abs = np.float32(1e-4) * np.float32(size) * np.float32(size)
-    ids = np.arange(n, dtype=np.uint32)
-    assert n <= 1024
+    ids = np.arange(n, dtype=np.uint32) if ids is None else np.asarray(ids, np.uint32)
+    assert n <= 1024 and int(ids.max(initial=0)) < 1024
     keys = (d2f.astype(np.float32).view(np.uint32) & np.uint32(0xFFFFFC00)) | ids
     if chunks is None:
         chunks, lbs = [np.arange(n)], np.zeros(1, np.float32)
-    lane_lists = [np.full(NLS, INF_KEY, np.uint32) for _ in range(LPK)]
-    q = (KF + LPK - 1) // LPK
+    width = NL if fast else nls
+    lane_lists = [np.full(width, INF_KEY, np.uint32) for _ in range(lpk)]
+    q = (KF + lpk - 1) // lpk
     for ch, lb in zip(chunks, lbs):
-        tq = max(l[q - 1] for l in lane_lists)                   # the largest of the lanes' q-th keys bounds the K-th
-        T = key_value([tq])[0]
+        if fast:
+            T = min(key_value([l[KF - 1]])[0] for l in lane_lists)   # every lane's K-th key bounds the K-th from above
+        else:
+            T = key_value([max(l[q - 1] for l in lane_lists)])[0]   # the largest of the lanes' q-th keys bounds the K-th
         with np.errstate(invalid="ignore", over="ignore"):
             if np.float32(lb) > np.float32(T + T * K_REL + np.float32(3.0) * eps_abs):
                 continue                                         # the voxel cannot matter any more
-        for lane in range(LPK):
-            mine = keys[ch[lane::LPK]]                            # dealt round-robin inside the voxel
+        ch = np.asarray(ch)
+        for lane in range(lpk):
+            mine = keys[ch[lane::lpk]]                            # dealt round-robin inside the voxel
             merged = np.sort(np.concatenate([lane_lists[lane], mine]))
-            lane_lists[lane] = merged[:NLS]
-    own_last = [l[NLS - 1] for l in lane_lists]
-    merged = np.sort(np.concatenate(lane_lists))[:32]
+            lane_lists[lane] = merged[:width]
+    own_last = [l[width - 1] for l in lane_lists]
+    merged = np.sort(np.concatenate(lane_lists + [np.full(32, INF_KEY, np.uint32)]))[:32]
     kv = key_value(merged)
+    pos = {int(k): i for i, k in enumerate(keys)}
+    slot_cand = np.array([pos.get(int(k), -1) for k in merged])
+    out = dict(keys=merged, slot_cand=slot_cand, m=0, j0=0, b1=0)
     if not np.isfinite(kv[KF - 1]):
-        return True, None, None                                   # fewer than K tracked: the kernel never gets here (total < Kmin)
+        out["flagged"] = True                                     # fewer than K tracked: the kernel never gets here (total < Kmin)
+        return out
     T = kv[KF - 1]
     lim = np.float32(T + T * K_REL + np.float32(2.5) * eps_abs)
     kvK, v0 = kv[KF], kv[0]
@@ -67,11 +77,27 @@ def select_model(d2_exact, d2f, size=1.0, chunks=None, lbs=None):
     b1 = int((kv[:NS] <= lim0).sum())
     with np.errstate(invalid="ignore"):
         j0 = int(((kv[:KF] + kv[:KF] * K_REL + np.float32(2.5) * eps_abs) < kvK).sum())
-    flagged = (not kv[NS] > lim) or any(not key_value([o])[0] > lim for o in own_last) or \
-              (m > KF and j0 < K_ZONE0) or b1 > K_BEST_MAX or b1 > j0
-    if flagged:
+    if fast:   # k1_fast resolves every slot inside the window exactly: only the certifier
+        flagged = not kv[NS] > lim
+        j0, b1 = 0, m
+    else:
+        flagged = (not kv[NS] > lim) or any(not key_value([o])[0] > lim for o in own_last) or \
+                  (m > KF and j0 < K_ZONE0) or b1 > K_BEST_MAX or b1 > j0
+    out.update(flagged=bool(flagged), m=m, j0=j0, b1=b1,
+               lane_full=any(not key_value([o])[0] > lim for o in own_last) and not fast)
+    return out
+
+
+def select_model(d2_exact, d2f, size=1.0, chunks=None, lbs=None, lpk=LPK, nls=NLS, fast=False, ids=None):
+    """Returns (flagged, chosen candidate indices (set), nearest candidate index).  d2_exact: float64 exact squared
+    distances; d2f: float32 values the kernel would have computed; chunks: list of index arrays visited in order
+    ("voxels") with lower bounds lbs (float32) used for the skip rule; default: one chunk, no skipping.  lpk / nls:
+    lanes per keypoint and keys per lane of k1_scan (4 / 14 and 2 / 20 are compiled); fast=True: k1_fast."""
+    v = scan_verdict(d2f, size, chunks, lbs, lpk, nls, fast, ids)
+    if v["flagged"]:
         return True, None, None
-    slot_ids = (merged & np.uint32(1023)).astype(np.int64)
+    m, j0, b1 = v["m"], v["j0"], v["b1"]
+    slot_ids = v["slot_cand"].astype(np.int64)
     chosen = list(slot_ids[:j0])
     zone = slot_ids[j0:m]
     if m > KF:
@@ -129,6 +155,51 @@ def test_certified_answers_are_exact(kind):
         assert certified >= 300                    # the certificate is not vacuous: ordinary inputs pass it
     if kind == "tiny":
         assert certified == 0                      # distances of the order of the FP32 error: everything goes the exact way
+
+
+FORMS = {"scan4": dict(lpk=4, nls=14), "scan2": dict(lpk=2, nls=20), "fast1": dict(lpk=1, fast=True),
+         "fast2": dict(lpk=2, fast=True), "fast4": dict(lpk=4, fast=True)}
+
+
+@pytest.mark.parametrize("form", list(FORMS))
+@pytest.mark.parametrize("kind", ["random", "near_ties", "cluster", "nearest_tie"])
+def test_certified_answers_are_exact_on_every_form(kind, form):
+    """The same attack on every compiled lane layout: k1_scan with 2 lanes of 20 keys, k1_fast with 1, 2 or 4 lanes of
+    NL keys and the certifier alone."""
+    rng = np.random.default_rng(sum(map(ord, kind + form)))
+    certified = 0
+    for trial in range(200):
+        n = int(rng.integers(64, 400))
+        d2 = adversarial_set(rng, kind, n)
+        noise = rng.choice([-1.0, 1.0, 0.0], n) * 1e-4 * rng.choice([1.0, 0.999, 0.5, 0.0], n)
+        d2f = np.maximum(d2 + noise, 0.0).astype(np.float32)
+        flagged, chosen, near = select_model(d2, d2f, **FORMS[form])
+        want_set, want_near = exact_answer(d2)
+        if not flagged:
+            certified += 1
+            assert chosen == want_set and near == want_near, (kind, form, trial)
+    if kind == "random":
+        assert certified >= 150
+
+
+def test_lane_certificate_counts_what_one_lane_holds():
+    """k1_scan deals a voxel's point i to lane i % LPK: when the K nearest crowd into one lane, that lane's list of NLS keys
+    is full inside the window and the keypoint is flagged (it cannot tell whether it dropped one), one fewer and it is
+    certified."""
+    for lpk, nls in ((4, 14), (2, 20)):
+        for in_lane in (nls - 1, nls, nls + 1):
+            if in_lane > KF:
+                continue
+            near = np.linspace(0.05, 0.3, KF)                     # the K nearest; everything else lies far outside the window
+            order = np.random.default_rng(in_lane).permutation(KF)
+            d2 = np.full(80, 0.8) + np.arange(80) * 1e-3
+            lane0 = np.arange(0, 80, lpk)
+            others = np.setdiff1d(np.arange(80), lane0)
+            d2[lane0[:in_lane]] = near[order[:in_lane]]
+            d2[others[:KF - in_lane]] = near[order[in_lane:]]
+            v = scan_verdict(d2.astype(np.float32), lpk=lpk, nls=nls, chunks=np.split(np.arange(80), 4),
+                             lbs=np.zeros(4, np.float32))
+            assert v["lane_full"] == (in_lane >= nls) and v["flagged"] == (in_lane >= nls), (lpk, nls, in_lane)
 
 
 def test_voxel_skip_never_drops_a_true_neighbour():
