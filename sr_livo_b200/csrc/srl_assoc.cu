@@ -257,23 +257,14 @@ __device__ __forceinline__ void select_exact(const float* __restrict__ blocks, c
     nfound = __popc(__ballot_sync(FULL, lane < K && bd < KINF));
 }
 
-// The pass's result straight into mapped pinned host memory (one warp): 32 sums, system fence, sequence flag.  The host
-// spins on the flag (srl_api.cu: wait_host_result) — no D2H copy, no stream synchronize on the critical path.
-__device__ __forceinline__ void publish_to_host(const K1Args& A, double tot, int lane) {
-    if (!A.host_out) return;
-    A.host_out[lane] = tot;
-    __syncwarp();
-    if (lane == 0) st_release_sys(reinterpret_cast<unsigned long long*>(A.host_out + 32), A.host_seq);
-}
-
 template <int NCH, bool DEBUG, int MINB>
-__global__ void __launch_bounds__(kK1Threads, MINB) k1_assoc(const __grid_constant__ K1Args A) {
+__global__ void __launch_bounds__(kK1Threads, MINB) k1_assoc(const __grid_constant__ PassArgs A) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int lane = threadIdx.x & 31;
     const int warp = threadIdx.x >> 5;
     __shared__ PassConst s_c;
-    if (!load_pass_const(A.dev, A.wait_pose, A.pose_ticket, A.end_ticket, A.c, s_c)) return;   // device-resident loop already ended: nothing to do
-    if (cap_chunk_done(A.cap_state)) return;   // capped pass: k* is in an earlier chunk
+    if (!load_pass_const(A.link, A.c, s_c)) return;   // device-resident loop already ended: nothing to do
+    if (cap_chunk_done(A.link)) return;   // capped pass: k* is in an earlier chunk
     const PassConst& c = s_c;
     const int K = c.K;
     const int nb = c.nb;
@@ -294,16 +285,13 @@ __global__ void __launch_bounds__(kK1Threads, MINB) k1_assoc(const __grid_consta
     unsigned fallbacks = 0;           // warp-uniform: keypoints that needed the exact selection
 
     // fallback launch with nothing flagged in this pass (the usual case): one warp forwards the fast form's sums
-    if (A.only_flagged && A.stats && __ldcg(A.stats + 2) == 0ull) {
+    if (A.only_flagged && __ldcg(&A.stats->flagged) == 0ull) {
         if (blockIdx.x == 0 && warp == 0) {
-            double tot = A.prev_out32 ? A.prev_out32[lane] : 0.0;
-            const bool finalised = __ldcg(A.stats + 3) != 0ull;   // k1_fit already finalised the pass (exchange, publication)
+            const double tot = A.prev_out32 ? A.prev_out32[lane] : 0.0;
+            const bool finalised = __ldcg(&A.stats->finalised) != 0ull;   // by k1_fit
             __syncwarp();
-            if (A.comm.world > 1 && !finalised) tot = comm_exchange(A.comm, tot, lane);
-            if (lane == 0 && finalised) A.stats[3] = 0ull;
-            A.out32[lane] = tot;
-            publish_to_host(A, tot, lane);
-            if (!finalised && !A.rows) publish_sums_to_loop(A.dev, A.pose_ticket, tot, lane);   // capped: k2_cap_reduce publishes
+            if (lane == 0 && finalised) A.stats->finalised = 0ull;
+            finalise_pass(A, finalised, tot, lane);
         }
         return;
     }
@@ -341,7 +329,7 @@ __global__ void __launch_bounds__(kK1Threads, MINB) k1_assoc(const __grid_consta
                 ofx = (float)cx; ofy = (float)cy; ofz = (float)cz;
                 rfx = (float)(pwx - (double)ofx); rfy = (float)(pwy - (double)ofy); rfz = (float)(pwz - (double)ofz);
             }
-            if (DEBUG && A.dbg_world) { A.dbg_world[3 * k] = pwx; A.dbg_world[3 * k + 1] = pwy; A.dbg_world[3 * k + 2] = pwz; }
+            if (DEBUG && A.out.dbg_world) { A.out.dbg_world[3 * k] = pwx; A.out.dbg_world[3 * k + 1] = pwy; A.out.dbg_world[3 * k + 2] = pwz; }
         }
         int my_count = 0;   // neighbours found for this lane's keypoint (0 = not a full neighbourhood)
 
@@ -370,7 +358,7 @@ __global__ void __launch_bounds__(kK1Threads, MINB) k1_assoc(const __grid_consta
                     const int vx = ckx + ox, vy = cky + oy, vz = ckz + oz;
                     vis = ((ox + nb) * W + (oy + nb)) * W + (oz + nb);   // reference scan order (:379-381)
                     unsigned b, cn;
-                    if (map_find(A.slots, A.mask, vx, vy, vz, b, cn) && (int)cn >= c.thr_occ) {   // :386-390
+                    if (map_find(A.map.slots, A.map.mask, vx, vy, vz, b, cn) && (int)cn >= c.thr_occ) {   // :386-390
                         cnt = cn; blk = b;
                         sblk[vis] = (int)b;
                         // conservative lower bound of the distance to any point stored under key (vx,vy,vz):
@@ -396,15 +384,15 @@ __global__ void __launch_bounds__(kK1Threads, MINB) k1_assoc(const __grid_consta
             unsigned bid;
             int nfound;
             u64 key = ~0ull;
-            const bool sure = select_fast<NCH>(A.blocks, cv, q, K, eps, lane, bf, bid, nfound, scanned);
-            if (!sure) { select_exact<NCH>(A.blocks, cv, q, K, lane, key, bid, nfound, scanned); ++fallbacks; }
+            const bool sure = select_fast<NCH>(A.map.blocks, cv, q, K, eps, lane, bf, bid, nfound, scanned);
+            if (!sure) { select_exact<NCH>(A.map.blocks, cv, q, K, lane, key, bid, nfound, scanned); ++fallbacks; }
 
             if (nfound >= c.Kmin) {
                 unsigned pt = 0;
                 if (lane < nfound) {
                     pt = (unsigned)sblk[bid >> 5] * kBlockFloats + 4u * (bid & 31u);
                     if (sure) {   // exact distance of the selected points, reference operation order (:394-395)
-                        const float4 mp = __ldg(reinterpret_cast<const float4*>(A.blocks + pt));
+                        const float4 mp = __ldg(reinterpret_cast<const float4*>(A.map.blocks + pt));
                         const double mx = (double)mp.x, my = (double)mp.y, mz = (double)mp.z;
                         const double dx = SRL_SUB(mx, q.px), dy = SRL_SUB(my, q.py), dz = SRL_SUB(mz, q.pz);
                         key = (u64)__double_as_longlong(SRL_ADD(SRL_MUL(dx, dx), SRL_ADD(SRL_MUL(dy, dy), SRL_MUL(dz, dz))));
@@ -438,14 +426,14 @@ __global__ void __launch_bounds__(kK1Threads, MINB) k1_assoc(const __grid_consta
                     if (DEBUG) {
                         const long long kk = A.k_begin + g * 32 + kp;
                         const int v = (int)(bid >> 5), i = (int)(bid & 31u);
-                        if (A.dbg_nbr) {
-                            short* d = A.dbg_nbr + (kk * K + lane) * 4;
+                        if (A.out.dbg_nbr) {
+                            short* d = A.out.dbg_nbr + (kk * K + lane) * 4;
                             d[0] = (short)(ckx + v / (W * W) - nb);
                             d[1] = (short)(cky + (v / W) % W - nb);
                             d[2] = (short)(ckz + v % W - nb);
                             d[3] = (short)i;
                         }
-                        if (A.dbg_nbr_dist) A.dbg_nbr_dist[kk * K + lane] = sqrt(__longlong_as_double((long long)key));
+                        if (A.out.dbg_nbr_dist) A.out.dbg_nbr_dist[kk * K + lane] = sqrt(__longlong_as_double((long long)key));
                     }
                 }
                 if (lane == kp) my_count = nfound;
@@ -461,7 +449,7 @@ __global__ void __launch_bounds__(kK1Threads, MINB) k1_assoc(const __grid_consta
         int status = 0;
         if (valid && my_count > 0) {
             PlaneRow row;
-            TileNb acc_nb{A.blocks, tile, lane};
+            TileNb acc_nb{A.map.blocks, tile, lane};
             float n0x, n0y, n0z;
             acc_nb.get(0, n0x, n0y, n0z);
             plane_residual<0>(acc_nb, my_count, (double)n0x, (double)n0y, (double)n0z, c, pwx, pwy, pwz, bx, by, bz, row);
@@ -484,28 +472,28 @@ __global__ void __launch_bounds__(kK1Threads, MINB) k1_assoc(const __grid_consta
                 v[27] = row.distance * row.distance;   // :104
                 v[28] = 1.0;
             }
-            if (A.rows) {   // per-keypoint rows for the ordered max_num_residuals cap (:107)
-                double* rr = A.rows + 8 * k;
+            if (A.out.rows) {   // per-keypoint rows for the ordered max_num_residuals cap (:107)
+                double* rr = A.out.rows + 8 * k;
 #pragma unroll
                 for (int i = 0; i < 6; ++i) rr[i] = row.J[i];
                 rr[6] = h; rr[7] = row.distance * row.distance;
                 // k2_cap_reduce reads NaN planarity from rr[0]: set it explicitly, the weight is finite when power_planarity == 0
                 if (row.nan_planarity) rr[0] = __longlong_as_double(0x7ff8000000000000ll);
             }
-            if (DEBUG && A.dbg_plane) {
-                double* d = A.dbg_plane + 16 * k;
+            if (DEBUG && A.out.dbg_plane) {
+                double* d = A.out.dbg_plane + 16 * k;
                 d[0] = bx; d[1] = by; d[2] = bz; d[3] = row.nx; d[4] = row.ny; d[5] = row.nz;
 #pragma unroll
                 for (int i = 0; i < 6; ++i) d[6 + i] = row.accepted ? row.J[i] : 0.0;
                 d[12] = row.offset; d[13] = row.distance; d[14] = row.weight; d[15] = row.a2D;
             }
         }
-        if (valid && A.status) A.status[k] = status;
+        if (valid && A.out.status) A.out.status[k] = status;
         acc += transpose_reduce32(v, lane);
         __syncwarp();   // the neighbour tile is rewritten by the next group
     }
     if (lane == 30) acc += (double)scanned;
-    if (A.stats && lane == 0 && fallbacks) atomicAdd(A.stats, (unsigned long long)fallbacks);
+    if (lane == 0 && fallbacks) atomicAdd(&A.stats->exact_fallbacks, (unsigned long long)fallbacks);
 
     // ---------------------------------------------------------------------- block + grid reduction
     __shared__ double s_acc[kK1Warps][32];
@@ -536,11 +524,8 @@ __global__ void __launch_bounds__(kK1Threads, MINB) k1_assoc(const __grid_consta
 #pragma unroll
             for (int w = 0; w < kK1Warps; ++w) tot += s_acc[w][lane];
             if (A.prev_out32) tot += A.prev_out32[lane];   // fallback launch: add k1_fast's sums (fixed order)
-            if (A.comm.world > 1) tot = comm_exchange(A.comm, tot, lane);
-            A.out32[lane] = tot;
-            if (lane == 0) { *A.ticket = 0u; if (A.only_flagged && A.stats) A.stats[2] = 0ull; }
-            publish_to_host(A, tot, lane);
-            if (!A.rows) publish_sums_to_loop(A.dev, A.pose_ticket, tot, lane);   // capped: k2_cap_reduce publishes
+            if (lane == 0) { *A.ticket = 0u; if (A.only_flagged) A.stats->flagged = 0ull; }
+            finalise_pass(A, false, tot, lane);
         }
     }
 }
@@ -561,7 +546,7 @@ __global__ void __launch_bounds__(1024, 1) k2_cap_reduce(const __grid_constant__
     __shared__ long long s_kstar;
     __shared__ int s_found;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    if (!wait_pass_ticket(A.dev, A.wait_pose, A.pose_ticket, A.end_ticket)) return;   // the loop has ended
+    if (!wait_pass_ticket(A.link)) return;   // the loop has ended
     const bool fresh = A.chunk == 0;
     if (!fresh && __ldcg(A.state + 1)) return;   // k* is in an earlier chunk of this pass
     long long run_acc = fresh ? 0 : A.state[0];
@@ -644,7 +629,7 @@ __global__ void __launch_bounds__(1024, 1) k2_cap_reduce(const __grid_constant__
         double v = 0.0;
         if (own) { v = (fresh ? 0.0 : A.out32[lane]) + tot; A.out32[lane] = v; }   // chunks append
         if (lane == 0 && A.chunks_run) *A.chunks_run += 1ull;
-        if (A.dev && (s_found || A.last)) publish_sums_to_loop(A.dev, A.pose_ticket, v, lane);
+        if (s_found || A.last) publish_sums_to_loop(A.link, v, lane);
     }
     if (tid == 0) { A.state[0] = run_acc; A.state[1] = s_found; A.state[2] = s_kstar; }
 }
@@ -687,7 +672,7 @@ static void upload_offsets(int device) {
 
 size_t k1_smem_bytes(int K) { return (size_t)kK1Warps * ((size_t)(K * NBS) * sizeof(unsigned) + 128 * sizeof(int)); }
 
-typedef void (*K1Fn)(const K1Args);
+typedef void (*K1Fn)(const PassArgs);
 static int g_minb = -1;
 void k1_set_min_blocks(int v) { if (v == 2 || v == 3 || v == 4) g_minb = v; }
 int k1_min_blocks() {   // resident blocks per SM the kernel is compiled for; SRL_K1_MINB=2|3|4 selects the variant
@@ -711,7 +696,7 @@ static K1Fn pick_k1(int nb, bool debug) {
     return debug ? pick_minb<4, true>() : pick_minb<4, false>();
 }
 
-cudaError_t launch_k1(const K1Args& a, int grid, bool debug, int device, cudaStream_t stream, bool pdl) {
+cudaError_t launch_k1(const PassArgs& a, int grid, bool debug, int device, cudaStream_t stream, bool pdl) {
     upload_offsets(device);
     const size_t smem = k1_smem_bytes(a.c.K);
     K1Fn fn = pick_k1(a.c.nb, debug);

@@ -26,10 +26,10 @@ struct __align__(16) Slot {
     unsigned int count;
 };
 
-struct MapView {
+struct MapView {               // the map as the pass kernels address it
     Slot* slots;
     unsigned int mask;        // capacity - 1
-    float* blocks;            // n_blocks * 64 floats
+    float* blocks;            // n_blocks * kBlockFloats floats
 };
 
 __host__ __device__ __forceinline__ unsigned long long pack_key(int x, int y, int z) {

@@ -449,13 +449,13 @@ __global__ void __launch_bounds__(kIekfThreads, 1) k_iekf_loop(const __grid_cons
 //      given sums to the loop the way a pass's last block does.  The pass constants it loads are never read.
 __global__ void __launch_bounds__(32) k_iekf_feed(const __grid_constant__ IekfFeedArgs A) {
     __shared__ PassConst s_c;
-    if (!load_pass_const(A.dev, A.wait_pose, A.ticket, A.end_ticket, A.c, s_c)) return;
+    if (!load_pass_const(A.link, A.c, s_c)) return;
     if (A.delay_cycles > 0) {
         const long long t0 = clock64();
         while (clock64() - t0 < A.delay_cycles) {}
     }
     __syncwarp();
-    publish_sums_to_loop(A.dev, A.ticket, A.sums[threadIdx.x], threadIdx.x);
+    publish_sums_to_loop(A.link, A.sums[threadIdx.x], threadIdx.x);
 }
 cudaError_t preload_iekf_feed() {
     cudaFuncAttributes at;

@@ -86,11 +86,18 @@ struct IekfLoopArgs {
 };
 cudaError_t launch_iekf_loop(const IekfLoopArgs& a, cudaStream_t stream);
 cudaError_t launch_iekf_abort(IekfDev* dev, cudaStream_t stream);
-struct IekfFeedArgs {         // srl_iekf_replay: a one-warp stand-in for pass `ticket - base` (k_iekf_feed)
+// How a pass kernel is tied to the device-resident loop (dev == nullptr: a host-driven pass).  The pass's last block leaves
+// its sums in dev->sums and bumps sums_seq to pose_ticket + 1.
+struct PassLink {
     IekfDev* dev;
-    const double* sums;       // device, the 32 sums this pass hands to the loop
-    unsigned long long ticket, end_ticket;
+    unsigned long long pose_ticket;   // with wait_pose the kernel first waits for pose_seq >= pose_ticket and takes its constants from
+    unsigned long long end_ticket;    // dev->pc; pose_seq >= end_ticket says the loop has ended: the kernel leaves at once
     int wait_pose;
+    const long long* cap_state;  // chunk j >= 1 of a capped pass: k2_cap_reduce's state; the grid leaves when k* is already found
+};
+struct IekfFeedArgs {         // srl_iekf_replay: a one-warp stand-in for pass `link.pose_ticket - base` (k_iekf_feed)
+    PassLink link;
+    const double* sums;       // device, the 32 sums this pass hands to the loop
     long long delay_cycles;   // > 0: spin this many SM clock ticks before publishing
     PassConst c;              // by-value constants of load_pass_const (unused)
 };
@@ -158,76 +165,60 @@ __device__ __forceinline__ double comm_exchange(const CommDev& cm, double tot, i
 }
 #endif
 
-struct K1Args {
-    PassConst c;
-    const Slot* slots;
-    unsigned int mask;
-    const float* blocks;
-    const double* raw;        // sweep, n*3 (device)
-    long long k_begin, k_end; // this rank's shard
-    double* partials;         // [grid][32]
-    unsigned int* ticket;
+// ---- arguments of the pass kernels ------------------------------------------------------------------------------
+struct PassSink {             // where a pass's final 32 sums go (finalise_pass)
     double* out32;            // device, 32 doubles
-    double* rows;             // optional n*8 (J6, h, d^2)
-    int* status;              // optional n
-    double* dbg_world;        // optional debug outputs (device)
-    short* dbg_nbr;
-    double* dbg_nbr_dist;
-    double* dbg_plane;
-    const unsigned char* only_flagged;   // optional: process only keypoints whose flag is set (k1_fast's ambiguous ones)
-    const double* prev_out32;            // optional: 32 doubles added to the final sums
-    unsigned long long* stats;   // optional device counters: [0] keypoints that took the exact-selection fallback
-    float eps_scale;             // 1 normally; +inf forces the exact selection for every keypoint (tests)
-    CommDev comm;                // multi-GPU: the last block exchanges the 32 sums with the peers over NVLink
-    double* host_out;            // optional mapped pinned host buffer: the final 32 sums are also written there, then
-    unsigned long long host_seq; // host_out[32] (as u64) = host_seq after a system fence: the host spins on it instead of
-                                 // a D2H copy + stream synchronize
-    IekfDev* dev;                // device-resident loop: the pass's last block leaves its sums in dev->sums and bumps sums_seq;
-    unsigned long long pose_ticket;   // with wait_pose the kernel first waits for pose_seq >= pose_ticket and takes its constants from
-    unsigned long long end_ticket;   // dev->pc; pose_seq >= end_ticket says the loop has ended: the kernel leaves at once
-    int wait_pose;
-    const long long* cap_state;  // chunk j >= 1 of a capped pass in the device-resident loop: k2_cap_reduce's state; the grid
-                                 // leaves when k* is already found (with rows set, k2_cap_reduce alone publishes the pass)
+    double* host_out;            // optional mapped pinned host buffer: the sums are also written there, then host_out[32] (as u64) =
+    unsigned long long host_seq; // host_seq with a system-scope release: the host spins on it instead of a D2H copy + synchronize
+    CommDev comm;             // multi-GPU: the sums are first exchanged with the peers over NVLink
 };
-
-constexpr int kFastWarps = 4;
-constexpr int kFastThreads = kFastWarps * 32;
-
-struct FastArgs {               // k1_fast (srl_fast.cu)
-    PassConst c;
-    const Slot* slots;
-    unsigned int mask;
-    const float* blocks;
-    const double* raw;          // sweep, n*3 (device)
-    const unsigned* order;      // sorted position -> keypoint index (nullptr: identity)
-    long long s_begin, s_end;   // this rank's range of sorted positions
-    double* partials;
-    unsigned int* ticket;
-    double* out32;
-    unsigned char* flags;       // per keypoint: 1 = ambiguous, redo with k1_assoc's exact selection
-    int* status;
+struct KeypointOut {          // optional per-keypoint outputs (device)
+    int* status;              // n
+    double* rows;             // n*8 (J6, h, d^2) for the ordered residual cap (k2_cap_reduce), in keypoint order
     double* dbg_world;
     short* dbg_nbr;
     double* dbg_nbr_dist;
     double* dbg_plane;
-    unsigned long long* stats;  // [1] += ambiguous keypoints
-    int force_amb_mod;          // test knob: > 0 flags every keypoint whose index is a multiple of it
-    // split form (k1_scan -> k1_fit): per sorted position, the NS boundary-inclusive candidates of the keypoint
-    unsigned* cand_rows;        // one 96-byte row per sorted position: 23 x u32 (block * 20 + index in block) + header word
-                                // (byte 0: 0 = < K candidates, K..NS = candidates inside the window, 255 = ambiguous;
-                                //  byte 1: slots certainly among the K nearest; byte 2: slots that can be the nearest)
+};
+struct PassStats {            // one per ctx, in HBM, zero between passes except the two counters
+    unsigned long long exact_fallbacks;   // counter: keypoints that took k1_assoc's exact selection
+    unsigned long long fast_ambiguous;    // counter: keypoints k1_fast / k1_scan flagged as ambiguous
+    unsigned long long flagged;     // keypoints flagged in the pass in flight; the fallback launch's last block resets it
+    unsigned long long finalised;   // k1_fit finalised the pass in flight (nothing was flagged); the fallback launch, which then
+                                    // only forwards the sums, resets it
+    int probe[2];                   // scratch of probe_concurrent_kernels
+};
+
+struct PassArgs {             // k1_scan, k1_fit, k1_fast and k1_assoc
+    PassConst c;
+    MapView map;
+    const double* raw;        // sweep, n*3 (device)
+    long long k_begin, k_end; // this rank's range: of sorted positions when `order` is set, of keypoint indices otherwise
+    double* partials;         // [grid][32]
+    unsigned int* ticket;
+    PassSink sink;
+    KeypointOut out;
+    PassStats* stats;
+    PassLink link;
+    // fast and split forms (k1_fast, k1_scan -> k1_fit)
+    const unsigned* order;    // sorted position -> keypoint index (nullptr: identity)
+    unsigned char* flags;     // per keypoint: 1 = ambiguous, redo with k1_assoc's exact selection
+    int force_amb_mod;        // test knob: > 0 flags every keypoint whose index is a multiple of it
+    unsigned* cand_rows;      // k1_scan -> k1_fit, one 96-byte row per sorted position: 23 x u32 (block * 20 + index in block) +
+                              // header word (byte 0: 0 = < K candidates, K..NS = candidates inside the window, 255 = ambiguous;
+                              //  byte 1: slots certainly among the K nearest; byte 2: slots that can be the nearest)
     unsigned long long* scan_count;   // candidates visited by k1_scan, folded into component 30 by k1_fit's last block
-    double* host_out;                 // optional: mapped host buffer; k1_fit publishes the final sums there when no keypoint
-    unsigned long long host_seq;      // was flagged in this pass (see K1Args::host_out)
-    CommDev comm;                     // multi-GPU: k1_fit's last block runs the exchange in that case
-    IekfDev* dev;                     // device-resident loop (see K1Args::dev)
-    unsigned long long pose_ticket, end_ticket;
-    int wait_pose;
-    double* rows;                     // optional n*8 per-keypoint rows (J6, h, d^2) for the ordered residual cap (k2_cap_reduce)
     unsigned int* chunk_tickets;      // k1_fit's two-level grid reduction: one ticket and one 32-double sum per chunk of 32 blocks
     double* chunk_sums;
-    const long long* cap_state;       // see K1Args::cap_state
+    // k1_assoc
+    const unsigned char* only_flagged;   // fallback launch: process only keypoints whose flag is set
+    const double* prev_out32;            // fallback launch: the first launch's 32 sums, added to the final sums
+    float eps_scale;             // 1 normally; +inf forces the exact selection for every keypoint (tests)
 };
+static_assert(sizeof(PassArgs) <= 1024, "the pass kernels' argument block stays far below the 4 KB kernel parameter space");
+
+constexpr int kFastWarps = 4;
+constexpr int kFastThreads = kFastWarps * 32;
 
 struct K2Args {                 // k2_cap_reduce: one chunk of the ordered residual cap (srl_assoc.cu)
     const double* rows;         // n*8 per-keypoint rows (J6, h, d^2) written by the chunk's pass kernels
@@ -241,9 +232,7 @@ struct K2Args {                 // k2_cap_reduce: one chunk of the ordered resid
     int last;                   // the pass's last chunk: it publishes even when k* was not found
     const double* pass_out32;   // optional: the chunk's pass sums; their [30] (candidates scanned) is added to out32[30]
     unsigned long long* chunks_run;   // optional device counter of the chunks that did work
-    IekfDev* dev;               // device-resident loop (see K1Args::dev): the chunk that finds k*, or the last one, publishes out32
-    unsigned long long pose_ticket, end_ticket;
-    int wait_pose;
+    PassLink link;              // device-resident loop: the chunk that finds k*, or the last one, publishes out32
 };
 
 #if defined(__CUDACC__)
@@ -253,23 +242,20 @@ struct K2Args {                 // k2_cap_reduce: one chunk of the ordered resid
 // no-ops for a kernel launched without the attribute.
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-// Every pass kernel reads its constants from shared memory: filled from the by-value argument (host-driven pass, pass 0
-// of the device-resident loop) or from the loop state once the ESIKF block has published them.  Returns false when the
-// loop has already ended (the whole grid leaves).
 // The ticket half of load_pass_const: lets the successor launch, waits for the predecessor, then (wait_pose) for the pose
-// of pass `ticket`.  Returns false when the loop has already ended (the whole grid leaves).
-__device__ __forceinline__ bool wait_pass_ticket(const IekfDev* dev, int wait_pose, unsigned long long ticket, unsigned long long end_ticket) {
+// of pass `pose_ticket`.  Returns false when the loop has already ended (the whole grid leaves).
+__device__ __forceinline__ bool wait_pass_ticket(const PassLink link) {
     pdl_trigger();
     pdl_wait();
-    if (dev && wait_pose) {
+    if (link.dev && link.wait_pose) {
         __shared__ int s_go;
         if (threadIdx.x == 0) {
-            const unsigned long long* ps = &dev->pose_seq;
+            const unsigned long long* ps = &link.dev->pose_seq;
             long long spins = 0;
             unsigned long long v;
-            while ((v = ld_relaxed_gpu(ps)) < ticket) { if (++spins > (1ll << 26)) { v = ~0ull; break; } }   // the ESIKF block died: leave, do not hang
+            while ((v = ld_relaxed_gpu(ps)) < link.pose_ticket) { if (++spins > (1ll << 26)) { v = ~0ull; break; } }   // the ESIKF block died: leave, do not hang
             if (v != ~0ull) v = ld_acquire_gpu(ps);
-            s_go = v < end_ticket ? 1 : 0;   // a ticket beyond the sweep's passes = the loop has ended (also a later sweep's)
+            s_go = v < link.end_ticket ? 1 : 0;   // a ticket beyond the sweep's passes = the loop has ended (also a later sweep's)
         }
         __syncthreads();
         if (!s_go) return false;
@@ -278,16 +264,18 @@ __device__ __forceinline__ bool wait_pass_ticket(const IekfDev* dev, int wait_po
 }
 // Chunk j >= 1 of a capped pass (device-resident loop): k* was found by an earlier chunk's k2_cap_reduce, which completed
 // before this kernel passed pdl_wait, so every thread reads the same word and the whole grid leaves together.
-__device__ __forceinline__ bool cap_chunk_done(const long long* cap_state) {
-    return cap_state && __ldcg(cap_state + 1) != 0;
+__device__ __forceinline__ bool cap_chunk_done(const PassLink& link) {
+    return link.cap_state && __ldcg(link.cap_state + 1) != 0;
 }
-__device__ __forceinline__ bool load_pass_const(const IekfDev* dev, int wait_pose, unsigned long long ticket, unsigned long long end_ticket,
-                                                const PassConst& by_value, PassConst& s_c) {
+// Every pass kernel reads its constants from shared memory: filled from the by-value argument (host-driven pass, pass 0
+// of the device-resident loop) or from the loop state once the ESIKF block has published them.  Returns false when the
+// loop has already ended (the whole grid leaves).
+__device__ __forceinline__ bool load_pass_const(const PassLink link, const PassConst& by_value, PassConst& s_c) {
     constexpr int ND = (int)(sizeof(PassConst) / sizeof(double));
     static_assert(sizeof(PassConst) % sizeof(double) == 0, "PassConst is copied as doubles");
-    if (!wait_pass_ticket(dev, wait_pose, ticket, end_ticket)) return false;
-    if (dev && wait_pose) {
-        if (threadIdx.x < ND) reinterpret_cast<double*>(&s_c)[threadIdx.x] = __ldcg(reinterpret_cast<const double*>(&dev->pc) + threadIdx.x);
+    if (!wait_pass_ticket(link)) return false;
+    if (link.dev && link.wait_pose) {
+        if (threadIdx.x < ND) reinterpret_cast<double*>(&s_c)[threadIdx.x] = __ldcg(reinterpret_cast<const double*>(&link.dev->pc) + threadIdx.x);
     } else if (threadIdx.x < ND) {   // by value: the kernel argument is __grid_constant__, so it can be indexed like memory (a
         // copy by thread 0 alone kept every warp of the block at the barrier below for ~10 % of k1_fit's duration)
         reinterpret_cast<double*>(&s_c)[threadIdx.x] = reinterpret_cast<const double*>(&by_value)[threadIdx.x];
@@ -296,21 +284,40 @@ __device__ __forceinline__ bool load_pass_const(const IekfDev* dev, int wait_pos
     return true;
 }
 // the pass's last block (one warp) hands the final sums to the ESIKF block
-__device__ __forceinline__ void publish_sums_to_loop(IekfDev* dev, unsigned long long ticket, double tot, int lane) {
-    if (!dev) return;
-    dev->sums[lane] = tot;
+__device__ __forceinline__ void publish_sums_to_loop(const PassLink& link, double tot, int lane) {
+    if (!link.dev) return;
+    link.dev->sums[lane] = tot;
     __syncwarp();
-    if (lane == 0) st_release_gpu(&dev->sums_seq, ticket + 1ull);
+    if (lane == 0) st_release_gpu(&link.dev->sums_seq, link.pose_ticket + 1ull);
+}
+// The pass's result straight into mapped pinned host memory (one warp): 32 sums, then the sequence word with a system-scope
+// release.  The host spins on that word (srl_api.cu: wait_host_seq) — no D2H copy, no stream synchronize on the critical path.
+__device__ __forceinline__ void publish_to_host(const PassSink& sink, double tot, int lane) {
+    if (!sink.host_out) return;
+    sink.host_out[lane] = tot;
+    __syncwarp();
+    if (lane == 0) st_release_sys(reinterpret_cast<unsigned long long*>(sink.host_out + 32), sink.host_seq);
+}
+// These are the pass's final sums: called by exactly one warp of the launch that holds them, `tot` in lane order.  Exchange
+// with the peers, out32, the host, the ESIKF block.  `forward`: an earlier launch of the pass (k1_fit) has already run the
+// exchange and handed the sums to the loop; this launch only writes the same values to out32 and to the host again.  A
+// capped pass (rows set) is handed to the loop by k2_cap_reduce alone.  A pass is published either to the host
+// (host-driven: link.dev is null) or to the loop, never both, so the order of those two steps decides nothing.
+__device__ __forceinline__ void finalise_pass(const PassArgs& A, bool forward, double tot, int lane) {
+    if (A.sink.comm.world > 1 && !forward) tot = comm_exchange(A.sink.comm, tot, lane);
+    A.sink.out32[lane] = tot;
+    publish_to_host(A.sink, tot, lane);
+    if (!forward && !A.out.rows) publish_sums_to_loop(A.link, tot, lane);
 }
 #endif
 
-cudaError_t launch_k1_fast(const FastArgs& a, int grid, bool debug, int device, cudaStream_t stream);
+cudaError_t launch_k1_fast(const PassArgs& a, int grid, bool debug, int device, cudaStream_t stream);
 // load every pass kernel (CUDA loads lazily at first launch, and a load waits for running kernels) and the offset tables;
 // *max_local is raised to the largest per-thread local memory (spill frame) of the kernels loaded
 cudaError_t preload_fast_kernels(int device, size_t* max_local);
 cudaError_t preload_assoc_kernels(int device, int K, size_t* max_local);
 constexpr int kSplitSlots = 23;   // = NS of srl_fast.cu: candidate slots k1_scan hands to k1_fit per keypoint
-cudaError_t launch_k1_split(const FastArgs& a, long long n, int max_grid, bool debug, int device, cudaStream_t stream, bool pdl);
+cudaError_t launch_k1_split(const PassArgs& a, long long n, int max_grid, bool debug, int device, cudaStream_t stream, bool pdl);
 // <<<>>> with the programmatic-stream-serialization attribute when pdl is set
 template <typename Args>
 inline cudaError_t launch_pass_kernel(void (*fn)(const Args), const Args& a, unsigned grid, unsigned block, size_t smem, cudaStream_t stream, bool pdl) {
@@ -335,7 +342,7 @@ int sweep_order_impl();             // -1 cluster kernel not verified yet, 1 ver
 size_t k1_smem_bytes(int K);
 int k1_max_blocks_per_sm(int K, int nb);
 void k1_set_min_blocks(int v);
-cudaError_t launch_k1(const K1Args& a, int grid, bool debug, int device, cudaStream_t stream, bool pdl = false);
+cudaError_t launch_k1(const PassArgs& a, int grid, bool debug, int device, cudaStream_t stream, bool pdl = false);
 cudaError_t launch_k2(const K2Args& a, cudaStream_t stream, bool pdl = false);
 cudaError_t launch_transform(const double* raw, long long n, const PassConst& c, double* out, cudaStream_t stream);
 
@@ -373,7 +380,7 @@ struct srl_ctx {
     unsigned long long* d_cap_chunks = nullptr;   // device-resident loop: k2_cap_reduce counts the capped chunks that did work
     int64_t cap_chunks_run = 0;              // counter "cap_chunks_run": capped chunks processed by the last update's passes
     bool cap_chunks_on_device = false;       // ... still to be read from d_cap_chunks
-    unsigned long long* d_stats = nullptr;   // 4 counters
+    srl::PassStats* d_stats = nullptr;
     double* d_fast_out = nullptr;            // k1_fast's 32 sums, added by the exact-fallback launch
     bool force_exact = false;
     int force_amb_mod = 0;                   // test knob for the k1_fast -> k1_assoc hand-over
