@@ -134,13 +134,18 @@ int64_t srl_ctx_kernel_launches(const srl_ctx* ctx);
 /* CUDA-event timing of the scan-matching kernel (k1_assoc) on the ctx stream: enable, then read the summed device
  * time and launch count of the passes since the last reset (bench.py "roofline"). Reading synchronises the stream. */
 int srl_ctx_set_timing(srl_ctx* ctx, int enable);
-/* tuning / test knobs (the kernel-variant selectors "split_lanes_per_keypoint", "fast_lanes_per_keypoint", "k1_min_blocks" and
- * "fast_min_blocks" choose among compiled template instances and are process-wide, everything else is per ctx):
+/* tuning / test knobs, all of them per ctx.  The kernel-variant selectors choose among compiled template instances; each
+ * also has an environment variable that srl_ctx_create reads (a value outside the allowed set leaves the default):
  * "force_exact_selection" (0|1: every keypoint takes k1_assoc's exact FP64 selection),
  * "k1_variant" (0 auto; 1: k1_fast, 3: k1_scan + k1_fit, both with the exact fallback where applicable; 2: k1_assoc
- * only), "split_lanes_per_keypoint" (2|4: lanes per keypoint in k1_scan), "k1_min_blocks" (2|3|4) and
- * "fast_min_blocks" (4|5|6|8): resident-blocks-per-SM variants of the two kernels, "fast_lanes_per_keypoint" (1|2|4:
- * lanes that share one keypoint's candidate scan in k1_fast), "fast_force_ambiguous_mod" (N > 0:
+ * only), "split_lanes_per_keypoint" (2|4, default 4, SRL_SPLIT_LPK: lanes per keypoint in k1_scan), "scan_min_blocks"
+ * (6|8, default 8, SRL_SCAN_MINB), "fit_min_blocks" (4|5|6, default 6, SRL_FIT_MINB), "k1_min_blocks" (2|3|4, default 3,
+ * SRL_K1_MINB) and "fast_min_blocks" (4|5|6|8, default 5, SRL_FAST_MINB): resident-blocks-per-SM variants of k1_scan,
+ * k1_fit, k1_assoc and k1_fast, "fast_lanes_per_keypoint" (1|2|4, default 1, SRL_FAST_LPK: lanes that share one
+ * keypoint's candidate scan in k1_fast), "cluster_order" (0|1|2|3, default 1, SRL_CLUSTER_ORDER: the sweep's Morton order
+ * by CUB's radix sort (0) or by the one-launch cluster sort (1; 2 and 3 its earlier versions), which the ctx's first four
+ * uses after the option is set check against CUB's order; setting it starts those checks again),
+ * "fast_force_ambiguous_mod" (N > 0:
  * k1_fast hands every N-th keypoint to k1_assoc, to test the hand-over), "device_loop" (1 default: srl_update_iekf[_dist]
  * keep the whole iterated update on the GPU — a persistent block runs the ESIKF algebra between the passes, all passes are
  * enqueued at once, one host wait, with or without the max_num_residuals cap; 0: the host-driven loop, which is also used
@@ -150,7 +155,9 @@ int srl_ctx_set_timing(srl_ctx* ctx, int enable);
  * ctx), "iekf_step_cycles_avg" (SM clock ticks of one ESIKF step, sums seen -> pose published; resets on read),
  * "cap_chunks_run" (keypoint chunks of the capped pass whose kernels did work: summed over the passes of the last
  * srl_update_iekf, or those of the last srl_build_plane_residuals call, whichever came last; 0 without the cap; reading
- * it after the device-resident loop synchronises the ctx stream). */
+ * it after the device-resident loop synchronises the ctx stream), "cluster_order_active" (the ctx's sweep-order sort: -1
+ * the cluster sort while its checks run, 1 the cluster sort checked, 0 CUB's).  The name of each integer option above
+ * ("k1_variant", "shuffle_rule", the kernel-variant selectors and "cluster_order") also reads back its current value. */
 int srl_ctx_set_option(srl_ctx* ctx, const char* name, int64_t value);
 int srl_ctx_get_counter(srl_ctx* ctx, const char* name, int64_t* value);
 int srl_ctx_pass_time(srl_ctx* ctx, double* total_ms, int64_t* launches, int reset);

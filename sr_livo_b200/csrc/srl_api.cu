@@ -141,16 +141,6 @@ static std::vector<long long> cap_chunk_bounds(long long n, long long cap) {
 
 constexpr bool kDefaultSplit = true;    // variant 0 (auto): k1_scan + k1_fit (H100, 100k-point sweep: 0.46 vs 0.75 ms per sweep for k1_fast in the same run, BASELINE.md)
 
-static int pass_grid(srl_ctx* ctx, long long n, int K, int nb) {
-    const long long n_groups = (n + 31) / 32;
-    long long want = n_groups;   // block-minor group assignment: one group per block first, then per warp
-    const long long resident = (long long)ctx->sm_count * k1_max_blocks_per_sm(K, nb);
-    if (want > resident) want = resident;
-    if (want < 1) want = 1;
-    if (want > ctx->max_grid) want = ctx->max_grid;
-    return (int)want;
-}
-
 }  // namespace srl
 
 using namespace srl;
@@ -213,9 +203,9 @@ static int ensure_order(srl_ctx* ctx, srl_sweep* sw) {
     if ((rc = ensure_buf(ctx, &sw->d_order, sw->capacity)) != SRL_OK) return rc;
     if (!sw->order_valid && sw->n > 0) {
         size_t need = 0;
-        sweep_compute_order(sw->d_raw, (long long)sw->n, sw->d_order, nullptr, 0, &need, ctx->stream);
+        sweep_compute_order(ctx->choice, sw->d_raw, (long long)sw->n, sw->d_order, nullptr, 0, &need, ctx->stream);
         if ((rc = ensure_scratch(ctx, need)) != SRL_OK) return rc;
-        SRL_CUDA(ctx, sweep_compute_order(sw->d_raw, (long long)sw->n, sw->d_order, ctx->d_scratch, ctx->scratch_bytes, &need, ctx->stream));
+        SRL_CUDA(ctx, sweep_compute_order(ctx->choice, sw->d_raw, (long long)sw->n, sw->d_order, ctx->d_scratch, ctx->scratch_bytes, &need, ctx->stream));
         sw->order_valid = true;
         ctx->launches += 1;
     }
@@ -231,15 +221,15 @@ static PassForm pass_form(const srl_ctx* ctx, const PassArgs& a) {
     return split ? PassForm::split : PassForm::fast;
 }
 // Everything a pass needs besides its kernel launches: buffers, the sweep's Morton order, cleared flags / candidate rows,
-// constant tables and (once per ctx) the kernels themselves; binds the sweep's buffers of the pass's form into `a`.
+// and (once per kernel choice) the kernels themselves; binds the sweep's buffers of the pass's form into `a`.
 // Idempotent.  The device-resident loop calls it BEFORE it launches the persistent ESIKF block: an allocation, a module
 // load (CUDA loads kernels lazily, and loading waits for running kernels) or a synchronous copy issued while that block
 // spins would deadlock against it.
 static int prepare_pass(srl_ctx* ctx, srl_sweep* sw, PassArgs& a) {
     if (!ctx->kernels_preloaded) {
         size_t max_local = 0;
-        SRL_CUDA(ctx, preload_fast_kernels(ctx->device, &max_local));
-        SRL_CUDA(ctx, preload_assoc_kernels(ctx->device, a.c.K, &max_local));
+        SRL_CUDA(ctx, preload_fast_kernels(ctx->choice, &max_local));
+        SRL_CUDA(ctx, preload_assoc_kernels(ctx->choice, a.c.K, &max_local));
         // The first launch of a kernel whose local memory (spills) exceeds the context's reservation makes the driver
         // grow that reservation, and the driver waits for the device to go idle to do it.  Launched behind the persistent
         // ESIKF block, which spins until the pass finishes, that wait never ends (k1_fast keeps a ~1.6 KB spill frame on
@@ -283,7 +273,7 @@ static int launch_pass(srl_ctx* ctx, srl_sweep* sw, PassArgs a, bool debug, bool
     }
     const PassForm form = pass_form(ctx, a);
     if (form == PassForm::assoc) {
-        SRL_CUDA(ctx, launch_k1(a, pass_grid(ctx, n, a.c.K, a.c.nb), debug, ctx->device, ctx->stream, pdl));
+        SRL_CUDA(ctx, launch_k1(ctx, a, n, debug, pdl));
         ctx->launches += 1;
     } else {
         PassArgs first = a;   // its sums go to d_fast_out; the range is one of SORTED positions unless the pass is capped
@@ -291,27 +281,43 @@ static int launch_pass(srl_ctx* ctx, srl_sweep* sw, PassArgs a, bool debug, bool
         if (form == PassForm::split) {
             // k1_fit finalises the pass itself when nothing was flagged (multi-GPU: after running the exchange); the
             // fallback launch then runs off the host's critical path and republishes the same values
-            SRL_CUDA(ctx, launch_k1_split(first, n, ctx->max_grid, debug, ctx->device, ctx->stream, pdl));
+            SRL_CUDA(ctx, launch_k1_split(ctx, first, n, debug, pdl));
             ctx->launches += 1;
         } else {
-            const long long kpw = 32 / k1_fast_lanes_per_keypoint();
-            const long long n_groups = (n + kpw - 1) / kpw;
-            // one group per warp when it fits (the block scheduler then balances the waves), grid-stride beyond that
-            long long grid = std::min<long long>((n_groups + kFastWarps - 1) / kFastWarps, (long long)ctx->max_grid);
-            grid = std::max<long long>(1, std::min<long long>(grid, ctx->max_grid));
-            SRL_CUDA(ctx, launch_k1_fast(first, (int)grid, debug, ctx->device, ctx->stream));
+            SRL_CUDA(ctx, launch_k1_fast(ctx, first, n, debug));
         }
         // exact selection for the keypoints the first launch could not decide; its last block adds the first launch's sums
         a.only_flagged = a.flags; a.prev_out32 = ctx->d_fast_out;
         if (a.order) { a.k_begin = 0; a.k_end = (long long)sw->n; }   // Morton order: the range's keypoints are scattered over the sweep
-        // almost always nothing is flagged: a one-block-per-SM grid walks the flags (32 per warp step) and leaves
-        const int fb_grid = (int)std::min<long long>(ctx->sm_count, std::max<long long>(1, ((long long)sw->n + 31) / 32));
-        SRL_CUDA(ctx, launch_k1(a, fb_grid, debug, ctx->device, ctx->stream, pdl));
+        SRL_CUDA(ctx, launch_k1(ctx, a, (long long)sw->n, debug, pdl));   // its grid covers the flags of the whole sweep
         ctx->launches += 2;
     }
     if (timing) { cudaEventRecord(ctx->ev1[ctx->ev_cur], ctx->stream); ctx->ev_pending[ctx->ev_cur] = true; }
     return SRL_OK;
 }
+
+// The integer options of srl_ctx_set_option: the values each accepts, where the ctx keeps it, and the environment variable
+// srl_ctx_create reads it from (a value outside the set leaves the default).  srl_ctx_get_counter reads each one back.
+struct IntOption {
+    const char* name;
+    std::vector<int> allowed;
+    int& (*field)(srl_ctx&);
+    const char* env;
+    const char* must_be;
+};
+static const IntOption kIntOptions[] = {
+    {"k1_variant", {0, 1, 2, 3}, [](srl_ctx& c) -> int& { return c.variant; }, nullptr,
+     "k1_variant must be 0 (auto), 1 (k1_fast), 2 (k1_assoc only) or 3 (k1_scan + k1_fit)"},
+    {"shuffle_rule", {0, 1}, [](srl_ctx& c) -> int& { return c.shuffle_rule; }, nullptr, "shuffle_rule must be 0 (Lemire) or 1 (division)"},
+    {"split_lanes_per_keypoint", {2, 4}, [](srl_ctx& c) -> int& { return c.choice.split_lpk; }, "SRL_SPLIT_LPK", "split_lanes_per_keypoint must be 2 or 4"},
+    {"scan_min_blocks", {6, 8}, [](srl_ctx& c) -> int& { return c.choice.scan_minb; }, "SRL_SCAN_MINB", "scan_min_blocks must be 6 or 8"},
+    {"fit_min_blocks", {4, 5, 6}, [](srl_ctx& c) -> int& { return c.choice.fit_minb; }, "SRL_FIT_MINB", "fit_min_blocks must be 4, 5 or 6"},
+    {"fast_lanes_per_keypoint", {1, 2, 4}, [](srl_ctx& c) -> int& { return c.choice.fast_lpk; }, "SRL_FAST_LPK", "fast_lanes_per_keypoint must be 1, 2 or 4"},
+    {"fast_min_blocks", {4, 5, 6, 8}, [](srl_ctx& c) -> int& { return c.choice.fast_minb; }, "SRL_FAST_MINB", "fast_min_blocks must be 4, 5, 6 or 8"},
+    {"k1_min_blocks", {2, 3, 4}, [](srl_ctx& c) -> int& { return c.choice.k1_minb; }, "SRL_K1_MINB", "k1_min_blocks must be 2, 3 or 4"},
+    {"cluster_order", {0, 1, 2, 3}, [](srl_ctx& c) -> int& { return c.choice.order_mode; }, "SRL_CLUSTER_ORDER", "cluster_order must be 0, 1, 2 or 3"},
+};
+static bool allowed(const IntOption& o, int64_t v) { return std::find(o.allowed.begin(), o.allowed.end(), v) != o.allowed.end(); }
 
 extern "C" {
 
@@ -361,7 +367,11 @@ int srl_ctx_create(int device, void* cuda_stream, srl_ctx** out) {
     std::memset(ctx->h_out32, 0, 64 * sizeof(double));
     std::memset(ctx->h_iekf, 0, sizeof(IekfHostOut));
     if (const char* e = getenv("SRL_DEVICE_LOOP")) ctx->device_loop = atoi(e) != 0;
-    if (const char* e = getenv("SRL_CLUSTER_ORDER")) sweep_order_set_impl(atoi(e));
+    for (const IntOption& o : kIntOptions) {
+        const char* e = o.env ? getenv(o.env) : nullptr;
+        if (e && allowed(o, atoi(e))) o.field(*ctx) = atoi(e);
+    }
+    ctx->choice.restart_order_checks();
     *out = ctx;
     return SRL_OK;
 }
@@ -395,37 +405,14 @@ int srl_ctx_set_option(srl_ctx* ctx, const char* name, int64_t value) {
     const std::string n(name);
     if (n == "force_exact_selection") { ctx->force_exact = value != 0; return SRL_OK; }
     if (n == "fast_force_ambiguous_mod") { ctx->force_amb_mod = (int)value; return SRL_OK; }
-    if (n == "fast_lanes_per_keypoint") {
-        if (value != 1 && value != 2 && value != 4) return set_err(ctx, SRL_BAD_ARG, "fast_lanes_per_keypoint must be 1, 2 or 4");
-        k1_fast_set_lanes_per_keypoint((int)value);
-        return SRL_OK;
-    }
     if (n == "device_loop") { ctx->device_loop = value != 0; return SRL_OK; }
-    if (n == "shuffle_rule") {
-        if (value != 0 && value != 1) return set_err(ctx, SRL_BAD_ARG, "shuffle_rule must be 0 (Lemire) or 1 (division)");
-        ctx->shuffle_rule = (int)value;
-        return SRL_OK;
-    }
     if (n == "shuffle_on_host") { ctx->shuffle_on_host = value != 0; return SRL_OK; }
-    if (n == "cluster_order") { sweep_order_set_impl((int)value); return SRL_OK; }   // process-wide
-    if (n == "split_lanes_per_keypoint") {
-        if (value != 2 && value != 4) return set_err(ctx, SRL_BAD_ARG, "split_lanes_per_keypoint must be 2 or 4");
-        k1_split_set_lanes_per_keypoint((int)value);
-        return SRL_OK;
-    }
-    if (n == "fast_min_blocks") {
-        if (value != 4 && value != 5 && value != 6 && value != 8) return set_err(ctx, SRL_BAD_ARG, "fast_min_blocks must be 4, 5, 6 or 8");
-        k1_fast_set_min_blocks((int)value);
-        return SRL_OK;
-    }
-    if (n == "k1_variant") {
-        if (value < 0 || value > 3) return set_err(ctx, SRL_BAD_ARG, "k1_variant must be 0 (auto), 1 (k1_fast), 2 (k1_assoc only) or 3 (k1_scan + k1_fit)");
-        ctx->variant = (int)value;
-        return SRL_OK;
-    }
-    if (n == "k1_min_blocks") {
-        if (value != 2 && value != 3 && value != 4) return set_err(ctx, SRL_BAD_ARG, "k1_min_blocks must be 2, 3 or 4");
-        k1_set_min_blocks((int)value);
+    for (const IntOption& o : kIntOptions) {
+        if (n != o.name) continue;
+        if (!allowed(o, value)) return set_err(ctx, SRL_BAD_ARG, o.must_be);
+        o.field(*ctx) = (int)value;
+        if (n == "cluster_order") ctx->choice.restart_order_checks();
+        ctx->kernels_preloaded = false;   // the next pass loads the instances of the choice (before any persistent block spins)
         return SRL_OK;
     }
     return set_err(ctx, SRL_BAD_ARG, "unknown option " + n);
@@ -460,7 +447,9 @@ int srl_ctx_get_counter(srl_ctx* ctx, const char* name, int64_t* value) {
     }
     if (n == "kernel_launches") { *value = ctx->launches; return SRL_OK; }
     if (n.rfind("iekf_stage_", 0) == 0 && n.size() == 12 && n[11] >= '0' && n[11] <= '7') { *value = ctx->h_iekf->stage_cycles[n[11] - '0']; return SRL_OK; }
-    if (n == "cluster_order_active") { *value = sweep_order_impl(); return SRL_OK; }
+    if (n == "cluster_order_active") { *value = ctx->choice.order_state; return SRL_OK; }
+    for (const IntOption& o : kIntOptions)
+        if (n == o.name) { *value = o.field(*ctx); return SRL_OK; }
     if (n == "device_loop_active") { *value = device_loop_usable(ctx) ? 1 : 0; return SRL_OK; }
     if (n == "iekf_step_cycles_avg") {   // device-resident loop: average SM clock ticks of one ESIKF step (resets on read)
         *value = ctx->step_cycles_n ? (int64_t)(ctx->step_cycles_sum / (double)ctx->step_cycles_n) : 0;

@@ -20,13 +20,13 @@
 //
 // The 32-double result block: [0..20] HTH upper triangle (row-major a<=b), [21..26] H^T h, [27] sum d^2,
 // [28] residuals, [29] keypoints with a full neighbourhood, [30] map points scanned, [31] NaN-planarity count.
-#include <cstdlib>
+#include <algorithm>
 
 #include "srl_internal.h"
 
 namespace srl {
 
-__constant__ signed char c_off[125 * 4];   // voxel offsets ordered by |offset|^2; first 27 = the nb=1 cube
+__constant__ VoxelOffsets<125> c_off = voxel_offsets<125>();   // voxel offsets ordered by |offset|^2; first 27 = the nb=1 cube
 
 constexpr unsigned FULL = 0xffffffffu;
 constexpr int NBS = 33;   // padded stride of the per-warp neighbour tile (bank-conflict free both ways)
@@ -648,87 +648,47 @@ __global__ void k_transform(const double* __restrict__ raw, long long n, PassCon
 // ---------------------------------------------------------------------------------------------
 // host launchers
 // ---------------------------------------------------------------------------------------------
-static bool g_off_uploaded[64] = {false};
-
-static void upload_offsets(int device) {
-    if (device >= 0 && device < 64 && g_off_uploaded[device]) return;
-    // all 125 offsets of the 5x5x5 cube ordered by squared norm; the 27 with |.|inf <= 1 come first
-    signed char tab[125 * 4];
-    int n = 0;
-    for (int pass = 0; pass < 2; ++pass)
-        for (int d2 = 0; d2 <= 12; ++d2)
-            for (int x = -2; x <= 2; ++x)
-                for (int y = -2; y <= 2; ++y)
-                    for (int z = -2; z <= 2; ++z) {
-                        const bool inner = x >= -1 && x <= 1 && y >= -1 && y <= 1 && z >= -1 && z <= 1;
-                        if ((pass == 0) != inner) continue;
-                        if (x * x + y * y + z * z != d2) continue;
-                        tab[4 * n] = (signed char)x; tab[4 * n + 1] = (signed char)y; tab[4 * n + 2] = (signed char)z; tab[4 * n + 3] = 0;
-                        ++n;
-                    }
-    cudaMemcpyToSymbol(c_off, tab, sizeof(tab));
-    if (device >= 0 && device < 64) g_off_uploaded[device] = true;
-}
-
-size_t k1_smem_bytes(int K) { return (size_t)kK1Warps * ((size_t)(K * NBS) * sizeof(unsigned) + 128 * sizeof(int)); }
+static size_t k1_smem_bytes(int K) { return (size_t)kK1Warps * ((size_t)(K * NBS) * sizeof(unsigned) + 128 * sizeof(int)); }
 
 typedef void (*K1Fn)(const PassArgs);
-static int g_minb = -1;
-void k1_set_min_blocks(int v) { if (v == 2 || v == 3 || v == 4) g_minb = v; }
-int k1_min_blocks() {   // resident blocks per SM the kernel is compiled for; SRL_K1_MINB=2|3|4 selects the variant
-    if (g_minb < 0) {
-        const char* e = getenv("SRL_K1_MINB");
-        int v = e ? atoi(e) : 3;
-        g_minb = (v == 2 || v == 3 || v == 4) ? v : 3;
-    }
-    return g_minb;
-}
-template <int NCH, bool DBG>
-static K1Fn pick_minb() {
-    switch (k1_min_blocks()) {
-        case 2: return k1_assoc<NCH, DBG, 2>;
-        case 4: return k1_assoc<NCH, DBG, 4>;
-        default: return k1_assoc<NCH, DBG, 3>;
-    }
-}
-static K1Fn pick_k1(int nb, bool debug) {
-    if (nb <= 1) return debug ? pick_minb<1, true>() : pick_minb<1, false>();
-    return debug ? pick_minb<4, true>() : pick_minb<4, false>();
+// The compiled k1_assoc instances: NCH = 1 for voxel_neighborhood <= 1, 4 for nb = 2, by k1_min_blocks.
+struct AssocInstance { int nch, minb; K1Fn fn, dbg; };
+static const AssocInstance kAssoc[] = {
+    {1, 2, k1_assoc<1, false, 2>, k1_assoc<1, true, 2>}, {1, 3, k1_assoc<1, false, 3>, k1_assoc<1, true, 3>},
+    {1, 4, k1_assoc<1, false, 4>, k1_assoc<1, true, 4>}, {4, 2, k1_assoc<4, false, 2>, k1_assoc<4, true, 2>},
+    {4, 3, k1_assoc<4, false, 3>, k1_assoc<4, true, 3>}, {4, 4, k1_assoc<4, false, 4>, k1_assoc<4, true, 4>}};
+static K1Fn pick_assoc(const KernelChoice& ch, int nb, bool debug) {
+    const int nch = nb <= 1 ? 1 : 4;
+    for (const AssocInstance& i : kAssoc)
+        if (i.nch == nch && i.minb == ch.k1_minb) return debug ? i.dbg : i.fn;
+    return nullptr;
 }
 
-cudaError_t launch_k1(const PassArgs& a, int grid, bool debug, int device, cudaStream_t stream, bool pdl) {
-    upload_offsets(device);
+// One 32-keypoint group per block, up to the blocks of the non-debug instance that are resident at once (grid-stride
+// beyond).  The fallback launch (a.only_flagged) almost always finds nothing flagged: one block per SM walks the flags
+// (32 per warp step) and leaves.
+cudaError_t launch_k1(const srl_ctx* ctx, const PassArgs& a, long long n, bool debug, bool pdl) {
     const size_t smem = k1_smem_bytes(a.c.K);
-    K1Fn fn = pick_k1(a.c.nb, debug);
+    const K1Fn fn = pick_assoc(ctx->choice, a.c.nb, debug), product = pick_assoc(ctx->choice, a.c.nb, false);
+    if (!fn) return cudaErrorInvalidDeviceFunction;
     cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e == cudaSuccess && product != fn) e = cudaFuncSetAttribute(product, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
-    return launch_pass_kernel(fn, a, (unsigned)grid, kK1Threads, smem, stream, pdl);
+    int per_sm = 1;
+    if (!a.only_flagged && (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, product, kK1Threads, smem) != cudaSuccess || per_sm < 1)) per_sm = 1;
+    const long long grid = std::max<long long>(1, std::min<long long>({(n + 31) / 32, (long long)ctx->sm_count * per_sm, ctx->max_grid}));
+    return launch_pass_kernel(fn, a, (unsigned)grid, kK1Threads, smem, ctx->stream, pdl);
 }
 
-cudaError_t preload_assoc_kernels(int device, int K, size_t* max_local) {
-    upload_offsets(device);
-    cudaFuncAttributes at;
+cudaError_t preload_assoc_kernels(const KernelChoice& ch, int K, size_t* max_local) {
     const size_t smem = k1_smem_bytes(K > 0 ? K : 20);
     for (int nb = 1; nb <= 2; ++nb) {
-        K1Fn fn = pick_k1(nb, false);
-        cudaError_t e = cudaFuncGetAttributes(&at, fn);
+        const K1Fn fn = pick_assoc(ch, nb, false);
+        cudaError_t e = preload_kernel((const void*)fn, max_local);
         if (e == cudaSuccess) e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
-        if (at.localSizeBytes > *max_local) *max_local = at.localSizeBytes;
     }
-    cudaError_t e = cudaFuncGetAttributes(&at, k2_cap_reduce);   // the capped pass's reduction runs behind the ESIKF block too
-    if (e != cudaSuccess) return e;
-    if (at.localSizeBytes > *max_local) *max_local = at.localSizeBytes;
-    return cudaSuccess;
-}
-
-int k1_max_blocks_per_sm(int K, int nb) {
-    int nblk = 0;
-    K1Fn fn = pick_k1(nb, false);
-    const size_t smem = k1_smem_bytes(K);
-    cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nblk, fn, kK1Threads, smem) != cudaSuccess) return 1;
-    return nblk < 1 ? 1 : nblk;
+    return preload_kernel((const void*)k2_cap_reduce, max_local);   // the capped pass's reduction runs behind the ESIKF block too
 }
 
 cudaError_t launch_k2(const K2Args& a, cudaStream_t stream, bool pdl) {

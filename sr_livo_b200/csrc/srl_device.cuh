@@ -45,6 +45,31 @@ __host__ __device__ __forceinline__ unsigned int hash_key(int x, int y, int z) {
     return h;
 }
 
+// The order in which the pass kernels visit the voxels around a keypoint's voxel: first the 27 offsets with |.|inf <= 1,
+// then the other 98 of the 5x5x5 cube, each part by squared norm, then x, y, z ascending.  N = 125 is k1_assoc's table
+// (c_off), N = 27 the nb <= 1 table of k1_fast / k1_scan / k1_fit (c_off_fast).  Entry i is (x, y, z, 0) at [4i, 4i + 4).
+template <int N>
+struct VoxelOffsets {
+    signed char v[4 * N];
+    __host__ __device__ constexpr signed char operator[](int i) const { return v[i]; }
+};
+template <int N>
+constexpr VoxelOffsets<N> voxel_offsets() {
+    VoxelOffsets<N> t{};
+    int n = 0;
+    for (int outer = 0; outer <= 1; ++outer)
+        for (int d2 = 0; d2 <= 12; ++d2)
+            for (int x = -2; x <= 2; ++x)
+                for (int y = -2; y <= 2; ++y)
+                    for (int z = -2; z <= 2; ++z) {
+                        const bool inner = x >= -1 && x <= 1 && y >= -1 && y <= 1 && z >= -1 && z <= 1;
+                        if (inner == (outer == 1) || x * x + y * y + z * z != d2 || n == N) continue;
+                        t.v[4 * n] = (signed char)x; t.v[4 * n + 1] = (signed char)y; t.v[4 * n + 2] = (signed char)z;
+                        ++n;
+                    }
+    return t;
+}
+
 #if defined(__CUDACC__)
 // read-only probe (query kernels): linear probing, one 16-byte load per step
 __device__ __forceinline__ bool map_find(const Slot* __restrict__ slots, unsigned int mask, int x, int y, int z,

@@ -19,7 +19,6 @@
 // Handles voxel_neighborhood <= 1 and max/min_number_neighbors == 20 (every reference config outside the first
 // 20 init frames); anything else goes to k1_assoc alone.
 #include <algorithm>
-#include <cstdlib>
 
 #include <cooperative_groups.h>
 #include <cub/cub.cuh>
@@ -28,7 +27,7 @@
 
 namespace srl {
 
-__constant__ signed char c_off_fast[27 * 4];   // the 27 offsets of the nb<=1 cube ordered by |offset|^2 (centre first)
+__constant__ VoxelOffsets<27> c_off_fast = voxel_offsets<27>();   // the 27 offsets of the nb<=1 cube ordered by |offset|^2 (centre first)
 
 constexpr unsigned FULLM = 0xffffffffu;
 constexpr int KF = 20;            // neighbours kept by the fast path
@@ -1328,24 +1327,24 @@ __global__ void k_order_mismatch(const unsigned* __restrict__ a, const unsigned*
 
 // scratch needs 3 * n * 4 bytes (aligned); returns cudaErrorNotSupported when no cluster size is launchable or n exceeds
 // what the cluster holds in registers (16 CTAs: 131072 keys, 8 CTAs: 65536) -- the caller then uses CUB
-static int s_cluster = 0;   // 0: not decided yet; -1: unsupported; else the cluster size in use
-static int g_order_variant = 3;   // 3: keys in registers + CTA-local digit order before the stores; 2: registers, direct scatter; 1: first version
-static long long sweep_cluster_capacity() { return s_cluster < 0 ? 0 : (long long)(s_cluster > 0 ? s_cluster : 16) * kSortKeysPerCta; }
-static cudaError_t sweep_order_cluster(const double* d_raw, long long n, unsigned* d_order, void* scratch, cudaStream_t stream) {
+static long long sweep_cluster_capacity(const KernelChoice& ch) {
+    return ch.cluster_size < 0 ? 0 : (long long)(ch.cluster_size > 0 ? ch.cluster_size : 16) * kSortKeysPerCta;
+}
+static cudaError_t sweep_order_cluster(KernelChoice& ch, const double* d_raw, long long n, unsigned* d_order, void* scratch, cudaStream_t stream) {
     auto al = [](size_t x) { return (x + 255) / 256 * 256; };
     char* p = static_cast<char*>(scratch);
     unsigned* ka = reinterpret_cast<unsigned*>(p); p += al(n * 4);
     unsigned* kb = reinterpret_cast<unsigned*>(p); p += al(n * 4);
     unsigned* ia = reinterpret_cast<unsigned*>(p);
-    if (s_cluster < 0) return cudaErrorNotSupported;
+    if (ch.cluster_size < 0) return cudaErrorNotSupported;
     const int sizes[2] = {16, 8};
     for (int t = 0; t < 2; ++t) {
-        const int cs = s_cluster > 0 ? s_cluster : sizes[t];
+        const int cs = ch.cluster_size > 0 ? ch.cluster_size : sizes[t];
         if (n > (long long)cs * kSortKeysPerCta) {
-            if (s_cluster > 0) return cudaErrorNotSupported;   // this sweep is too long; the kernel stays in use for shorter ones
+            if (ch.cluster_size > 0) return cudaErrorNotSupported;   // this sweep is too long; the kernel stays in use for shorter ones
             continue;
         }
-        if (s_cluster == 0) {   // first launch: opt in to the 16-CTA cluster and to the staging buffer
+        if (ch.cluster_size == 0) {   // first launch: opt in to the 16-CTA cluster and to the staging buffer
             if (cs > 8 && (cudaFuncSetAttribute(k_sweep_order_cluster<true>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess ||
                            cudaFuncSetAttribute(k_sweep_order_cluster<false>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess ||
                            cudaFuncSetAttribute(k_sweep_order_cluster_v1, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess)) { cudaGetLastError(); continue; }
@@ -1358,55 +1357,23 @@ static cudaError_t sweep_order_cluster(const double* d_raw, long long n, unsigne
         at[0].val.clusterDim.x = (unsigned)cs; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
         cfg.attrs = at; cfg.numAttrs = 1;
         cudaError_t e;
-        if (g_order_variant == 1) e = cudaLaunchKernelEx(&cfg, k_sweep_order_cluster_v1, d_raw, n, 1.0, ka, ia, kb, d_order);
-        else if (g_order_variant == 2) e = cudaLaunchKernelEx(&cfg, k_sweep_order_cluster<false>, d_raw, (int)n, 1.0, ka, ia, kb, d_order);
-        else {
+        if (ch.order_mode == 3) e = cudaLaunchKernelEx(&cfg, k_sweep_order_cluster_v1, d_raw, n, 1.0, ka, ia, kb, d_order);
+        else if (ch.order_mode == 2) e = cudaLaunchKernelEx(&cfg, k_sweep_order_cluster<false>, d_raw, (int)n, 1.0, ka, ia, kb, d_order);
+        else {   // keys in registers + CTA-local digit order before the stores
             cfg.dynamicSmemBytes = 2 * kSortKeysPerCta * sizeof(unsigned);
             e = cudaLaunchKernelEx(&cfg, k_sweep_order_cluster<true>, d_raw, (int)n, 1.0, ka, ia, kb, d_order);
         }
-        if (e == cudaSuccess) { s_cluster = cs; return cudaSuccess; }
+        if (e == cudaSuccess) { ch.cluster_size = cs; return cudaSuccess; }
         cudaGetLastError();
-        if (s_cluster > 0) break;
+        if (ch.cluster_size > 0) break;
     }
-    s_cluster = -1;
+    ch.cluster_size = -1;
     return cudaErrorNotSupported;
 }
 
-static int g_order_impl = -1;   // -1: cluster kernel, still being verified against CUB; 1: cluster kernel (verified); 0: CUB
-static int g_order_checks_left = 4;   // the first uses in a process run both sorts and compare the orders on the device
-void sweep_order_set_impl(int v) { g_order_impl = v ? -1 : 0; g_order_checks_left = 4; if (v >= 1 && v <= 3) g_order_variant = v == 1 ? 3 : (v == 2 ? 2 : 1); }   // 1 default kernel, 2/3 the earlier variants
-int sweep_order_impl() { return g_order_impl; }
-
-cudaError_t sweep_compute_order(const double* d_raw, long long n, unsigned* d_order, void* scratch, size_t scratch_bytes,
-                                size_t* needed, cudaStream_t stream) {
+// CUB's radix sort of the keys; scratch: three n-word arrays, then CUB's `tmp` bytes
+static cudaError_t sweep_order_cub(const double* d_raw, long long n, unsigned* d_order, void* scratch, size_t tmp, cudaStream_t stream) {
     auto al = [](size_t x) { return (x + 255) / 256 * 256; };
-    size_t tmp = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, tmp, (unsigned*)nullptr, (unsigned*)nullptr, (unsigned*)nullptr, (unsigned*)nullptr, (int)n, 0, 24, stream);
-    const size_t need = al(n * 4) * 4 + al(tmp) + 256;
-    if (needed) *needed = need;
-    if (!scratch || scratch_bytes < need) return cudaSuccess;
-    if (g_order_impl != 0 && n <= sweep_cluster_capacity()) {
-        if (g_order_impl == 1) {
-            if (sweep_order_cluster(d_raw, n, d_order, scratch, stream) == cudaSuccess) return cudaSuccess;
-            if (s_cluster < 0) g_order_impl = 0;   // else: only this sweep is too long for the cluster
-        } else {
-            // first uses: run both, compare on the device, keep the cluster kernel only if the orders are identical
-            char* q = static_cast<char*>(scratch) + al(n * 4) * 3 + al(tmp);
-            unsigned* ref = reinterpret_cast<unsigned*>(q);                      // the 4th n-word array
-            unsigned* cnt = reinterpret_cast<unsigned*>(q + al(n * 4));
-            g_order_impl = 0;
-            cudaError_t e = sweep_compute_order(d_raw, n, ref, scratch, scratch_bytes, nullptr, stream);   // CUB (first 3 arrays + its temp) into `ref`
-            if (e != cudaSuccess) return e;
-            unsigned mism = 1u;
-            if (sweep_order_cluster(d_raw, n, d_order, scratch, stream) == cudaSuccess) {
-                cudaMemsetAsync(cnt, 0, 4, stream);
-                k_order_mismatch<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(d_order, ref, n, cnt);
-                if (cudaMemcpyAsync(&mism, cnt, 4, cudaMemcpyDeviceToHost, stream) != cudaSuccess || cudaStreamSynchronize(stream) != cudaSuccess) { cudaGetLastError(); mism = 1u; }
-            }
-            if (mism == 0u) { g_order_impl = --g_order_checks_left > 0 ? -1 : 1; return cudaSuccess; }
-            return cudaMemcpyAsync(d_order, ref, (size_t)n * 4, cudaMemcpyDeviceToDevice, stream);   // keep CUB's order, and CUB from now on
-        }
-    }
     char* p = static_cast<char*>(scratch);
     unsigned* ka = reinterpret_cast<unsigned*>(p); p += al(n * 4);
     unsigned* kb = reinterpret_cast<unsigned*>(p); p += al(n * 4);
@@ -1418,112 +1385,107 @@ cudaError_t sweep_compute_order(const double* d_raw, long long n, unsigned* d_or
     return cub::DeviceRadixSort::SortPairs(p, tmp, ka, kb, ia, d_order, (int)n, 0, 24, stream);
 }
 
+cudaError_t sweep_compute_order(KernelChoice& ch, const double* d_raw, long long n, unsigned* d_order, void* scratch,
+                                size_t scratch_bytes, size_t* needed, cudaStream_t stream) {
+    auto al = [](size_t x) { return (x + 255) / 256 * 256; };
+    size_t tmp = 0;
+    cub::DeviceRadixSort::SortPairs(nullptr, tmp, (unsigned*)nullptr, (unsigned*)nullptr, (unsigned*)nullptr, (unsigned*)nullptr, (int)n, 0, 24, stream);
+    const size_t need = al(n * 4) * 4 + al(tmp) + 256;
+    if (needed) *needed = need;
+    if (!scratch || scratch_bytes < need) return cudaSuccess;
+    if (ch.order_state != 0 && n <= sweep_cluster_capacity(ch)) {
+        if (ch.order_state == 1) {
+            if (sweep_order_cluster(ch, d_raw, n, d_order, scratch, stream) == cudaSuccess) return cudaSuccess;
+            if (ch.cluster_size < 0) ch.order_state = 0;   // else: only this sweep is too long for the cluster
+        } else {
+            // first uses: run both, compare on the device, keep the cluster kernel only if the orders are identical
+            char* q = static_cast<char*>(scratch) + al(n * 4) * 3 + al(tmp);
+            unsigned* ref = reinterpret_cast<unsigned*>(q);                      // the 4th n-word array
+            unsigned* cnt = reinterpret_cast<unsigned*>(q + al(n * 4));
+            ch.order_state = 0;
+            cudaError_t e = sweep_order_cub(d_raw, n, ref, scratch, tmp, stream);
+            if (e != cudaSuccess) return e;
+            unsigned mism = 1u;
+            if (sweep_order_cluster(ch, d_raw, n, d_order, scratch, stream) == cudaSuccess) {
+                cudaMemsetAsync(cnt, 0, 4, stream);
+                k_order_mismatch<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(d_order, ref, n, cnt);
+                if (cudaMemcpyAsync(&mism, cnt, 4, cudaMemcpyDeviceToHost, stream) != cudaSuccess || cudaStreamSynchronize(stream) != cudaSuccess) { cudaGetLastError(); mism = 1u; }
+            }
+            if (mism == 0u) { ch.order_state = --ch.order_checks_left > 0 ? -1 : 1; return cudaSuccess; }
+            return cudaMemcpyAsync(d_order, ref, (size_t)n * 4, cudaMemcpyDeviceToDevice, stream);   // keep CUB's order, and CUB from now on
+        }
+    }
+    return sweep_order_cub(d_raw, n, d_order, scratch, tmp, stream);
+}
+
 // ---------------------------------------------------------------------------------------------------------
-static bool g_fast_off_uploaded[64] = {false};
-static void upload_fast_offsets(int device) {
-    if (device >= 0 && device < 64 && g_fast_off_uploaded[device]) return;
-    signed char tab[27 * 4];
-    int n = 0;
-    for (int d2 = 0; d2 <= 3; ++d2)
-        for (int x = -1; x <= 1; ++x)
-            for (int y = -1; y <= 1; ++y)
-                for (int z = -1; z <= 1; ++z) {
-                    if (x * x + y * y + z * z != d2) continue;
-                    tab[4 * n] = (signed char)x; tab[4 * n + 1] = (signed char)y; tab[4 * n + 2] = (signed char)z; tab[4 * n + 3] = 0;
-                    ++n;
-                }
-    cudaMemcpyToSymbol(c_off_fast, tab, sizeof(tab));
-    if (device >= 0 && device < 64) g_fast_off_uploaded[device] = true;
-}
-
+// The compiled instances of the fast and split forms, keyed by the KernelChoice fields that select them.  Debug instances
+// are loaded lazily at their first launch: only srl_build_plane_residuals asks for debug outputs, and it drives its pass
+// from the host, so no persistent ESIKF block can be spinning while one loads.
 typedef void (*FastFn)(const PassArgs);
-static int g_fast_minb = -1, g_fast_lpk = -1;
-void k1_fast_set_min_blocks(int v) { if (v == 4 || v == 5 || v == 6 || v == 8) g_fast_minb = v; }
-void k1_fast_set_lanes_per_keypoint(int v) { if (v == 1 || v == 2 || v == 4) g_fast_lpk = v; }
-static int fast_minb() {   // SRL_FAST_MINB=4|5|6|8 selects the compiled variant (default 5)
-    if (g_fast_minb < 0) {
-        const char* e = getenv("SRL_FAST_MINB");
-        const int v = e ? atoi(e) : 5;
-        g_fast_minb = (v == 4 || v == 5 || v == 6 || v == 8) ? v : 5;
-    }
-    return g_fast_minb;
+struct FastInstance { int minb, lpk; FastFn fn, dbg; };
+static const FastInstance kFast[] = {
+    {4, 1, k1_fast<false, 4, 2, 1>, k1_fast<true, 4, 2, 1>}, {4, 2, k1_fast<false, 4, 2, 2>, k1_fast<true, 4, 2, 2>},
+    {4, 4, k1_fast<false, 4, 2, 4>, k1_fast<true, 4, 2, 4>}, {5, 1, k1_fast<false, 5, 2, 1>, k1_fast<true, 5, 2, 1>},
+    {5, 2, k1_fast<false, 5, 2, 2>, k1_fast<true, 5, 2, 2>}, {5, 4, k1_fast<false, 5, 2, 4>, k1_fast<true, 5, 2, 4>},
+    {6, 1, k1_fast<false, 6, 2, 1>, k1_fast<true, 6, 2, 1>}, {6, 2, k1_fast<false, 6, 2, 2>, k1_fast<true, 6, 2, 2>},
+    {6, 4, k1_fast<false, 6, 2, 4>, k1_fast<true, 6, 2, 4>}, {8, 1, k1_fast<false, 8, 2, 1>, k1_fast<true, 8, 2, 1>},
+    {8, 2, k1_fast<false, 8, 2, 2>, k1_fast<true, 8, 2, 2>}, {8, 4, k1_fast<false, 8, 2, 4>, k1_fast<true, 8, 2, 4>}};
+struct ScanInstance { int lpk, minb; FastFn fn; };
+static const ScanInstance kScan[] = {
+    {4, 8, k1_scan<4, 14, 8>}, {4, 6, k1_scan<4, 14, 6>}, {2, 8, k1_scan<2, 20, 8>}, {2, 6, k1_scan<2, 20, 6>}};
+struct FitInstance { int minb; FastFn fn; };
+static const FitInstance kFit[] = {{4, k1_fit<false, 4>}, {5, k1_fit<false, 5>}, {6, k1_fit<false, 6>}};
+static const FastFn kFitDebug = k1_fit<true, 4>;
+
+static FastFn pick_fast(const KernelChoice& ch, bool debug) {
+    for (const FastInstance& i : kFast)
+        if (i.minb == ch.fast_minb && i.lpk == ch.fast_lpk) return debug ? i.dbg : i.fn;
+    return nullptr;
 }
-int k1_fast_lanes_per_keypoint() {     // SRL_FAST_LPK=1|2|4 (default 1)
-    if (g_fast_lpk < 0) {
-        const char* e = getenv("SRL_FAST_LPK");
-        const int v = e ? atoi(e) : 1;
-        g_fast_lpk = (v == 1 || v == 2 || v == 4) ? v : 1;
-    }
-    return g_fast_lpk;
+static FastFn pick_scan(const KernelChoice& ch) {
+    for (const ScanInstance& i : kScan)
+        if (i.lpk == ch.split_lpk && i.minb == ch.scan_minb) return i.fn;
+    return nullptr;
 }
-template <bool DBG, int LPK>
-static FastFn pick_fast_mb() {
-    switch (fast_minb()) {
-        case 4: return k1_fast<DBG, 4, 2, LPK>;
-        case 6: return k1_fast<DBG, 6, 2, LPK>;
-        case 8: return k1_fast<DBG, 8, 2, LPK>;
-        default: return k1_fast<DBG, 5, 2, LPK>;
-    }
-}
-template <bool DBG>
-static FastFn pick_fast() {
-    switch (k1_fast_lanes_per_keypoint()) {
-        case 1: return pick_fast_mb<DBG, 1>();
-        case 4: return pick_fast_mb<DBG, 4>();
-        default: return pick_fast_mb<DBG, 2>();
-    }
+static FastFn pick_fit(const KernelChoice& ch, bool debug) {
+    if (debug) return kFitDebug;
+    for (const FitInstance& i : kFit)
+        if (i.minb == ch.fit_minb) return i.fn;
+    return nullptr;
 }
 
-cudaError_t launch_k1_fast(const PassArgs& a, int grid, bool debug, int device, cudaStream_t stream) {
-    upload_fast_offsets(device);
-    FastFn fn = debug ? pick_fast<true>() : pick_fast<false>();
-    fn<<<grid, kFastThreads, 0, stream>>>(a);
+// one group of 32 / lanes-per-keypoint keypoints per warp when it fits (the block scheduler then balances the waves),
+// grid-stride beyond that
+cudaError_t launch_k1_fast(const srl_ctx* ctx, const PassArgs& a, long long n, bool debug) {
+    const FastFn fn = pick_fast(ctx->choice, debug);
+    if (!fn) return cudaErrorInvalidDeviceFunction;
+    const long long kpw = 32 / ctx->choice.fast_lpk;
+    const long long n_groups = (n + kpw - 1) / kpw;
+    const long long grid = std::max<long long>(1, std::min<long long>((n_groups + kFastWarps - 1) / kFastWarps, ctx->max_grid));
+    fn<<<(unsigned)grid, kFastThreads, 0, ctx->stream>>>(a);
     return cudaGetLastError();
 }
 
-static int g_split_lpk = -1;
-void k1_split_set_lanes_per_keypoint(int v) { if (v == 2 || v == 4) g_split_lpk = v; }
-static int env_int(const char* name, int dflt) { const char* e = getenv(name); return e ? atoi(e) : dflt; }
-
-// k1_scan then k1_fit on the same stream.  SRL_SPLIT_LPK=2|4 (lanes per keypoint), SRL_SCAN_MINB / SRL_FIT_MINB pick
-// the compiled register budgets.
-cudaError_t launch_k1_split(const PassArgs& a, long long n, int max_grid, bool debug, int device, cudaStream_t stream, bool pdl) {
-    upload_fast_offsets(device);
-    if (g_split_lpk < 0) { const int v = env_int("SRL_SPLIT_LPK", 4); g_split_lpk = (v == 2) ? 2 : 4; }
-    static const int scan_minb = env_int("SRL_SCAN_MINB", 8), fit_minb = env_int("SRL_FIT_MINB", 6);
-    const long long kpw = 32 / g_split_lpk;
+// k1_scan then k1_fit on the same stream
+cudaError_t launch_k1_split(const srl_ctx* ctx, const PassArgs& a, long long n, bool debug, bool pdl) {
+    const FastFn scan = pick_scan(ctx->choice), fit = pick_fit(ctx->choice, debug);
+    if (!scan || !fit) return cudaErrorInvalidDeviceFunction;
+    const long long kpw = 32 / ctx->choice.split_lpk;
     const long long n_groups = (n + kpw - 1) / kpw;
     const long long grid_a = std::max<long long>(1, std::min<long long>((n_groups + 3) / 4, 1 << 20));
-    FastFn scan;
-    if (g_split_lpk == 4) scan = scan_minb == 6 ? k1_scan<4, 14, 6> : k1_scan<4, 14, 8>;
-    else scan = scan_minb == 6 ? k1_scan<2, 20, 6> : k1_scan<2, 20, 8>;
-    cudaError_t e = launch_pass_kernel(scan, a, (unsigned)grid_a, kScanThreads, 0, stream, pdl);
+    cudaError_t e = launch_pass_kernel(scan, a, (unsigned)grid_a, kScanThreads, 0, ctx->stream, pdl);
     if (e != cudaSuccess) return e;
-    const long long grid_b = std::max<long long>(1, std::min<long long>(((n + 31) / 32 + kFastWarps - 1) / kFastWarps, max_grid));
-    FastFn fit;
-    if (debug) fit = k1_fit<true, 4>;
-    else fit = fit_minb == 6 ? k1_fit<false, 6> : (fit_minb == 4 ? k1_fit<false, 4> : k1_fit<false, 5>);
-    return launch_pass_kernel(fit, a, (unsigned)grid_b, kFastThreads, 0, stream, pdl);
+    const long long grid_b = std::max<long long>(1, std::min<long long>(((n + 31) / 32 + kFastWarps - 1) / kFastWarps, ctx->max_grid));
+    return launch_pass_kernel(fit, a, (unsigned)grid_b, kFastThreads, 0, ctx->stream, pdl);
 }
 
-cudaError_t preload_fast_kernels(int device, size_t* max_local) {
-    upload_fast_offsets(device);
-    cudaFuncAttributes at;
-    const FastFn fns[] = {k1_scan<4, 14, 8>, k1_scan<4, 14, 6>, k1_scan<2, 20, 8>, k1_scan<2, 20, 6>,
-                          k1_fit<false, 4>, k1_fit<false, 5>, k1_fit<false, 6>,
-                          pick_fast_mb<false, 1>(), pick_fast_mb<false, 2>(), pick_fast_mb<false, 4>()};
-    for (FastFn fn : fns) {
-        const cudaError_t e = cudaFuncGetAttributes(&at, fn);
+cudaError_t preload_fast_kernels(const KernelChoice& ch, size_t* max_local) {
+    for (const FastFn fn : {pick_scan(ch), pick_fit(ch, false), pick_fast(ch, false)}) {
+        const cudaError_t e = preload_kernel((const void*)fn, max_local);
         if (e != cudaSuccess) return e;
-        if (at.localSizeBytes > *max_local) *max_local = at.localSizeBytes;
     }
     return cudaSuccess;
-}
-
-int k1_fast_max_blocks_per_sm() {
-    int nblk = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nblk, pick_fast<false>(), kFastThreads, 0) != cudaSuccess) return 1;
-    return nblk < 1 ? 1 : nblk;
 }
 
 }  // namespace srl

@@ -311,13 +311,29 @@ __device__ __forceinline__ void finalise_pass(const PassArgs& A, bool forward, d
 }
 #endif
 
-cudaError_t launch_k1_fast(const PassArgs& a, int grid, bool debug, int device, cudaStream_t stream);
-// load every pass kernel (CUDA loads lazily at first launch, and a load waits for running kernels) and the offset tables;
-// *max_local is raised to the largest per-thread local memory (spill frame) of the kernels loaded
-cudaError_t preload_fast_kernels(int device, size_t* max_local);
-cudaError_t preload_assoc_kernels(int device, int K, size_t* max_local);
+// Which compiled instance of each pass kernel a ctx launches, and the state of its sweep-order sort.  Filled once by
+// srl_ctx_create (defaults, then the SRL_* environment variables), changed by srl_ctx_set_option.
+struct KernelChoice {
+    int split_lpk = 4, scan_minb = 8, fit_minb = 6;   // k1_scan lanes per keypoint and blocks per SM, k1_fit blocks per SM
+    int fast_lpk = 1, fast_minb = 5;                  // k1_fast
+    int k1_minb = 3;                                  // k1_assoc
+    int order_mode = 1;          // option "cluster_order": 0 CUB; 1, 2, 3 the cluster kernel (default, direct scatter, first version)
+    int order_state = -1;        // -1 the cluster kernel is being verified against CUB, 1 verified and in use, 0 CUB
+    int order_checks_left = 4;   // the first uses after the mode is set run both sorts and compare the orders on the device
+    int cluster_size = 0;        // 0 not decided yet (first launch), -1 no cluster size is launchable, else the size in use
+    void restart_order_checks() { order_state = order_mode ? -1 : 0; order_checks_left = 4; }
+};
+// Load the instances a non-debug pass of `ch` can launch, of every pass form (CUDA loads lazily at first launch, and a
+// load waits for running kernels); *max_local is raised to their largest per-thread local memory (spill frame).
+cudaError_t preload_fast_kernels(const KernelChoice& ch, size_t* max_local);
+cudaError_t preload_assoc_kernels(const KernelChoice& ch, int K, size_t* max_local);
+inline cudaError_t preload_kernel(const void* fn, size_t* max_local) {
+    cudaFuncAttributes at;
+    const cudaError_t e = cudaFuncGetAttributes(&at, fn);
+    if (e == cudaSuccess && at.localSizeBytes > *max_local) *max_local = at.localSizeBytes;
+    return e;
+}
 constexpr int kSplitSlots = 23;   // = NS of srl_fast.cu: candidate slots k1_scan hands to k1_fit per keypoint
-cudaError_t launch_k1_split(const PassArgs& a, long long n, int max_grid, bool debug, int device, cudaStream_t stream, bool pdl);
 // <<<>>> with the programmatic-stream-serialization attribute when pdl is set
 template <typename Args>
 inline cudaError_t launch_pass_kernel(void (*fn)(const Args), const Args& a, unsigned grid, unsigned block, size_t smem, cudaStream_t stream, bool pdl) {
@@ -329,20 +345,16 @@ inline cudaError_t launch_pass_kernel(void (*fn)(const Args), const Args& a, uns
     cfg.attrs = at; cfg.numAttrs = pdl ? 1 : 0;
     return cudaLaunchKernelEx(&cfg, fn, a);
 }
-void k1_split_set_lanes_per_keypoint(int v);
-int k1_fast_max_blocks_per_sm();
-void k1_fast_set_min_blocks(int v);
-void k1_fast_set_lanes_per_keypoint(int v);
-int k1_fast_lanes_per_keypoint();
-cudaError_t sweep_compute_order(const double* d_raw, long long n, unsigned* d_order, void* scratch, size_t scratch_bytes,
-                                size_t* needed, cudaStream_t stream);
-void sweep_order_set_impl(int v);   // 1: the single-launch cluster sort (verified against the CUB order at first use), 0: CUB
-int sweep_order_impl();             // -1 cluster kernel not verified yet, 1 verified and in use, 0 CUB
+// The Morton order of a sweep's n keypoints into d_order, by the sort ch.order_state selects.  With scratch == nullptr
+// (or too small) only *needed is set.
+cudaError_t sweep_compute_order(KernelChoice& ch, const double* d_raw, long long n, unsigned* d_order, void* scratch,
+                                size_t scratch_bytes, size_t* needed, cudaStream_t stream);
 
-size_t k1_smem_bytes(int K);
-int k1_max_blocks_per_sm(int K, int nb);
-void k1_set_min_blocks(int v);
-cudaError_t launch_k1(const PassArgs& a, int grid, bool debug, int device, cudaStream_t stream, bool pdl = false);
+// The pass launchers, on ctx->stream with the instance of ctx->choice; each computes its own grid for the pass's n keypoints.
+// k1_assoc (the assoc form, or with a.only_flagged set the fallback launch of the fast and split forms)
+cudaError_t launch_k1(const srl_ctx* ctx, const PassArgs& a, long long n, bool debug, bool pdl = false);
+cudaError_t launch_k1_fast(const srl_ctx* ctx, const PassArgs& a, long long n, bool debug);
+cudaError_t launch_k1_split(const srl_ctx* ctx, const PassArgs& a, long long n, bool debug, bool pdl);
 cudaError_t launch_k2(const K2Args& a, cudaStream_t stream, bool pdl = false);
 cudaError_t launch_transform(const double* raw, long long n, const PassConst& c, double* out, cudaStream_t stream);
 
@@ -385,9 +397,10 @@ struct srl_ctx {
     bool force_exact = false;
     int force_amb_mod = 0;                   // test knob for the k1_fast -> k1_assoc hand-over
     int variant = 0;                         // 0 auto, 1 = k1_fast, 2 = k1_assoc only, 3 = k1_scan + k1_fit (1 and 3 with the exact fallback)
+    srl::KernelChoice choice;
     unsigned long long* d_scan_count = nullptr;
     // device-resident updateIEKF loop (row N1)
-    bool kernels_preloaded = false;
+    bool kernels_preloaded = false;          // the instances `choice` can launch are loaded; setting an integer option clears it
     int shuffle_rule = 0;                    // option "shuffle_rule": srl_build_frame's draws, 0 Lemire (libstdc++ with __int128), 1 division
     bool shuffle_on_host = false;            // option "shuffle_on_host": srl_build_frame's shuffles as a host Fisher-Yates + upload
     int concurrent_kernels = -1;             // -1 not probed yet; 0: kernels of this process are serialised (profiler): host loop
