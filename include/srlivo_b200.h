@@ -495,6 +495,38 @@ int srl_color_map_select_for_projection(srl_color_map* cm, const srl_camera* cam
 int srl_color_map_gather_points(srl_color_map* cm, const uint32_t* point_ids, size_t n, float* xyz, int16_t* rgb,
                                 int16_t* n_rgb, float* cov, int16_t* key_index);
 
+/* ---- the optical-flow tracker's pyramidal Lucas-Kanade (DESIGN.md row N6): LKOpticalFlowKernel (include/lkpyramid.h:65-131),
+ * trackImage (src/lkpyramid.cpp:755-795), called by opticalFlowTracker::init and ::trackImage (src/opticalFlowTracker.cpp:134,196).
+ * Bit for bit the reference: points, status, return value and every pyramid level. */
+typedef struct srl_lk srl_lk;
+#define SRL_LK_COUNT 1                  /* cv::TermCriteria::COUNT */
+#define SRL_LK_EPS 2                    /* cv::TermCriteria::EPS */
+typedef struct srl_lk_params {
+    int32_t win_w, win_h;               /* lk_win_size, 3..31 each */
+    int32_t max_level;                  /* 0..8; the first image's pyramid build lowers it for good (:609-619) */
+    int32_t criteria_type;              /* SRL_LK_COUNT | SRL_LK_EPS */
+    int32_t max_count;                  /* normalised as setTerminationCriteria (:670-682): 30 without COUNT, else clamped to 0..100 */
+    double epsilon;                     /* 0.01 without EPS, else clamped to 0..10 */
+    int32_t flags;                      /* OPTFLOW_* bits; neither changes trackImage's outputs (no err output here) */
+    double min_eig_threshold;
+} srl_lk_params;
+int srl_lk_create(srl_ctx* ctx, const srl_lk_params* params, srl_lk** out);
+void srl_lk_destroy(srl_lk* lk);
+/* trackImage(gray, last_pts, curr_pts, status): gray is cols x rows bytes, rows `pitch` bytes apart; last_pts and curr_pts are n
+ * (x, y) float pairs, status n bytes; *n_tracked = the sum of status.  The first image only builds its pyramid: curr_pts =
+ * last_pts, status untouched, *n_tracked = 0.  n = 0 still consumes the image.  Every buffer is host or device memory.
+ * SRL_BAD_ARG for an image not larger than the window, or of another size than the first image. */
+int srl_lk_track_image(srl_lk* lk, const uint8_t* gray, int cols, int rows, size_t pitch, const float* last_pts, size_t n,
+                       float* curr_pts, uint8_t* status, int64_t* n_tracked);
+/* getMaxLevel() and the first image's size (0 x 0 before it) */
+int srl_lk_info(srl_lk* lk, int32_t* max_level, int32_t* cols, int32_t* rows);
+/* test hook: level `level` of the last image's pyramid (which 0) or of the image before it (which 1), padding included:
+ * img (level rows + 2 win_h) x (level cols + 2 win_w) bytes, deriv the same count of (Ix, Iy) int16 pairs (either may be NULL;
+ * host or device).  Level l is ((cols + 1) / 2 applied l times) wide, likewise high. */
+int srl_lk_download_level(srl_lk* lk, int which, int level, uint8_t* img, int16_t* deriv);
+/* device time of the last srl_lk_track_image: image upload + pyramid + derivatives, then the point tracking (CUDA events) */
+int srl_lk_last_times(srl_lk* lk, double* pyramid_ms, double* track_ms);
+
 /* eskfEstimator::observe (src/eskfEstimator.cpp:219-230) — host math, exported for parity tests */
 int srl_eskf_observe(srl_eskf_state* eskf, const double d_x[17]);
 

@@ -21,6 +21,7 @@
 //   addPointToPcl + publishCLoudWorld src/lioOptimization.cpp:432,552 srl::LioBackend::addPointsToMapPublished
 //   pubColorPoints / saveColorPoints  src/lioOptimization.cpp:1210,1386 srl::LioBackend::pubColorPoints / saveColorPoints
 //   rgbMapTracker::selectPointsForProjection src/rgbMapTracker.cpp:45 srl::LioBackend::selectPointsForProjection / gatherColorPoints
+//   LKOpticalFlowKernel::trackImage   src/lkpyramid.cpp:755         srl::LKOpticalFlowKernel::trackImage (on LioBackend::context())
 #pragma once
 
 #include <array>
@@ -255,6 +256,7 @@ public:
         check(srl_color_map_gather_points(color_, ids.data(), ids.size(), xyz, rgb, n_rgb, cov, nullptr), "srl_color_map_gather_points");
     }
     srl_color_map* colorMap() { return color_; }
+    srl_ctx* context() { return ctx_; }
 
 private:
     srl_ctx* ctx_ = nullptr;
@@ -283,6 +285,58 @@ private:
         check(rc, "srl_update_iekf");
         s.success = sm.success != 0;
         return s;
+    }
+};
+
+// LKOpticalFlowKernel (include/lkpyramid.h:65-131) on the GPU, bit for bit: the constructor takes the reference's arguments
+// and defaults (criteria = (type, max_count, epsilon) of cv::TermCriteria, SRL_LK_COUNT | SRL_LK_EPS), trackImage mirrors
+// src/lkpyramid.cpp:755.  Points are (x, y) float pairs, the layout of std::vector<cv::Point2f>; every pointer overload takes
+// host or device memory.  The kernel must be destroyed before its context.
+class LKOpticalFlowKernel {
+public:
+    LKOpticalFlowKernel(srl_ctx* ctx, int win_w = 21, int win_h = 21, int maxLevel = 3, int criteria_type = SRL_LK_COUNT | SRL_LK_EPS,
+                        int max_count = 30, double epsilon = 0.01, int flags = 0, double minEigThreshold = 1e-4)
+        : ctx_(ctx) {
+        const srl_lk_params p{win_w, win_h, maxLevel, criteria_type, max_count, epsilon, flags, minEigThreshold};
+        check(srl_lk_create(ctx, &p, &lk_), "srl_lk_create");
+    }
+    ~LKOpticalFlowKernel() { if (lk_) srl_lk_destroy(lk_); }
+    LKOpticalFlowKernel(const LKOpticalFlowKernel&) = delete;
+    LKOpticalFlowKernel& operator=(const LKOpticalFlowKernel&) = delete;
+
+    // trackImage(curr_img, last_tracked_pts, curr_tracked_pts, status): curr_pts is resized to n, status to n except on the
+    // first image (which only builds the pyramid and returns 0, as the reference does); returns the number of tracked points
+    int trackImage(const uint8_t* gray, int cols, int rows, size_t pitch, const std::vector<float>& last_xy, std::vector<float>& curr_xy,
+                   std::vector<uint8_t>& status) {
+        const size_t n = last_xy.size() / 2;
+        curr_xy.resize(n * 2);
+        int32_t ml = 0, c0 = 0, r0 = 0;
+        check(srl_lk_info(lk_, &ml, &c0, &r0), "srl_lk_info");
+        std::vector<uint8_t> untouched;     // the first image leaves the caller's status as it is
+        if (c0 != 0) status.assign(n, 1);   // later images: status is resized, every entry starts at 1
+        else untouched.assign(n, 1);
+        int64_t k = 0;
+        check(srl_lk_track_image(lk_, gray, cols, rows, pitch, last_xy.data(), n, curr_xy.data(), c0 != 0 ? status.data() : untouched.data(), &k),
+              "srl_lk_track_image");
+        return (int)k;
+    }
+    // device (or host) buffers of n points, e.g. the selection's device uv straight in
+    int trackImage(const uint8_t* gray, int cols, int rows, size_t pitch, const float* last_xy, size_t n, float* curr_xy, uint8_t* status) {
+        int64_t k = 0;
+        check(srl_lk_track_image(lk_, gray, cols, rows, pitch, last_xy, n, curr_xy, status, &k), "srl_lk_track_image");
+        return (int)k;
+    }
+    int getMaxLevel() {
+        int32_t ml = 0;
+        check(srl_lk_info(lk_, &ml, nullptr, nullptr), "srl_lk_info");
+        return ml;
+    }
+
+private:
+    srl_ctx* ctx_ = nullptr;
+    srl_lk* lk_ = nullptr;
+    void check(int rc, const char* what) {
+        if (rc != SRL_OK) throw std::runtime_error(std::string(what) + ": " + (ctx_ ? srl_last_error(ctx_) : "no context"));
     }
 };
 

@@ -71,6 +71,12 @@ class Camera(C.Structure):
                 ("cols", C.c_int32), ("rows", C.c_int32)]
 
 
+class LkParams(C.Structure):
+    """srl_lk_params: LKOpticalFlowKernel's constructor arguments (include/lkpyramid.h:100-106)."""
+    _fields_ = [("win_w", C.c_int32), ("win_h", C.c_int32), ("max_level", C.c_int32), ("criteria_type", C.c_int32), ("max_count", C.c_int32),
+                ("epsilon", C.c_double), ("flags", C.c_int32), ("min_eig_threshold", C.c_double)]
+
+
 class ProjectionParams(C.Structure):
     """srl_projection_params: the arguments of rgbMapTracker::selectPointsForProjection and the tracker's depth bounds."""
     _fields_ = [("minimum_dis", C.c_double), ("skip_step", C.c_int32), ("use_all_points", C.c_int32), ("minimum_depth", C.c_double),
@@ -120,6 +126,7 @@ EXPORTS = [
     "srl_cloud_frame_create", "srl_cloud_frame_destroy", "srl_cloud_frame_size", "srl_cloud_frame_device", "srl_cloud_frame_download",
     "srl_build_frame", "srl_shuffle_replay", "srl_map_insert_published", "srl_map_insert_sweep_published", "srl_color_map_export",
     "srl_color_map_select_for_projection", "srl_color_map_gather_points",
+    "srl_lk_create", "srl_lk_destroy", "srl_lk_track_image", "srl_lk_info", "srl_lk_download_level", "srl_lk_last_times",
 ]
 
 _lib = None
@@ -215,6 +222,13 @@ def lib():
     L.srl_color_map_export.argtypes = [vp, i32, i32, vp, vp, sz, C.POINTER(i64)]
     L.srl_color_map_select_for_projection.argtypes = [vp, C.POINTER(Camera), C.POINTER(ProjectionParams), vp, vp, vp, sz, C.POINTER(i64)]
     L.srl_color_map_gather_points.argtypes = [vp, vp, sz, vp, vp, vp, vp, vp]
+    L.srl_lk_create.argtypes = [vp, C.POINTER(LkParams), C.POINTER(vp)]
+    L.srl_lk_destroy.argtypes = [vp]
+    L.srl_lk_destroy.restype = None
+    L.srl_lk_track_image.argtypes = [vp, vp, C.c_int, C.c_int, sz, vp, sz, vp, vp, C.POINTER(i64)]
+    L.srl_lk_info.argtypes = [vp] + [C.POINTER(i32)] * 3
+    L.srl_lk_download_level.argtypes = [vp, C.c_int, C.c_int, vp, vp]
+    L.srl_lk_last_times.argtypes = [vp, C.POINTER(dbl), C.POINTER(dbl)]
     L.srl_cloud_frame_create.argtypes = [vp, sz, C.POINTER(vp)]
     L.srl_cloud_frame_destroy.argtypes = [vp]
     L.srl_cloud_frame_destroy.restype = None

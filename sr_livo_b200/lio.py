@@ -12,6 +12,7 @@ Names and argument meaning follow the reference so the parity tests read like it
   addPointToPcl / publishCLoudWorld     src/lioOptimization.cpp:432,552 -> LioOptimization.addPointsToMapPublished
   pubColorPoints / saveColorPoints      src/lioOptimization.cpp:1210,1386 -> ColorVoxelMap.pubColorPoints / saveColorPoints
   rgbMapTracker::selectPointsForProjection src/rgbMapTracker.cpp:45     -> ColorVoxelMap.selectPointsForProjection / gatherPoints
+  LKOpticalFlowKernel::trackImage       src/lkpyramid.cpp:755           -> LKOpticalFlowKernel.trackImage
 
 Error behaviour: optimizeSummary.success=false <-> OptimizeSummary.success False (SRL_TOO_FEW_RESIDUALS);
 the reference's `throw std::runtime_error("error")` on NaN planarity <-> RuntimeError; everything else raises
@@ -764,5 +765,95 @@ class LioOptimization:
         return summ, fq, ft, world
 
 
+COUNT, EPS = 1, 2   # cv::TermCriteria::COUNT, ::EPS
+
+
+def tracker_lk_params() -> dict:
+    """The LKOpticalFlowKernel opticalFlowTracker's constructor makes (src/opticalFlowTracker.cpp:5-8): a 21 x 21 window, 3 levels,
+    COUNT | EPS with 10 iterations and epsilon 0.05, flags cv_OPTFLOW_LK_GET_MIN_EIGENVALS (8), the default min_eig_threshold."""
+    return dict(win_size=(21, 21), max_level=3, criteria=(COUNT | EPS, 10, 0.05), flags=8, min_eig_threshold=1e-4)
+
+
+class LKOpticalFlowKernel:
+    """LKOpticalFlowKernel (include/lkpyramid.h:65-131, srl_lk_*): the optical-flow tracker's pyramidal Lucas-Kanade on the GPU, bit
+    for bit the reference.  criteria = (type, max_count, epsilon) as cv::TermCriteria; the defaults are the reference's own
+    constructor defaults.  Each image's pyramid stays on the device as the previous image of the next call."""
+
+    def __init__(self, ctx: Context, win_size=(21, 21), max_level: int = 3, criteria=(COUNT | EPS, 30, 0.01), flags: int = 0,
+                 min_eig_threshold: float = 1e-4):
+        self.ctx = ctx
+        t, c, e = criteria
+        self.params = capi.LkParams(int(win_size[0]), int(win_size[1]), int(max_level), int(t), int(c), float(e), int(flags),
+                                    float(min_eig_threshold))
+        h = C.c_void_p()
+        _check(ctx.h, lib().srl_lk_create(ctx.h, C.byref(self.params), C.byref(h)))
+        self.h = h
+
+    def close(self):
+        if getattr(self, "h", None):
+            lib().srl_lk_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def trackImage(self, gray, last_pts, out=None):
+        """trackImage (src/lkpyramid.cpp:755-795): (curr_pts (n, 2) float32, status (n,) uint8, n_tracked).  gray: (rows, cols) uint8
+        with unit column stride (a numpy array or a torch tensor, host or CUDA; rows may be padded); last_pts: (n, 2) float32 (the
+        selection's uv as it comes).  out = (curr_pts, status) buffers receive the result; without it they are made on last_pts'
+        side (numpy, or a torch tensor on its device), status filled with ones.  The first image only builds its pyramid:
+        curr_pts = last_pts, status as it was, n_tracked 0."""
+        if _is_tensor(gray):
+            if str(gray.dtype) != "torch.uint8" or gray.dim() != 2 or gray.stride(1) != 1:
+                raise TypeError("expected a 2-D torch.uint8 image with unit column stride")
+            p_img, rows, cols, pitch = gray.data_ptr(), gray.shape[0], gray.shape[1], gray.stride(0)
+        else:
+            if not (isinstance(gray, np.ndarray) and gray.dtype == np.uint8 and gray.ndim == 2 and gray.strides[1] == 1):
+                raise TypeError("expected a 2-D uint8 array with unit column stride")
+            p_img, rows, cols, pitch = gray.ctypes.data, gray.shape[0], gray.shape[1], gray.strides[0]
+        p_last, n = _addr(last_pts, np.float32, 2)
+        if out is None:
+            curr = _empty_like_input(last_pts, n, 2, np.float32)
+            status = _empty_like_input(last_pts, n, 1, np.uint8).reshape(-1)
+            status[:] = 1
+        else:
+            curr, status = out
+        p_curr, n_curr = _addr(curr, np.float32, 2)
+        p_st, n_st = _addr(status, np.uint8, 1)
+        if n_curr < n or n_st < n:
+            raise ValueError("out buffers hold fewer points than last_pts")
+        k = C.c_int64(0)
+        _check(self.ctx.h, lib().srl_lk_track_image(self.h, C.c_void_p(p_img), int(cols), int(rows), int(pitch), C.c_void_p(p_last), n,
+                                                    C.c_void_p(p_curr), C.c_void_p(p_st), C.byref(k)))
+        return curr[:n], status[:n], k.value
+
+    def getMaxLevel(self) -> int:
+        v = C.c_int32(0)
+        _check(self.ctx.h, lib().srl_lk_info(self.h, C.byref(v), None, None))
+        return v.value
+
+    def level(self, which: int, level: int):
+        """Test hook: (padded image, padded (Ix, Iy) int16 buffer) of a pyramid level; which 0 is the last image's, 1 the one before."""
+        ml, cols, rows = C.c_int32(0), C.c_int32(0), C.c_int32(0)
+        _check(self.ctx.h, lib().srl_lk_info(self.h, C.byref(ml), C.byref(cols), C.byref(rows)))
+        w, h = cols.value, rows.value
+        for _ in range(level):
+            w, h = (w + 1) // 2, (h + 1) // 2
+        shape = (h + 2 * self.params.win_h, w + 2 * self.params.win_w)
+        img, der = np.zeros(shape, np.uint8), np.zeros(shape + (2,), np.int16)
+        _check(self.ctx.h, lib().srl_lk_download_level(self.h, int(which), int(level), ptr(img), ptr(der)))
+        return img, der
+
+    def lastTimes(self) -> tuple[float, float]:
+        """(ms of image upload + pyramid + derivatives, ms of the point tracking) of the last trackImage, CUDA events."""
+        a, b = C.c_double(0), C.c_double(0)
+        _check(self.ctx.h, lib().srl_lk_last_times(self.h, C.byref(a), C.byref(b)))
+        return a.value, b.value
+
+
 __all__ = ["Context", "VoxelHashMap", "ColorVoxelMap", "Sweep", "EskfEstimator", "LioOptimization", "OptimizeSummary", "PlaneResiduals",
-           "IcpParams", "r3live_params", "r3live_map_options", "r3live_compressed_map_options", "make_frame", "SrlError", "write_pcd_xyzrgb"]
+           "IcpParams", "r3live_params", "r3live_map_options", "r3live_compressed_map_options", "make_frame", "SrlError", "write_pcd_xyzrgb",
+           "LKOpticalFlowKernel", "tracker_lk_params"]
