@@ -440,7 +440,10 @@ int srl_color_map_add_points(srl_color_map* cm, const double* xyz_world, size_t 
                              double time_last_process, int32_t to_rendering, int64_t* n_stored);
 /* renderPointsInRecentVoxel: every point of every recently visited voxel is projected into the frame (pinhole, scale 1),
  * tested against the FoV margin, coloured by bilinear interpolation of the BGR8 image (host or device, rows*cols*3,
- * OpenCV's saturating Vec3b arithmetic) and fused with rgbPoint::updateRgb; *n_rendered = render_point_count. */
+ * OpenCV's saturating Vec3b arithmetic) and fused with rgbPoint::updateRgb; *n_rendered = render_point_count.
+ * cam->fov_margin must be >= 0, else SRL_BAD_ARG before anything is staged or launched (NaN included): a negative margin
+ * would read outside the image with non-zero weights, which the reference leaves undefined (DESIGN.md section 5).  Reads
+ * stay inside the rows*cols*3 image. */
 int srl_color_map_render_recent(srl_color_map* cm, const srl_camera* cam, const uint8_t* image_bgr, double obs_time, int64_t* n_rendered);
 /* colour state in the voxel order of srl_map_download(srl_color_map_voxels(cm)): rgb nv*cap*3, n_rgb nv*cap, cov nv*cap*3,
  * obs_dist nv*cap, last_obs nv*cap, last_visited nv */

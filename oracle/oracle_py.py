@@ -422,10 +422,14 @@ class OracleColorMap:
         return int(lib().orc_color_add_points(self._h, _ptr(xyz), xyz.shape[0], self.voxel_size, self.cap, self.min_dist,
                                               add_point_step, time_sweep_end, time_last_process, 1 if to_rendering else 0))
 
-    def render(self, cam15, image_bgr, obs_time) -> int:
+    def render(self, cam15, image_bgr, obs_time, rows=None) -> int:
+        """rows: the frame's image_rows when image_bgr holds more rows than the frame (a buffer padded below the image, so the
+        zero-weight taps of row `rows` are read from memory the caller owns); default image_bgr.shape[0]."""
         cam = _f64(cam15).reshape(15)
         img = np.ascontiguousarray(image_bgr, np.uint8)
-        return int(lib().orc_color_render(self._h, _ptr(cam), _ptr(img), img.shape[0], img.shape[1], float(obs_time)))
+        rows = img.shape[0] if rows is None else int(rows)
+        assert rows <= img.shape[0]
+        return int(lib().orc_color_render(self._h, _ptr(cam), _ptr(img), rows, img.shape[1], float(obs_time)))
 
     def counts(self):
         L = lib()

@@ -570,7 +570,10 @@ int64_t ref_color_render(void* ctx, const double* cam, const uint8_t* image_bgr,
     std::vector<point3D> none;
     cloudFrame frame(none, &st);
     frame.image_rows = rows; frame.image_cols = cols;
-    frame.rgb_image.create(rows, cols, 3);
+    // zero rows below the image: getSubPixel reads row `rows` (with weight 0) for a point at v == rows - 1 exactly, and at
+    // u == cols - 1 too the pixel after that row
+    frame.rgb_image.create(rows + 2, cols, 3);
+    frame.rgb_image.rows = rows;
     std::memcpy(frame.rgb_image.data, image_bgr, (size_t)rows * cols * 3);
     std::vector<voxelId> voxels = T->voxels_recent_visited;
     T->renderPointsInRecentVoxel(L->color_voxel_map, &frame, &voxels, obs_time);

@@ -395,13 +395,20 @@ __device__ __forceinline__ unsigned render_point(const float* __restrict__ bp, C
     const double frac_r = __dsub_rn(v, (double)fr), frac_c = __dsub_rn(u, (double)fc);
     const double w00 = __dmul_rn(__dsub_rn(1.0, frac_r), __dsub_rn(1.0, frac_c)), w10 = __dmul_rn(frac_r, __dsub_rn(1.0, frac_c));
     const double w01 = __dmul_rn(__dsub_rn(1.0, frac_r), frac_c), w11 = __dmul_rn(frac_r, frac_c);
+    // The +1 taps are clamped to the last row / column (no step down / right there), which changes no value for
+    // fov_margin >= 0 (negative margins are refused by srl_color_map_render_recent): fr + 1 == rows needs ceil(v) <= rows - 1,
+    // because the window's upper bound fl(1 - fov) * rows is at most rows; so v == rows - 1 exactly, frac_r == 0 and
+    // w10 == w11 == 0.  The same holds for columns.  The lower bound v >= fl(fov * rows) + 1 >= 1 keeps fr >= 0.  The
+    // reference reads row `rows` there with weight 0.
+    const unsigned char* p00 = img + ((size_t)fr * c.cols + fc) * 3;
+    const size_t down = fr + 1 < c.rows ? (size_t)c.cols * 3 : 0, right = fc + 1 < c.cols ? 3 : 0;
     double color[3];
 #pragma unroll
     for (int ch = 0; ch < 3; ++ch) {
-        const unsigned char a = sat_u8(__dmul_rn((double)img[((size_t)fr * c.cols + fc) * 3 + ch], w00));
-        const unsigned char b = sat_u8(__dmul_rn((double)img[((size_t)(fr + 1) * c.cols + fc) * 3 + ch], w10));
-        const unsigned char cc = sat_u8(__dmul_rn((double)img[((size_t)fr * c.cols + fc + 1) * 3 + ch], w01));
-        const unsigned char d = sat_u8(__dmul_rn((double)img[((size_t)(fr + 1) * c.cols + fc + 1) * 3 + ch], w11));
+        const unsigned char a = sat_u8(__dmul_rn((double)p00[ch], w00));
+        const unsigned char b = sat_u8(__dmul_rn((double)p00[down + ch], w10));
+        const unsigned char cc = sat_u8(__dmul_rn((double)p00[right + ch], w01));
+        const unsigned char d = sat_u8(__dmul_rn((double)p00[down + right + ch], w11));
         color[ch] = (double)sat_add_u8(sat_add_u8(sat_add_u8(a, b), cc), d);
     }
     // rgbPoint::updateRgb (src/cloudMap.cpp:59-101), mixed float / double arithmetic as written there
@@ -1534,6 +1541,9 @@ int srl_color_map_add_points(srl_color_map* cm, const double* xyz_world, size_t 
 int srl_color_map_render_recent(srl_color_map* cm, const srl_camera* cam, const uint8_t* image_bgr, double obs_time, int64_t* n_rendered) {
     if (!cm || !cam || !image_bgr || cam->cols < 2 || cam->rows < 2) return SRL_BAD_ARG;
     srl_ctx* ctx = cm->ctx;
+    // a negative margin widens the window past the image with non-zero weights: reads outside the image (the reference's
+    // behaviour is undefined there, and it only renders with margin 0.005).  !(>= 0) also refuses NaN.
+    if (!(cam->fov_margin >= 0.0)) return set_err(ctx, SRL_BAD_ARG, "srl_color_map_render_recent: fov_margin must be >= 0");
     srl_map* m = cm->vox;
     cudaStream_t st = ctx->stream;
     SRL_CUDA(ctx, cudaSetDevice(ctx->device));

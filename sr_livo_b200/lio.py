@@ -280,6 +280,10 @@ class ColorVoxelMap:
         return stored.value
 
     def renderPointsInRecentVoxel(self, camera: "capi.Camera", image_bgr, obs_time: float) -> int:
+        """rgbMapTracker::renderPointsInRecentVoxel (srl_color_map_render_recent) with a (rows, cols, 3) BGR8 host image; returns
+        render_point_count.  camera.fov_margin must be >= 0 (SRL_BAD_ARG otherwise, NaN included, and the map is untouched):
+        a negative margin would sample outside the image, which the reference leaves undefined.  The selection
+        (selectPointsForProjection) still takes negative margins."""
         img = np.ascontiguousarray(image_bgr, np.uint8)
         assert img.shape == (camera.rows, camera.cols, 3)
         n = C.c_int64(0)
