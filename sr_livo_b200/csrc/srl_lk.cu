@@ -18,6 +18,11 @@
 //     8-9 the scalar tails (x >= 8 * (w / 8)); then bbuf = qb0 + qb1, ib1 = tail1 + (bbuf0 + bbuf2), ib2 = tail2 + (bbuf1 + bbuf3)
 // The integer products are exact; the partial sums exceed 2^24, so their order decides the bits.  Every float operation that
 // matters is an explicit _rn intrinsic (no contraction; the file is also built with --fmad=false), sqrt and division are IEEE.
+// Magnitudes (tests/test_lk_edges_pin.py pins them on 0/255 scenes): |Scharr| <= 4080, |diff| <= 8160, so every weighted sum
+// fits 32 bits and packs/subs never saturate, while a madd pair reaches 2 * 8160 * 4080 > 2^24 and a tail product 8160 * 4080:
+// their int -> float conversions round, as _mm_cvtepi32_ps / cvtsi2ss round them, to nearest even (__int2float_rn).
+// Non-finite and huge coordinates: cvFloor gives INT_MIN outside the int range and for NaN, so such a point is outside at
+// every level and only scaled; a NaN comes back as the input NaN with its quiet bit set, as the reference's x86 code returns it.
 #include <algorithm>
 #include <cfloat>
 #include <climits>
@@ -265,6 +270,10 @@ __global__ void __launch_bounds__(kLkBlock) k_lk_track(const __grid_constant__ L
         __syncwarp();   // the chains are done with Iw / dIw before the next level rewrites them
     }
     if (lane == 0) {
+        // A NaN coordinate is outside at every level, so its output is only ever scaled.  The reference's x86 products return
+        // that NaN with its quiet bit set; PTX arithmetic returns the canonical NaN, so the input's bits are restored here.
+        if (isnan(p0.x)) cur.x = __int_as_float(__float_as_int(p0.x) | 0x00400000);
+        if (isnan(p0.y)) cur.y = __int_as_float(__float_as_int(p0.y) | 0x00400000);
         A.next_pts[pt] = cur;
         A.status[pt] = st;
         if (st) atomicAdd(A.n_tracked, 1ull);
