@@ -42,6 +42,8 @@ def lib():
     L.orc_map_snapshot.argtypes = [P, I32, P, P, P]
     L.orc_map_snapshot.restype = I64
     L.orc_map_load.argtypes = [P, P, P, P, I64, I32]
+    L.orc_map_remove_far.argtypes = [P, P, D]
+    L.orc_map_remove_far.restype = I64
     L.orc_map_add_points_published.argtypes = [P, P, I64, D, I32, D, I32, D, P, C.POINTER(I64)]
     L.orc_map_add_points_published.restype = I64
     L.orc_color_create.restype = P
@@ -85,6 +87,11 @@ class OracleMap:
         added = lib().orc_map_add_points_published(self._h, _ptr(xyz), xyz.shape[0], voxel_size, max_num_points_in_voxel,
                                                    min_distance_points, min_num_points, float(translation_z), _ptr(out), C.byref(n_pub))
         return int(added), out[:n_pub.value].copy()
+
+    def remove_far(self, location, distance: float) -> int:
+        """removePointsFarFromLocation (src/lioOptimization.cpp:556-572): voxels erased."""
+        loc = _f64(location).reshape(3)
+        return int(lib().orc_map_remove_far(self._h, _ptr(loc), float(distance)))
 
     def snapshot(self, cap=20):
         n = int(lib().orc_map_num_voxels(self._h))

@@ -207,6 +207,16 @@ def _point(R, R_il, t_il, raw, trans):
     return [p[i] + trans[i] for i in range(3)]
 
 
+def transform_point_fp64(raw_xyz, q, t, R_il, t_il) -> np.ndarray:
+    """transformPoint (src/utility.cpp:314-318) in FP64, one IEEE rounding per operation: R(q) (R_il raw + t_il) + t, with
+    toRotationMatrix of q as given and Eigen's a0 + (a1 + a2) products."""
+    R = qrot([float(v) for v in np.asarray(q, np.float64).reshape(4)])
+    Ril = [float(v) for v in np.asarray(R_il, np.float64).reshape(9)]
+    til = [float(v) for v in np.asarray(t_il, np.float64).reshape(3)]
+    tt = [float(v) for v in np.asarray(t, np.float64).reshape(3)]
+    return np.array([_point(R, Ril, til, p, tt) for p in np.asarray(raw_xyz, np.float64).reshape(-1, 3).tolist()]).reshape(-1, 3)
+
+
 # ---- FP64 decisions ------------------------------------------------------------------------------------------------
 def time_points(t0: float, rel) -> np.ndarray:
     """time_point = time_frame_begin + relative_time / 1000.0 (numpy float64: one IEEE rounding per operation)."""

@@ -210,8 +210,8 @@ def test_narrow_color_map_still_takes_the_lio_insert(ctx):
     cm = lio.ColorVoxelMap(ctx, voxel_size=SIZE, max_num_points_in_voxel=20, max_voxels=1 << 12, min_distance_points=FINE)
     try:
         vox = C.c_void_p(L.srl_color_map_voxels(cm.h))
-        pts = sweep(seed=12, n_dense=2000)
-        pts = pts[np.abs(pts).max(axis=1) < 3000.0]        # the LIO map drops |x / size| >= 32765 (DESIGN.md section 5)
+        pts = sweep(seed=12, n_dense=2000)                 # 1000 of its points lie past |x / size| = 32768, where keys wrap in
+                                                           # both maps as in the reference (DESIGN.md section 5)
         n = C.c_int64(0)
         assert L.srl_map_insert(vox, capi.ptr(np.ascontiguousarray(pts)), pts.shape[0], FINE, 0, C.byref(n)) == capi.SRL_OK
         om = O.OracleMap()
