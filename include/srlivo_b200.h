@@ -398,7 +398,7 @@ int srl_shuffle_replay(srl_ctx* ctx, const uint64_t* words, size_t n_words, size
  * A colour map = a voxel map (same HBM layout as srl_map; srl_color_map_voxels exposes it for download / stats) whose
  * points carry (rgb, N_rgb, cov_rgb, observe_distance, last_observe_time), the fine occupancy set hashmap_3d_points
  * (cells of min_distance_points) that decides which stored points enter rgb_points_vec, and the list of voxels
- * visited for the first time by the sweeps since the last rendering (voxels_recent_visited). */
+ * the last rendering sweep visited for the first time (voxels_recent_visited). */
 typedef struct srl_color_map srl_color_map;
 typedef struct srl_camera {      /* the state fields cloudFrame::project3dTo2d / if2dPointsAvailable read (include/state.h) */
     double q_camera_world[4];    /* x, y, z, w */
@@ -417,7 +417,7 @@ typedef struct srl_camera {      /* the state fields cloudFrame::project3dTo2d /
  * 10.6 GB for 2^20 voxels at cap 100); srl_color_map_create_growable commits initial_voxels (and initial_voxels * max(cap,
  * 20) rgb points) and grows like srl_map_create_growable: the voxel arrays with the voxels, the rgb list and the fine set
  * with the rgb points, the two recent-voxel lists with their length, each doubling up to its limit (max_voxels, max_voxels
- * * max(cap, 20) rgb points, 4 * max_voxels + 1024 recent entries).  Growth happens inside srl_color_map_add_points and,
+ * * max(cap, 20) rgb points, max_voxels recent entries).  Growth happens inside srl_color_map_add_points and,
  * for cap <= 20, inside srl_map_insert / srl_map_upload on srl_color_map_voxels(cm); never inside the renderer.
  * 1 <= initial_voxels <= max_voxels, else SRL_BAD_ARG.
  * Keys (voxel and fine cell) are static_cast<short>(x / size) as the reference compiles on x86-64: the low 16 bits of the
@@ -435,7 +435,9 @@ int srl_color_map_stats(srl_color_map* cm, int64_t* n_voxels, int64_t* n_points,
                         int64_t* n_new_recent);
 /* the loop of addPointsToMap over the registered frame (:533-542): every add_point_step-th point, sweep order, through
  * addPointToColorMap (min_num_points = 0).  xyz_world: host or device, n*3 doubles.  to_rendering mirrors the flag of
- * addPointsToMap (clears voxels_recent_visited_temp first, publishes it to the renderer afterwards). */
+ * addPointsToMap (clears voxels_recent_visited_temp first, publishes it to the renderer afterwards).  A call without
+ * rendering updates the voxels' last-visited times but lists no voxel: the reference clears what such a call appends
+ * before it publishes anything.  So the recent list holds at most one entry per voxel. */
 int srl_color_map_add_points(srl_color_map* cm, const double* xyz_world, size_t n, int32_t add_point_step, double time_sweep_end,
                              double time_last_process, int32_t to_rendering, int64_t* n_stored);
 /* renderPointsInRecentVoxel: every point of every recently visited voxel is projected into the frame (pinhole, scale 1),

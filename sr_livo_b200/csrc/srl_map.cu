@@ -238,7 +238,7 @@ __global__ void k_first_in_cell(const unsigned long long* __restrict__ keys_sort
 // The colour map is a second voxel map (same slot table / block pool) whose points carry a colour estimate, plus
 //   * a fine occupancy set (cells of min_distance_points, the reference's Hash_map_3d hashmap_3d_points) that decides
 //     which stored points also enter rgb_points_vec, and
-//   * the list of voxels first visited by the current sweep(s) (voxels_recent_visited_temp), which the renderer walks.
+//   * the list of voxels the last rendering sweep visited first (voxels_recent_visited), which the renderer walks.
 // addPointToColorMap is sequential in the reference; the same (sort by voxel, replay per voxel in sweep order) scheme as K3
 // reproduces it: a voxel accepts the first (cap - count) offered points, a fine cell is claimed by the first ACCEPTED
 // point of the sweep that falls into it, and both lists are emitted in sweep order.
@@ -323,14 +323,13 @@ __global__ void k_color_seg_keys(const unsigned long long* __restrict__ keys, co
     const int s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s < *n_seg_p) seg_key[s] = keys[seg_start[s]];
 }
-// after sorting the visited voxels by the sweep position of their first point: append them to the recent list
+// after sorting the visited voxels by the sweep position of their first point: write them as the (emptied) recent list
 __global__ void k_color_append_recent(const unsigned int* __restrict__ first_sorted, const unsigned long long* __restrict__ key_sorted,
-                                      int n_seg, unsigned long long* recent, long long* counters, long long capacity) {
+                                      int n_seg, unsigned long long* recent, long long* counters) {
     const int t = blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= n_seg || first_sorted[t] == kNoIndex) return;
-    const long long base = counters[1];
-    if (base + t < capacity) recent[base + t] = key_sorted[t];
-    if (t + 1 == n_seg || first_sorted[t + 1] == kNoIndex) counters[3] = t + 1;   // how many were appended (applied by the host)
+    recent[t] = key_sorted[t];
+    if (t + 1 == n_seg || first_sorted[t + 1] == kNoIndex) counters[3] = t + 1;   // how many were listed (read by the host)
 }
 // accepted points only keep their fine key
 __global__ void k_color_mask_fine(unsigned long long* fkeys, const unsigned int* __restrict__ accept_id, long long m) {
@@ -817,13 +816,13 @@ struct srl_color_map {
     srl::VmArray rgb_mem;
     unsigned int* d_rgb_points = nullptr;   // rgb_points_vec: point ids (block * block_pts + index)
     size_t max_rgb_points = 0, committed_rgb_points = 0;
-    // per recent voxel (committed_recent of at most recent_capacity)
+    // per recent voxel (committed_recent of at most recent_capacity = max_voxels: a call lists each voxel at most once)
     srl::VmArray recent_temp_mem, recent_mem;
-    unsigned long long* d_recent_temp = nullptr;   // voxels_recent_visited_temp (packed keys)
+    unsigned long long* d_recent_temp = nullptr;   // voxels_recent_visited_temp of the current rendering call (packed keys)
     unsigned long long* d_recent = nullptr;        // map_tracker->voxels_recent_visited
     size_t recent_capacity = 0, committed_recent = 0;
-    long long* d_counters = nullptr;        // [0] rgb points, [1] recent_temp size, [2] scratch, [3] scratch
-    int64_t n_rgb_points = 0, n_recent_temp = 0, n_recent = 0, n_new_recent = 0;
+    long long* d_counters = nullptr;        // [0] rgb points, [3] recent voxels listed by the call
+    int64_t n_rgb_points = 0, n_recent = 0, n_new_recent = 0;
 };
 
 // the colour state of committed_voxels voxels (called by map_grow before the blocks grow)
@@ -1371,7 +1370,7 @@ int srl_color_map_create_growable(srl_ctx* ctx, double voxel_size, int32_t max_n
                                     : map_create(ctx, voxel_size, max_num_points_in_voxel, block_pts, initial_voxels, max_voxels, &cm->vox);
     if (rc != SRL_OK) { delete cm; return rc; }
     cm->max_rgb_points = max_voxels * (size_t)block_pts;
-    cm->recent_capacity = 4 * max_voxels + 1024;
+    cm->recent_capacity = max_voxels;
     cudaError_t e;
     if ((rc = vm_reserve(ctx, cm->cpts_mem, cm->max_rgb_points * sizeof(ColorPoint))) != SRL_OK ||
         (rc = vm_reserve(ctx, cm->last_visited_mem, max_voxels * sizeof(double))) != SRL_OK ||
@@ -1380,7 +1379,7 @@ int srl_color_map_create_growable(srl_ctx* ctx, double voxel_size, int32_t max_n
         (rc = vm_reserve(ctx, cm->recent_mem, cm->recent_capacity * sizeof(unsigned long long))) != SRL_OK ||
         (rc = color_map_grow_voxels(cm, initial_voxels)) != SRL_OK ||
         (rc = color_map_grow_rgb(cm, initial_voxels * (size_t)block_pts)) != SRL_OK ||
-        (rc = color_map_grow_recent(cm, 4 * initial_voxels + 1024)) != SRL_OK) {
+        (rc = color_map_grow_recent(cm, initial_voxels)) != SRL_OK) {
         srl_color_map_destroy(cm);
         return rc;
     }
@@ -1446,8 +1445,11 @@ int srl_color_map_add_points(srl_color_map* cm, const double* xyz_world, size_t 
     cudaStream_t st = ctx->stream;
     SRL_CUDA(ctx, cudaSetDevice(ctx->device));
     if (n_stored) *n_stored = 0;
-    if (to_rendering) cm->n_recent_temp = 0;                                   // :523-527
-    const int64_t recent_before = cm->n_recent_temp;                           // :529
+    // The reference appends to voxels_recent_visited_temp in every call, but only a rendering call publishes the list, and it
+    // clears it first (:523-527, :544-550): what a call without rendering appends is never read.  Such a call lists nothing;
+    // only its last_visited updates matter.  A rendering call lists each voxel at most once, so the list never outgrows
+    // max_voxels, and number_of_new_visited_voxel is its whole length.
+    int64_t n_listed = 0;
     const size_t msel = (n + (size_t)add_point_step - 1) / (size_t)add_point_step;   // points with idx % step == 0
     if (msel > 0x7fffffffULL) return set_err(ctx, SRL_BAD_ARG, "srl_color_map_add_points: too many points");
     if (msel) {
@@ -1493,23 +1495,20 @@ int srl_color_map_add_points(srl_color_map* cm, const double* xyz_world, size_t 
                                                   s.start, s.d_count, s.slot, s.is_new, (long long)msel, m->cap, m->block_pts, time_sweep_end,
                                                   time_last_process, accept_id, seg_first, m->d_counters);
             m->n_voxels += total_new;
-            // ---- recent list: the voxels this sweep visited for the first time, in the order of their first point
-            k_color_seg_keys<<<gs, T, 0, st>>>(s.keys_sorted, s.start, s.d_count, seg_key);
-            size_t tb = tmp_bytes;
-            cub::DeviceRadixSort::SortPairs(s.tmp, tb, seg_first, seg_first_sorted, seg_key, fk_b /* reused as sorted keys */, n_seg, 0, 32, st);
-            const long long host_cnt[4] = {cm->n_rgb_points, cm->n_recent_temp, 0, 0};
+            const long long host_cnt[4] = {cm->n_rgb_points, 0, 0, 0};
             SRL_CUDA(ctx, cudaMemcpyAsync(cm->d_counters, host_cnt, sizeof(host_cnt), cudaMemcpyHostToDevice, st));
-            // at most n_seg entries are appended; below the limit the committed list holds all of them, so only the limit
-            // itself can cut the list short (the SRL_MAP_FULL test below)
-            if ((rc = color_map_grow_recent(cm, (size_t)cm->n_recent_temp + (size_t)n_seg)) != SRL_OK) return rc;
-            k_color_append_recent<<<gs, T, 0, st>>>(seg_first_sorted, fk_b, n_seg, cm->d_recent_temp, cm->d_counters, (long long)cm->committed_recent);
-            long long appended = 0;
-            SRL_CUDA(ctx, cudaMemcpyAsync(&appended, cm->d_counters + 3, sizeof(long long), cudaMemcpyDeviceToHost, st));
+            size_t tb = tmp_bytes;
+            if (to_rendering) {
+                // ---- recent list: the voxels this sweep visited for the first time, in the order of their first point.
+                // n_seg <= n_voxels <= max_voxels entries at most.
+                k_color_seg_keys<<<gs, T, 0, st>>>(s.keys_sorted, s.start, s.d_count, seg_key);
+                cub::DeviceRadixSort::SortPairs(s.tmp, tb, seg_first, seg_first_sorted, seg_key, fk_b /* reused as sorted keys */, n_seg, 0, 32, st);
+                if ((rc = color_map_grow_recent(cm, (size_t)n_seg)) != SRL_OK) return rc;
+                k_color_append_recent<<<gs, T, 0, st>>>(seg_first_sorted, fk_b, n_seg, cm->d_recent_temp, cm->d_counters);
+                SRL_CUDA(ctx, cudaMemcpyAsync(&n_listed, cm->d_counters + 3, sizeof(long long), cudaMemcpyDeviceToHost, st));
+            }
             SRL_CUDA(ctx, cudaMemcpyAsync(&after, m->d_counters, sizeof(long long), cudaMemcpyDeviceToHost, st));
             SRL_CUDA(ctx, cudaStreamSynchronize(st));
-            if ((size_t)(cm->n_recent_temp + appended) > cm->recent_capacity)
-                return set_err(ctx, SRL_MAP_FULL, "srl_color_map_add_points: recent-voxel list exhausted (render or clear it)");
-            cm->n_recent_temp += appended;
             if (n_stored) *n_stored = after - before;
             // ---- rgb_points_vec: the first accepted point of the sweep in every still-free fine cell, in sweep order.
             // Every winner is a stored point, so the list and the fine set grow for the points just stored, before any claim.
@@ -1534,9 +1533,8 @@ int srl_color_map_add_points(srl_color_map* cm, const double* xyz_world, size_t 
         }
     }
     if (to_rendering) {                                                         // :544-550
-        if (cm->n_recent_temp) SRL_CUDA(ctx, cudaMemcpyAsync(cm->d_recent, cm->d_recent_temp, (size_t)cm->n_recent_temp * 8, cudaMemcpyDeviceToDevice, st));
-        cm->n_recent = cm->n_recent_temp;
-        cm->n_new_recent = cm->n_recent - recent_before;
+        if (n_listed) SRL_CUDA(ctx, cudaMemcpyAsync(cm->d_recent, cm->d_recent_temp, (size_t)n_listed * 8, cudaMemcpyDeviceToDevice, st));
+        cm->n_recent = cm->n_new_recent = n_listed;
     }
     SRL_CUDA(ctx, cudaStreamSynchronize(st));
     return SRL_OK;
