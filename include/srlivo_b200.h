@@ -532,6 +532,36 @@ int srl_lk_download_level(srl_lk* lk, int which, int level, uint8_t* img, int16_
 /* device time of the last srl_lk_track_image: image upload + pyramid + derivatives, then the point tracking (CUDA events) */
 int srl_lk_last_times(srl_lk* lk, double* pyramid_ms, double* track_ms);
 
+/* ---- the camera image preparation (DESIGN.md row N7): imageProcessing::process (src/imageProcessing.cpp:91-125,166-200) turns
+ * each BGR8 camera image into rgb_image (undistorted, Y-equalised in YCrCb, BGR8) and gray_image (undistorted, COLOR_RGB2GRAY,
+ * CLAHE clip 3), bit for bit OpenCV's initUndistortRectifyMap(CV_16SC2) / remap(INTER_LINEAR) / cvtColor / CLAHE. */
+typedef struct srl_image srl_image;
+typedef struct srl_image_params {
+    int32_t image_width, image_height;  /* camera_parameter.image_width / image_height of the yaml */
+    double camera_intrinsic[9];         /* K, row-major */
+    double camera_dist_coeffs[5];       /* k1, k2, p1, p2, k3 */
+} srl_image_params;
+/* the first-image step (:93-104) for inputs of cols x rows: image_scale_factor = image_width / cols, fx, cx, fy, cy divided by
+ * it, the output (image_width / s, image_height / s) truncated, the CLAHE grid t = (int)max(out_cols * 32 / 640, 4) in both
+ * dimensions, and the undistortion map.  SRL_BAD_ARG for a non-positive size, a side over 32767, an output under 16 x 16,
+ * non-finite parameters or an intrinsic matrix without a finite inverse. */
+int srl_image_create(srl_ctx* ctx, const srl_image_params* params, int cols, int rows, srl_image** out);
+void srl_image_destroy(srl_image* img);
+/* process:120-125 for one image: bgr is cols x rows BGR8, rows `pitch` bytes apart (pitch >= cols * 3); rgb_out receives
+ * out_cols * out_rows * 3 bytes (BGR8, rgb_image), gray_out out_cols * out_rows bytes (gray_image), both contiguous.  Every
+ * buffer is host or device memory.  SRL_BAD_ARG for another size than the one given at creation, a short pitch or a NULL
+ * buffer; the object stays usable. */
+int srl_image_process(srl_image* img, const uint8_t* bgr, int cols, int rows, size_t pitch, uint8_t* rgb_out, uint8_t* gray_out);
+/* the output size, the CLAHE grid, image_scale_factor and the scaled intrinsics (row-major): the ones srl_camera and the
+ * vision updates must use.  Any output may be NULL. */
+int srl_image_info(srl_image* img, int32_t* out_cols, int32_t* out_rows, int32_t* tiles, double* scale_factor, double intrinsic[9]);
+/* test hook: the undistortion map as OpenCV's CV_16SC2 + CV_16UC1 pair: map1 out_cols * out_rows (x, y) int16 pairs, map2
+ * out_cols * out_rows uint16 (either may be NULL; host or device) */
+int srl_image_download_maps(srl_image* img, int16_t* map1, uint16_t* map2);
+/* device time of the last srl_image_process: the input upload (0 for a device image), remap + colour planes, both CLAHEs
+ * (CUDA events) */
+int srl_image_last_times(srl_image* img, double* upload_ms, double* remap_ms, double* clahe_ms);
+
 /* eskfEstimator::observe (src/eskfEstimator.cpp:219-230) — host math, exported for parity tests */
 int srl_eskf_observe(srl_eskf_state* eskf, const double d_x[17]);
 

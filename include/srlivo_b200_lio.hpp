@@ -22,6 +22,7 @@
 //   pubColorPoints / saveColorPoints  src/lioOptimization.cpp:1210,1386 srl::LioBackend::pubColorPoints / saveColorPoints
 //   rgbMapTracker::selectPointsForProjection src/rgbMapTracker.cpp:45 srl::LioBackend::selectPointsForProjection / gatherColorPoints
 //   LKOpticalFlowKernel::trackImage   src/lkpyramid.cpp:755         srl::LKOpticalFlowKernel::trackImage (on LioBackend::context())
+//   imageProcessing::process :91-125  src/imageProcessing.cpp:91    srl::ImageProcessing (undistortion, grey, CLAHE; on LioBackend::context())
 #pragma once
 
 #include <array>
@@ -335,6 +336,51 @@ public:
 private:
     srl_ctx* ctx_ = nullptr;
     srl_lk* lk_ = nullptr;
+    void check(int rc, const char* what) {
+        if (rc != SRL_OK) throw std::runtime_error(std::string(what) + ": " + (ctx_ ? srl_last_error(ctx_) : "no context"));
+    }
+};
+
+// The image preparation of imageProcessing::process (src/imageProcessing.cpp:91-125) on the GPU, bit for bit OpenCV's: the
+// constructor is the first-image step for inputs of cols x rows, process() turns one BGR8 image into rgb_image (BGR8) and
+// gray_image.  Every pointer takes host or device memory; outputs are contiguous, outputSize() in pixels.  The object must be
+// destroyed before its context.
+class ImageProcessing {
+public:
+    ImageProcessing(srl_ctx* ctx, int image_width, int image_height, const std::array<double, 9>& camera_intrinsic,
+                    const std::array<double, 5>& camera_dist_coeffs, int cols, int rows)
+        : ctx_(ctx) {
+        srl_image_params p{};
+        p.image_width = image_width;
+        p.image_height = image_height;
+        std::memcpy(p.camera_intrinsic, camera_intrinsic.data(), sizeof(p.camera_intrinsic));
+        std::memcpy(p.camera_dist_coeffs, camera_dist_coeffs.data(), sizeof(p.camera_dist_coeffs));
+        check(srl_image_create(ctx, &p, cols, rows, &img_), "srl_image_create");
+    }
+    ~ImageProcessing() { if (img_) srl_image_destroy(img_); }
+    ImageProcessing(const ImageProcessing&) = delete;
+    ImageProcessing& operator=(const ImageProcessing&) = delete;
+
+    // process:120-125: bgr rows are `pitch` bytes apart (a cv::Mat's step, a ROS image's step)
+    void process(const uint8_t* bgr, int cols, int rows, size_t pitch, uint8_t* rgb_out, uint8_t* gray_out) {
+        check(srl_image_process(img_, bgr, cols, rows, pitch, rgb_out, gray_out), "srl_image_process");
+    }
+    // (out_cols, out_rows): the size of rgb_image and gray_image
+    std::array<int, 2> outputSize() {
+        int32_t c = 0, r = 0;
+        check(srl_image_info(img_, &c, &r, nullptr, nullptr, nullptr), "srl_image_info");
+        return {c, r};
+    }
+    // the intrinsics divided by image_scale_factor (row-major), as camera_intrinsic holds them after the first image
+    std::array<double, 9> cameraIntrinsic() {
+        std::array<double, 9> k{};
+        check(srl_image_info(img_, nullptr, nullptr, nullptr, nullptr, k.data()), "srl_image_info");
+        return k;
+    }
+
+private:
+    srl_ctx* ctx_ = nullptr;
+    srl_image* img_ = nullptr;
     void check(int rc, const char* what) {
         if (rc != SRL_OK) throw std::runtime_error(std::string(what) + ": " + (ctx_ ? srl_last_error(ctx_) : "no context"));
     }

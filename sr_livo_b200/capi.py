@@ -77,6 +77,12 @@ class LkParams(C.Structure):
                 ("epsilon", C.c_double), ("flags", C.c_int32), ("min_eig_threshold", C.c_double)]
 
 
+class ImageParams(C.Structure):
+    """srl_image_params: the yaml's camera_parameter values imageProcessing is given (src/imageProcessing.cpp:32-53)."""
+    _fields_ = [("image_width", C.c_int32), ("image_height", C.c_int32), ("camera_intrinsic", C.c_double * 9),
+                ("camera_dist_coeffs", C.c_double * 5)]
+
+
 class ProjectionParams(C.Structure):
     """srl_projection_params: the arguments of rgbMapTracker::selectPointsForProjection and the tracker's depth bounds."""
     _fields_ = [("minimum_dis", C.c_double), ("skip_step", C.c_int32), ("use_all_points", C.c_int32), ("minimum_depth", C.c_double),
@@ -127,6 +133,7 @@ EXPORTS = [
     "srl_build_frame", "srl_shuffle_replay", "srl_map_insert_published", "srl_map_insert_sweep_published", "srl_color_map_export",
     "srl_color_map_select_for_projection", "srl_color_map_gather_points",
     "srl_lk_create", "srl_lk_destroy", "srl_lk_track_image", "srl_lk_info", "srl_lk_download_level", "srl_lk_last_times",
+    "srl_image_create", "srl_image_destroy", "srl_image_process", "srl_image_info", "srl_image_download_maps", "srl_image_last_times",
 ]
 
 _lib = None
@@ -229,6 +236,13 @@ def lib():
     L.srl_lk_info.argtypes = [vp] + [C.POINTER(i32)] * 3
     L.srl_lk_download_level.argtypes = [vp, C.c_int, C.c_int, vp, vp]
     L.srl_lk_last_times.argtypes = [vp, C.POINTER(dbl), C.POINTER(dbl)]
+    L.srl_image_create.argtypes = [vp, C.POINTER(ImageParams), C.c_int, C.c_int, C.POINTER(vp)]
+    L.srl_image_destroy.argtypes = [vp]
+    L.srl_image_destroy.restype = None
+    L.srl_image_process.argtypes = [vp, vp, C.c_int, C.c_int, sz, vp, vp]
+    L.srl_image_info.argtypes = [vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), C.POINTER(dbl), vp]
+    L.srl_image_download_maps.argtypes = [vp, vp, vp]
+    L.srl_image_last_times.argtypes = [vp, C.POINTER(dbl), C.POINTER(dbl), C.POINTER(dbl)]
     L.srl_cloud_frame_create.argtypes = [vp, sz, C.POINTER(vp)]
     L.srl_cloud_frame_destroy.argtypes = [vp]
     L.srl_cloud_frame_destroy.restype = None

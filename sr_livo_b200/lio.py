@@ -13,6 +13,7 @@ Names and argument meaning follow the reference so the parity tests read like it
   pubColorPoints / saveColorPoints      src/lioOptimization.cpp:1210,1386 -> ColorVoxelMap.pubColorPoints / saveColorPoints
   rgbMapTracker::selectPointsForProjection src/rgbMapTracker.cpp:45     -> ColorVoxelMap.selectPointsForProjection / gatherPoints
   LKOpticalFlowKernel::trackImage       src/lkpyramid.cpp:755           -> LKOpticalFlowKernel.trackImage
+  imageProcessing::process (:91-125)    src/imageProcessing.cpp:91      -> ImageProcessing.process
 
 Error behaviour: optimizeSummary.success=false <-> OptimizeSummary.success False (SRL_TOO_FEW_RESIDUALS);
 the reference's `throw std::runtime_error("error")` on NaN planarity <-> RuntimeError; everything else raises
@@ -283,14 +284,20 @@ class ColorVoxelMap:
         return stored.value
 
     def renderPointsInRecentVoxel(self, camera: "capi.Camera", image_bgr, obs_time: float) -> int:
-        """rgbMapTracker::renderPointsInRecentVoxel (srl_color_map_render_recent) with a (rows, cols, 3) BGR8 host image; returns
+        """rgbMapTracker::renderPointsInRecentVoxel (srl_color_map_render_recent) with a (rows, cols, 3) BGR8 image: a numpy array,
+        or a contiguous torch.uint8 tensor on the host or a CUDA device (ImageProcessing.process's rgb output as it is); returns
         render_point_count.  camera.fov_margin must be >= 0 (SRL_BAD_ARG otherwise, NaN included, and the map is untouched):
         a negative margin would sample outside the image, which the reference leaves undefined.  The selection
         (selectPointsForProjection) still takes negative margins."""
-        img = np.ascontiguousarray(image_bgr, np.uint8)
-        assert img.shape == (camera.rows, camera.cols, 3)
+        if _is_tensor(image_bgr):
+            assert tuple(image_bgr.shape) == (camera.rows, camera.cols, 3)
+            p_img, _ = _addr(image_bgr, np.uint8, 3)
+        else:
+            img = np.ascontiguousarray(image_bgr, np.uint8)
+            assert img.shape == (camera.rows, camera.cols, 3)
+            p_img = img.ctypes.data
         n = C.c_int64(0)
-        _check(self.ctx.h, lib().srl_color_map_render_recent(self.h, C.byref(camera), ptr(img), float(obs_time), C.byref(n)))
+        _check(self.ctx.h, lib().srl_color_map_render_recent(self.h, C.byref(camera), C.c_void_p(p_img), float(obs_time), C.byref(n)))
         return n.value
 
     def exportColorPoints(self, min_views: int = 1, order: int = 0, xyz=None, rgb=None):
@@ -861,6 +868,114 @@ class LKOpticalFlowKernel:
         return a.value, b.value
 
 
+def r3live_camera_params() -> dict:
+    """camera_parameter of config/r3live.yaml (and r3live_compressed.yaml): a 1280 x 1024 camera."""
+    return dict(image_width=1280, image_height=1024, camera_intrinsic=[863.4241, 0.0, 640.6808, 0.0, 863.4171, 518.3392, 0.0, 0.0, 1.0],
+                camera_dist_coeffs=[-0.1080, 0.1050, -1.2872e-04, 5.7923e-05, -0.0222])
+
+
+def ntu_camera_params() -> dict:
+    """camera_parameter of config/ntu.yaml: a 752 x 480 camera."""
+    return dict(image_width=752, image_height=480, camera_intrinsic=[425.0259, 0.0, 386.0152, 0.0, 426.7976, 241.9130, 0.0, 0.0, 1.0],
+                camera_dist_coeffs=[-0.2881, 0.0746, 7.7845e-04, -2.2779e-04, 0.0])
+
+
+def _image_2d(img, what):
+    """(address, rows, cols, row pitch in bytes) of a (rows, cols, 3) uint8 image with contiguous pixels; rows may be padded."""
+    if _is_tensor(img):
+        if str(img.dtype) != "torch.uint8" or img.dim() != 3 or img.shape[2] != 3 or img.stride(2) != 1 or img.stride(1) != 3:
+            raise TypeError(f"{what}: expected a (rows, cols, 3) torch.uint8 image with contiguous pixels")
+        return img.data_ptr(), img.shape[0], img.shape[1], img.stride(0)
+    if not (isinstance(img, np.ndarray) and img.dtype == np.uint8 and img.ndim == 3 and img.shape[2] == 3 and img.strides[2] == 1
+            and img.strides[1] == 3):
+        raise TypeError(f"{what}: expected a (rows, cols, 3) uint8 array with contiguous pixels")
+    return img.ctypes.data, img.shape[0], img.shape[1], img.strides[0]
+
+
+class ImageProcessing:
+    """The image preparation of imageProcessing::process (src/imageProcessing.cpp:91-125,166-200, srl_image_*) on the GPU, bit for
+    bit OpenCV's: undistortion (initUndistortRectifyMap CV_16SC2 + remap INTER_LINEAR), COLOR_RGB2GRAY and CLAHE clip 3 for
+    gray_image, BGR2YCrCb, CLAHE clip 1 on Y and YCrCb2BGR for rgb_image.  Construction is the first-image step for inputs of
+    cols x rows (the yaml's size unless given): the scale factor, the scaled intrinsics (camera_intrinsic()) and the map.
+    ImageProcessing(ctx, **r3live_camera_params())."""
+
+    def __init__(self, ctx: Context, image_width: int, image_height: int, camera_intrinsic, camera_dist_coeffs, cols: int | None = None,
+                 rows: int | None = None):
+        self.ctx = ctx
+        k = np.asarray(camera_intrinsic, np.float64).reshape(-1)
+        d = np.asarray(camera_dist_coeffs, np.float64).reshape(-1)
+        if k.size != 9 or d.size != 5:
+            raise ValueError("camera_intrinsic has 9 values and camera_dist_coeffs 5")
+        self.params = capi.ImageParams(int(image_width), int(image_height), (C.c_double * 9)(*k), (C.c_double * 5)(*d))
+        self.input_size = (int(image_width if cols is None else cols), int(image_height if rows is None else rows))
+        h = C.c_void_p()
+        _check(ctx.h, lib().srl_image_create(ctx.h, C.byref(self.params), self.input_size[0], self.input_size[1], C.byref(h)))
+        self.h = h
+
+    def close(self):
+        if getattr(self, "h", None):
+            lib().srl_image_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def _info(self):
+        c, r, t, s, k = C.c_int32(0), C.c_int32(0), C.c_int32(0), C.c_double(0), np.zeros(9, np.float64)
+        _check(self.ctx.h, lib().srl_image_info(self.h, C.byref(c), C.byref(r), C.byref(t), C.byref(s), ptr(k)))
+        return c.value, r.value, t.value, s.value, k
+
+    def output_size(self) -> tuple[int, int]:
+        """(out_cols, out_rows) of rgb_image and gray_image."""
+        return self._info()[:2]
+
+    def tiles(self) -> int:
+        """CLAHE's grid: tiles x tiles."""
+        return self._info()[2]
+
+    def scale_factor(self) -> float:
+        """image_scale_factor = image_width / input cols."""
+        return self._info()[3]
+
+    def camera_intrinsic(self) -> np.ndarray:
+        """(3, 3) K with fx, cx, fy, cy divided by the scale factor: what srl_camera and the vision updates use."""
+        return self._info()[4].reshape(3, 3)
+
+    def process(self, image_bgr, out=None):
+        """process:120-125 for one (rows, cols, 3) BGR8 image (numpy or torch, host or CUDA; rows may be padded, as a ROS step is):
+        (rgb_image (out_rows, out_cols, 3) BGR8, gray_image (out_rows, out_cols)).  out = (rgb, gray) buffers (contiguous, numpy or
+        torch, host or CUDA) receive them; without it numpy arrays are returned."""
+        p_img, rows, cols, pitch = _image_2d(image_bgr, "image_bgr")
+        oc, orows = self.output_size()
+        if out is None:
+            rgb, gray = np.empty((orows, oc, 3), np.uint8), np.empty((orows, oc), np.uint8)
+        else:
+            rgb, gray = out
+        p_rgb, n_rgb = _addr(rgb, np.uint8, 3)
+        p_gray, n_gray = _addr(gray, np.uint8, 1)
+        if n_rgb < oc * orows or n_gray < oc * orows:
+            raise ValueError(f"out buffers must hold {orows} x {oc} pixels")
+        _check(self.ctx.h, lib().srl_image_process(self.h, C.c_void_p(p_img), int(cols), int(rows), int(pitch), C.c_void_p(p_rgb),
+                                                   C.c_void_p(p_gray)))
+        return rgb, gray
+
+    def maps(self):
+        """Test hook: (map1 (out_rows, out_cols, 2) int16, map2 (out_rows, out_cols) uint16), OpenCV's CV_16SC2 + CV_16UC1 pair."""
+        oc, orows = self.output_size()
+        m1, m2 = np.zeros((orows, oc, 2), np.int16), np.zeros((orows, oc), np.uint16)
+        _check(self.ctx.h, lib().srl_image_download_maps(self.h, ptr(m1), ptr(m2)))
+        return m1, m2
+
+    def last_times(self) -> tuple[float, float, float]:
+        """(upload ms, remap + colour planes ms, both CLAHEs ms) of the last process, CUDA events."""
+        a, b, c = C.c_double(0), C.c_double(0), C.c_double(0)
+        _check(self.ctx.h, lib().srl_image_last_times(self.h, C.byref(a), C.byref(b), C.byref(c)))
+        return a.value, b.value, c.value
+
+
 __all__ = ["Context", "VoxelHashMap", "ColorVoxelMap", "Sweep", "EskfEstimator", "LioOptimization", "OptimizeSummary", "PlaneResiduals",
            "IcpParams", "r3live_params", "r3live_map_options", "r3live_compressed_map_options", "make_frame", "SrlError", "write_pcd_xyzrgb",
-           "LKOpticalFlowKernel", "tracker_lk_params"]
+           "LKOpticalFlowKernel", "tracker_lk_params", "ImageProcessing", "r3live_camera_params", "ntu_camera_params"]
