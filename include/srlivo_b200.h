@@ -562,6 +562,44 @@ int srl_image_download_maps(srl_image* img, int16_t* map1, uint16_t* map2);
  * (CUDA events) */
 int srl_image_last_times(srl_image* img, double* upload_ms, double* remap_ms, double* clahe_ms);
 
+/* ---- the two camera updates of process (DESIGN.md row N8): imageProcessing::vioEsikf (src/imageProcessing.cpp:220-380) and
+ * vioPhotometric (:402-552) with the reference's constants (2 iterations, intrinsics and extrinsics estimated, at least 10
+ * points, Huber threshold 1), over the colour map's points.  The handle keeps imageProcessing::covariance (11 x 11, row-major,
+ * setInitialCov at creation); vioPhotometric reads and writes its block (1..6, 1..6). */
+typedef struct srl_vio_state {   /* the p_state fields the two updates read and write (include/state.h) */
+    double rotation[4];          /* x, y, z, w: the IMU's orientation in the world */
+    double translation[3];
+    double R_imu_camera[9];      /* row-major */
+    double t_imu_camera[3];
+    double fx, fy, cx, cy, time_td;
+    double q_world_camera[4];    /* x, y, z, w */
+    double t_world_camera[3];
+    double q_camera_world[4];    /* iteration 0 projects with these two, as given */
+    double t_camera_world[3];
+} srl_vio_state;
+/* vioEsikf over the tracked set in the caller's order: ids (n colour-map point ids), uv (n matched (u, v) float pairs) and
+ * velocity (n image_velocity (du, dv) double pairs).  The positions come from the colour map as stored floats.  n_new_visited
+ * is map_tracker->number_of_new_visited_voxel: cam_measurement_weight = max(0.001, min(5.0 / n_new_visited, 0.01)).  *result
+ * is the reference's return value; state and covariance are updated in place when it is 1.  n < 10: *result = 0 and nothing
+ * changes.  ids, uv and velocity are host or device memory.  SRL_BAD_ARG (nothing written) for an id that names no stored
+ * point; SRL_SINGULAR (nothing written) for a zero or NaN pivot of the update's 11 x 11 system. */
+int srl_image_vio_esikf(srl_image* img, srl_color_map* cm, srl_vio_state* state, const uint32_t* ids, const float* uv,
+                        const double* velocity, size_t n, int32_t n_new_visited, int32_t* result);
+/* vioPhotometric on the prepared rgb_image `bgr` (BGR8, cols x rows, rows `pitch` bytes apart, host or device): each point with
+ * N_rgb >= 3 compares its colour state with the image's at its projection.  The image must have the handle's output size
+ * (srl_image_info), else SRL_BAD_ARG.  Image reads are clamped to the nearest row and column.  Otherwise as
+ * srl_image_vio_esikf (6 x 6 system); with fewer than 10 points of N_rgb >= 3 it returns *result = 1 and changes nothing. */
+int srl_image_vio_photometric(srl_image* img, srl_color_map* cm, srl_vio_state* state, const uint32_t* ids, const double* velocity,
+                              size_t n, int32_t n_new_visited, const uint8_t* bgr, int cols, int rows, size_t pitch, int32_t* result);
+/* imageProcessing::covariance: `set` (121 doubles, row-major) replaces it, then `get` receives it; either may be NULL */
+int srl_image_covariance(srl_image* img, const double* set, double* get);
+/* what the last call of each update did: iterations run (0 when it returned before iterating), points used in its last
+ * iteration, its last acc_residual as the reference's convergence tests read it; which = 0 vioEsikf, 1 vioPhotometric.  Any
+ * output may be NULL; SRL_BAD_ARG before the first launch of that update. */
+int srl_image_vio_last_summary(srl_image* img, int32_t which, int32_t* iterations, int32_t* points_used, double* acc_residual);
+/* device time of the last launch of each update (CUDA events around the kernel; inputs and the result copy excluded) */
+int srl_image_vio_last_times(srl_image* img, double* esikf_ms, double* photometric_ms);
+
 /* eskfEstimator::observe (src/eskfEstimator.cpp:219-230) — host math, exported for parity tests */
 int srl_eskf_observe(srl_eskf_state* eskf, const double d_x[17]);
 

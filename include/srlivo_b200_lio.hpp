@@ -377,6 +377,29 @@ public:
         check(srl_image_info(img_, nullptr, nullptr, nullptr, nullptr, k.data()), "srl_image_info");
         return k;
     }
+    // imageProcessing::vioEsikf over the tracked set in the caller's order (ids, matched uv float pairs, image_velocity double
+    // pairs; host or device); `state` is updated in place, the covariance inside the handle
+    bool vioEsikf(srl_color_map* cm, srl_vio_state& state, const uint32_t* ids, const float* uv, const double* velocity, size_t n,
+                  int n_new_visited) {
+        int32_t r = 0;
+        check(srl_image_vio_esikf(img_, cm, &state, ids, uv, velocity, n, n_new_visited, &r), "srl_image_vio_esikf");
+        return r != 0;
+    }
+    // imageProcessing::vioPhotometric on the prepared rgb_image (outputSize(), rows `pitch` bytes apart; host or device)
+    bool vioPhotometric(srl_color_map* cm, srl_vio_state& state, const uint32_t* ids, const double* velocity, size_t n, int n_new_visited,
+                        const uint8_t* bgr, int cols, int rows, size_t pitch) {
+        int32_t r = 0;
+        check(srl_image_vio_photometric(img_, cm, &state, ids, velocity, n, n_new_visited, bgr, cols, rows, pitch, &r),
+              "srl_image_vio_photometric");
+        return r != 0;
+    }
+    // imageProcessing::covariance, 11 x 11 row-major
+    std::array<double, 121> covariance() {
+        std::array<double, 121> c{};
+        check(srl_image_covariance(img_, nullptr, c.data()), "srl_image_covariance");
+        return c;
+    }
+    void setCovariance(const std::array<double, 121>& c) { check(srl_image_covariance(img_, c.data(), nullptr), "srl_image_covariance"); }
 
 private:
     srl_ctx* ctx_ = nullptr;

@@ -83,6 +83,14 @@ class ImageParams(C.Structure):
                 ("camera_dist_coeffs", C.c_double * 5)]
 
 
+class VioState(C.Structure):
+    """srl_vio_state: the p_state fields vioEsikf / vioPhotometric read and write (include/state.h); quaternions x, y, z, w."""
+    _fields_ = [("rotation", C.c_double * 4), ("translation", C.c_double * 3), ("R_imu_camera", C.c_double * 9),
+                ("t_imu_camera", C.c_double * 3), ("fx", C.c_double), ("fy", C.c_double), ("cx", C.c_double), ("cy", C.c_double),
+                ("time_td", C.c_double), ("q_world_camera", C.c_double * 4), ("t_world_camera", C.c_double * 3),
+                ("q_camera_world", C.c_double * 4), ("t_camera_world", C.c_double * 3)]
+
+
 class ProjectionParams(C.Structure):
     """srl_projection_params: the arguments of rgbMapTracker::selectPointsForProjection and the tracker's depth bounds."""
     _fields_ = [("minimum_dis", C.c_double), ("skip_step", C.c_int32), ("use_all_points", C.c_int32), ("minimum_depth", C.c_double),
@@ -134,6 +142,7 @@ EXPORTS = [
     "srl_color_map_select_for_projection", "srl_color_map_gather_points",
     "srl_lk_create", "srl_lk_destroy", "srl_lk_track_image", "srl_lk_info", "srl_lk_download_level", "srl_lk_last_times",
     "srl_image_create", "srl_image_destroy", "srl_image_process", "srl_image_info", "srl_image_download_maps", "srl_image_last_times",
+    "srl_image_vio_esikf", "srl_image_vio_photometric", "srl_image_covariance", "srl_image_vio_last_summary", "srl_image_vio_last_times",
 ]
 
 _lib = None
@@ -243,6 +252,11 @@ def lib():
     L.srl_image_info.argtypes = [vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), C.POINTER(dbl), vp]
     L.srl_image_download_maps.argtypes = [vp, vp, vp]
     L.srl_image_last_times.argtypes = [vp, C.POINTER(dbl), C.POINTER(dbl), C.POINTER(dbl)]
+    L.srl_image_vio_esikf.argtypes = [vp, vp, C.POINTER(VioState), vp, vp, vp, sz, i32, C.POINTER(i32)]
+    L.srl_image_vio_photometric.argtypes = [vp, vp, C.POINTER(VioState), vp, vp, sz, i32, vp, C.c_int, C.c_int, sz, C.POINTER(i32)]
+    L.srl_image_covariance.argtypes = [vp, vp, vp]
+    L.srl_image_vio_last_summary.argtypes = [vp, i32, C.POINTER(i32), C.POINTER(i32), C.POINTER(dbl)]
+    L.srl_image_vio_last_times.argtypes = [vp, C.POINTER(dbl), C.POINTER(dbl)]
     L.srl_cloud_frame_create.argtypes = [vp, sz, C.POINTER(vp)]
     L.srl_cloud_frame_destroy.argtypes = [vp]
     L.srl_cloud_frame_destroy.restype = None

@@ -20,6 +20,12 @@ constexpr int kBlockFloats = 80;   // 320 B
 constexpr int kBlockCap = 20;      // max_num_points_in_voxel supported by the block layout (all reference configs use 20)
 constexpr int kMetaKeyLo = 0 * 4 + 3, kMetaKeyHi = 1 * 4 + 3, kMetaCount = 2 * 4 + 3;   // float index of the w lanes used
 
+struct ColorPoint {            // colour state of one stored point of a colour map (rgbPoint minus position), index = block * block_pts + i
+    short rgb[3]; short n_rgb;
+    float cov[3]; float pad;
+    double obs_dist, last_obs;
+};
+
 struct __align__(16) Slot {
     unsigned long long key;   // 0 = empty
     unsigned int block;

@@ -229,22 +229,6 @@ bool inv3(const double* m, double* o) {
 
 }  // namespace
 
-struct srl_image {
-    srl_ctx* ctx = nullptr;
-    int device = 0;
-    int in_cols = 0, in_rows = 0;      // the input size fixed at creation
-    int cols = 0, rows = 0;            // the output size
-    int tiles = 0, tw = 0, th = 0;     // CLAHE's grid and its tile size
-    double scale = 1.;                 // image_scale_factor
-    double K[9] = {0};                 // the scaled intrinsics
-    short2* map1 = nullptr;
-    uint16_t* map2 = nullptr;
-    uint8_t* planes = nullptr;
-    uint8_t* lut = nullptr;
-    cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};   // call start, image uploaded, remapped, equalised
-    bool timed = false;
-};
-
 extern "C" {
 
 int srl_image_create(srl_ctx* ctx, const srl_image_params* p, int cols, int rows, srl_image** out) {
@@ -272,6 +256,7 @@ int srl_image_create(srl_ctx* ctx, const srl_image_params* p, int cols, int rows
     auto* im = new srl_image;
     im->ctx = ctx;
     im->device = ctx->device;
+    vio_initial_covariance(im->cov);
     im->in_cols = cols;
     im->in_rows = rows;
     im->cols = (int)oc;
@@ -292,6 +277,8 @@ int srl_image_create(srl_ctx* ctx, const srl_image_params* p, int cols, int rows
     if (e == cudaSuccess) e = cudaMalloc(&im->planes, n * kImgPlanes);
     if (e == cudaSuccess) e = cudaMalloc(&im->lut, (size_t)2 * t * t * 256);
     for (int i = 0; i < 4 && e == cudaSuccess; ++i) e = cudaEventCreate(&im->ev[i]);
+    for (int i = 0; i < 4 && e == cudaSuccess; ++i) e = cudaEventCreate(&im->vio_ev[i]);
+    if (e == cudaSuccess) e = cudaMalloc(&im->d_vio_out, sizeof(srl::VioOut));
     if (e == cudaSuccess) {
         MapArgs a = {};
         for (int k = 0; k < 9; ++k) a.ir[k] = ir[k];
@@ -328,7 +315,10 @@ void srl_image_destroy(srl_image* im) {
     if (im->map2) cudaFree(im->map2);
     if (im->planes) cudaFree(im->planes);
     if (im->lut) cudaFree(im->lut);
+    if (im->d_vio_out) cudaFree(im->d_vio_out);
     for (auto& e : im->ev)
+        if (e) cudaEventDestroy(e);
+    for (auto& e : im->vio_ev)
         if (e) cudaEventDestroy(e);
     delete im;
 }

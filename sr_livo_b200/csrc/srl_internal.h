@@ -311,6 +311,53 @@ __device__ __forceinline__ void finalise_pass(const PassArgs& A, bool forward, d
 }
 #endif
 
+#if defined(__CUDACC__)
+__device__ __forceinline__ unsigned char sat_u8(double v) {       // cv::saturate_cast<uchar>(double): cvRound (half to even), clamp
+    const long long r = __double2ll_rn(v);
+    return (unsigned char)(r < 0 ? 0 : (r > 255 ? 255 : r));
+}
+__device__ __forceinline__ unsigned char sat_add_u8(unsigned char a, unsigned char b) { const int r = (int)a + (int)b; return (unsigned char)(r > 255 ? 255 : r); }
+// an image index from a floored coordinate, clamped to [0, n - 1] (NaN to 0): every tap stays inside the image
+__device__ __forceinline__ int clamp_tap(double f, int n) { return f >= (double)(n - 1) ? n - 1 : (f > 0.0 ? (int)f : 0); }
+// getSubPixel<cv::Vec3b>(mat, row, col) (src/lioOptimization.cpp:71-98) of a BGR8 image: four saturated products and three
+// saturated sums per channel, the taps (floor | floor + 1) clamped to the nearest row and column.  Inside the image (row, col
+// >= 0 and floor + 1 within it, or a zero weight on the +1 tap) the values are the reference's.  The renderer and the
+// photometric camera update sample through it.
+__device__ __forceinline__ void sub_pixel_bgr(const unsigned char* __restrict__ img, size_t pitch, int cols, int rows, double row, double col,
+                                              unsigned char out[3]) {
+    const double fr = floor(row), fc = floor(col);
+    const double frac_r = __dsub_rn(row, fr), frac_c = __dsub_rn(col, fc);
+    const double w00 = __dmul_rn(__dsub_rn(1.0, frac_r), __dsub_rn(1.0, frac_c)), w10 = __dmul_rn(frac_r, __dsub_rn(1.0, frac_c));
+    const double w01 = __dmul_rn(__dsub_rn(1.0, frac_r), frac_c), w11 = __dmul_rn(frac_r, frac_c);
+    const int r0 = clamp_tap(fr, rows), r1 = clamp_tap(__dadd_rn(fr, 1.0), rows);
+    const int c0 = clamp_tap(fc, cols), c1 = clamp_tap(__dadd_rn(fc, 1.0), cols);
+    const unsigned char* p00 = img + (size_t)r0 * pitch + (size_t)c0 * 3;
+    const unsigned char* p10 = img + (size_t)r1 * pitch + (size_t)c0 * 3;
+    const unsigned char* p01 = img + (size_t)r0 * pitch + (size_t)c1 * 3;
+    const unsigned char* p11 = img + (size_t)r1 * pitch + (size_t)c1 * 3;
+#pragma unroll
+    for (int ch = 0; ch < 3; ++ch) {
+        const unsigned char a = sat_u8(__dmul_rn((double)p00[ch], w00));
+        const unsigned char b = sat_u8(__dmul_rn((double)p10[ch], w10));
+        const unsigned char cc = sat_u8(__dmul_rn((double)p01[ch], w01));
+        const unsigned char d = sat_u8(__dmul_rn((double)p11[ch], w11));
+        out[ch] = sat_add_u8(sat_add_u8(sat_add_u8(a, b), cc), d);
+    }
+}
+#endif
+
+// A colour map's stored points as the camera updates read them (srl_map.cu owns the map): position of point id in
+// blocks[(id / block_pts) * 4 * block_pts + 4 * (id % block_pts)], colour state in cpts[id]; an id is valid when its block is
+// below n_voxels and its index below the block's count.
+struct ColorMapView {
+    const float* blocks;
+    const ColorPoint* cpts;
+    int block_pts;
+    long long n_voxels;
+};
+ColorMapView color_map_view(const srl_color_map* cm);
+srl_ctx* color_map_ctx(const srl_color_map* cm);
+
 // Which compiled instance of each pass kernel a ctx launches, and the state of its sweep-order sort.  Filled once by
 // srl_ctx_create (defaults, then the SRL_* environment variables), changed by srl_ctx_set_option.
 struct KernelChoice {
@@ -419,6 +466,43 @@ struct srl_ctx {
     size_t scratch_bytes = 0;
     void* h_pinned = nullptr;
     size_t pinned_bytes = 0;
+};
+
+namespace srl {
+// What one launch of a camera update (srl_vio.cu) hands back in one device-to-host copy
+struct VioOut {
+    srl_vio_state state;
+    double cov[121];               // the whole 11 x 11 covariance (the photometric update rewrites its 6 x 6 block)
+    double acc_residual;           // of the last iteration run
+    int status;                    // SRL_OK, SRL_BAD_ARG (an id names no stored point), SRL_SINGULAR
+    int result;                    // the reference's return value
+    int iterations, points_used;
+};
+// imageProcessing::setInitialCov (src/imageProcessing.cpp:65-72)
+void vio_initial_covariance(double cov[121]);
+}  // namespace srl
+
+struct srl_image {
+    srl_ctx* ctx = nullptr;
+    int device = 0;
+    int in_cols = 0, in_rows = 0;      // the input size fixed at creation
+    int cols = 0, rows = 0;            // the output size
+    int tiles = 0, tw = 0, th = 0;     // CLAHE's grid and its tile size
+    double scale = 1.;                 // image_scale_factor
+    double K[9] = {0};                 // the scaled intrinsics
+    short2* map1 = nullptr;
+    uint16_t* map2 = nullptr;
+    uint8_t* planes = nullptr;
+    uint8_t* lut = nullptr;
+    cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};   // call start, image uploaded, remapped, equalised
+    bool timed = false;
+    // the camera updates (srl_vio.cu)
+    double cov[121] = {0};             // imageProcessing::covariance
+    srl::VioOut* d_vio_out = nullptr;  // device
+    cudaEvent_t vio_ev[4] = {nullptr, nullptr, nullptr, nullptr};   // before / after the esikf kernel, the photometric kernel
+    bool vio_ran[2] = {false, false}, vio_timed[2] = {false, false};
+    int vio_iterations[2] = {0, 0}, vio_points[2] = {0, 0};
+    double vio_acc[2] = {0., 0.};
 };
 
 namespace srl {

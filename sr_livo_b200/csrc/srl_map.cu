@@ -242,11 +242,6 @@ __global__ void k_first_in_cell(const unsigned long long* __restrict__ keys_sort
 // addPointToColorMap is sequential in the reference; the same (sort by voxel, replay per voxel in sweep order) scheme as K3
 // reproduces it: a voxel accepts the first (cap - count) offered points, a fine cell is claimed by the first ACCEPTED
 // point of the sweep that falls into it, and both lists are emitted in sweep order.
-struct ColorPoint {            // colour state of one stored point (rgbPoint minus position), index = block * block_pts + i
-    short rgb[3]; short n_rgb;
-    float cov[3]; float pad;
-    double obs_dist, last_obs;
-};
 constexpr unsigned kNoIndex = 0xffffffffu;
 constexpr int kColorMaxCap = 128;   // largest max_num_points_in_voxel of a colour map (the shipped configs use 20, 50 and 100)
 
@@ -362,11 +357,6 @@ __global__ void k_color_emit_rgb(Slot* fine, unsigned int fmask, const unsigned 
 }
 
 struct CamConst { double R[9], t_cw[3], t_wc[3], fx, fy, cx, cy, fov; int cols, rows; };
-__device__ __forceinline__ unsigned char sat_u8(double v) {       // cv::saturate_cast<uchar>(double): cvRound (half to even), clamp
-    const long long r = __double2ll_rn(v);
-    return (unsigned char)(r < 0 ? 0 : (r > 255 ? 255 : r));
-}
-__device__ __forceinline__ unsigned char sat_add_u8(unsigned char a, unsigned char b) { const int r = (int)a + (int)b; return (unsigned char)(r > 255 ? 255 : r); }
 // cloudFrame::project3dPointInThisImage with scale 1 (src/lioOptimization.cpp:142-198) of a stored position widened to double:
 // project3dTo2d (reject pcz < 0.001), then if2dPointsAvailable with the frame's own fov_margin.  Products and sums rounded one
 // by one like the host code.  The renderer and the tracker's selection both project through it.
@@ -393,27 +383,16 @@ __device__ __forceinline__ unsigned render_point(const float* __restrict__ bp, C
     double u, v;
     if (!project_in_image(c, px, py, pz, u, v)) return 0;
     const double dist = camera_distance(c, px, py, pz);
-    // getSubPixel<cv::Vec3b> (:71-98): four saturated products, three saturated sums per channel
-    const int fr = (int)floor(v), fc = (int)floor(u);
-    const double frac_r = __dsub_rn(v, (double)fr), frac_c = __dsub_rn(u, (double)fc);
-    const double w00 = __dmul_rn(__dsub_rn(1.0, frac_r), __dsub_rn(1.0, frac_c)), w10 = __dmul_rn(frac_r, __dsub_rn(1.0, frac_c));
-    const double w01 = __dmul_rn(__dsub_rn(1.0, frac_r), frac_c), w11 = __dmul_rn(frac_r, frac_c);
-    // The +1 taps are clamped to the last row / column (no step down / right there), which changes no value for
+    // getSubPixel<cv::Vec3b> (:71-98).  The +1 taps are clamped to the last row / column, which changes no value for
     // fov_margin >= 0 (negative margins are refused by srl_color_map_render_recent): fr + 1 == rows needs ceil(v) <= rows - 1,
     // because the window's upper bound fl(1 - fov) * rows is at most rows; so v == rows - 1 exactly, frac_r == 0 and
     // w10 == w11 == 0.  The same holds for columns.  The lower bound v >= fl(fov * rows) + 1 >= 1 keeps fr >= 0.  The
     // reference reads row `rows` there with weight 0.
-    const unsigned char* p00 = img + ((size_t)fr * c.cols + fc) * 3;
-    const size_t down = fr + 1 < c.rows ? (size_t)c.cols * 3 : 0, right = fc + 1 < c.cols ? 3 : 0;
+    unsigned char bgr[3];
+    sub_pixel_bgr(img, (size_t)c.cols * 3, c.cols, c.rows, v, u, bgr);
     double color[3];
 #pragma unroll
-    for (int ch = 0; ch < 3; ++ch) {
-        const unsigned char a = sat_u8(__dmul_rn((double)p00[ch], w00));
-        const unsigned char b = sat_u8(__dmul_rn((double)p00[down + ch], w10));
-        const unsigned char cc = sat_u8(__dmul_rn((double)p00[right + ch], w01));
-        const unsigned char d = sat_u8(__dmul_rn((double)p00[down + right + ch], w11));
-        color[ch] = (double)sat_add_u8(sat_add_u8(sat_add_u8(a, b), cc), d);
-    }
+    for (int ch = 0; ch < 3; ++ch) color[ch] = (double)bgr[ch];
     // rgbPoint::updateRgb (src/cloudMap.cpp:59-101), mixed float / double arithmetic as written there
     ColorPoint cp = *cpt;
     const double sigma = 15.0, process_noise_sigma = 0.1;
@@ -824,6 +803,11 @@ struct srl_color_map {
     long long* d_counters = nullptr;        // [0] rgb points, [3] recent voxels listed by the call
     int64_t n_rgb_points = 0, n_recent = 0, n_new_recent = 0;
 };
+
+ColorMapView srl::color_map_view(const srl_color_map* cm) {
+    return ColorMapView{cm->vox->d_blocks, cm->d_cpts, cm->vox->block_pts, (long long)cm->vox->n_voxels};
+}
+srl_ctx* srl::color_map_ctx(const srl_color_map* cm) { return cm->ctx; }
 
 // the colour state of committed_voxels voxels (called by map_grow before the blocks grow)
 static int color_map_grow_voxels(srl_color_map* cm, size_t committed_voxels) {

@@ -892,6 +892,15 @@ def _image_2d(img, what):
     return img.ctypes.data, img.shape[0], img.shape[1], img.strides[0]
 
 
+def _ids_addr(ids):
+    """(address, n) of point ids: a uint32 numpy array or a contiguous 32-bit torch tensor (int32 holds the ids' bits)."""
+    if _is_tensor(ids):
+        if ids.element_size() != 4 or not ids.is_contiguous() or ids.is_floating_point():
+            raise TypeError("expected a contiguous 32-bit integer tensor of point ids")
+        return ids.data_ptr(), ids.numel()
+    return _addr(ids, np.uint32, 1)
+
+
 class ImageProcessing:
     """The image preparation of imageProcessing::process (src/imageProcessing.cpp:91-125,166-200, srl_image_*) on the GPU, bit for
     bit OpenCV's: undistortion (initUndistortRectifyMap CV_16SC2 + remap INTER_LINEAR), COLOR_RGB2GRAY and CLAHE clip 3 for
@@ -975,7 +984,141 @@ class ImageProcessing:
         _check(self.ctx.h, lib().srl_image_last_times(self.h, C.byref(a), C.byref(b), C.byref(c)))
         return a.value, b.value, c.value
 
+    def covariance(self) -> np.ndarray:
+        """imageProcessing::covariance (11, 11): setInitialCov at construction, then what the camera updates leave."""
+        c = np.zeros((11, 11), np.float64)
+        _check(self.ctx.h, lib().srl_image_covariance(self.h, None, ptr(c)))
+        return c
+
+    def setCovariance(self, cov) -> None:
+        c = np.ascontiguousarray(np.asarray(cov, np.float64).reshape(11, 11))
+        _check(self.ctx.h, lib().srl_image_covariance(self.h, ptr(c), None))
+
+    def vioEsikf(self, cmap: "ColorVoxelMap", state: "CameraState", ids, uv, velocity, n_new_visited: int) -> bool:
+        """imageProcessing::vioEsikf (src/imageProcessing.cpp:220-380, srl_image_vio_esikf) over the tracked set in the caller's
+        order: ids (n,) uint32 colour-map point ids, uv (n, 2) float32 matched points (LKOpticalFlowKernel.trackImage's output
+        as it is), velocity (n, 2) float64 image velocities; numpy arrays or torch tensors, host or CUDA.  n_new_visited is the
+        colour map's stats()["recent"] after the rendering insert.  Updates `state` and the covariance in place; returns the reference's
+        result."""
+        p_ids, n = _ids_addr(ids)
+        p_uv, n_uv = _addr(uv, np.float32, 2)
+        p_vel, n_vel = _addr(velocity, np.float64, 2)
+        if n_uv != n or n_vel != n:
+            raise ValueError("ids, uv and velocity must hold the same number of points")
+        r = C.c_int32(0)
+        _check(self.ctx.h, lib().srl_image_vio_esikf(self.h, cmap.h, C.byref(state.c), C.c_void_p(p_ids), C.c_void_p(p_uv),
+                                                     C.c_void_p(p_vel), n, int(n_new_visited), C.byref(r)))
+        return bool(r.value)
+
+    def vioPhotometric(self, cmap: "ColorVoxelMap", state: "CameraState", ids, velocity, n_new_visited: int, rgb_image) -> bool:
+        """imageProcessing::vioPhotometric (:402-552, srl_image_vio_photometric) on the prepared rgb_image ((out_rows, out_cols,
+        3) BGR8, process()'s rgb output; numpy or torch, host or CUDA, rows may be padded); ids and velocity as for vioEsikf."""
+        p_ids, n = _ids_addr(ids)
+        p_vel, n_vel = _addr(velocity, np.float64, 2)
+        if n_vel != n:
+            raise ValueError("ids and velocity must hold the same number of points")
+        p_img, rows, cols, pitch = _image_2d(rgb_image, "rgb_image")
+        r = C.c_int32(0)
+        _check(self.ctx.h, lib().srl_image_vio_photometric(self.h, cmap.h, C.byref(state.c), C.c_void_p(p_ids), C.c_void_p(p_vel), n,
+                                                           int(n_new_visited), C.c_void_p(p_img), int(cols), int(rows), int(pitch),
+                                                           C.byref(r)))
+        return bool(r.value)
+
+    def vio_last_summary(self, which: int) -> tuple[int, int, float]:
+        """(iterations run, points used, acc_residual) of the last vioEsikf (0) or vioPhotometric (1)."""
+        it, used, acc = C.c_int32(0), C.c_int32(0), C.c_double(0)
+        _check(self.ctx.h, lib().srl_image_vio_last_summary(self.h, int(which), C.byref(it), C.byref(used), C.byref(acc)))
+        return it.value, used.value, acc.value
+
+    def vio_last_times(self) -> tuple[float, float]:
+        """(vioEsikf ms, vioPhotometric ms): device time of each update's last launch, CUDA events."""
+        a, b = C.c_double(0), C.c_double(0)
+        _check(self.ctx.h, lib().srl_image_vio_last_times(self.h, C.byref(a), C.byref(b)))
+        return a.value, b.value
+
+
+def _quat_to_rot(q):
+    """Eigen's Quaterniond::toRotationMatrix, q = (x, y, z, w)."""
+    x, y, z, w = (float(v) for v in q)
+    tx, ty, tz = 2.0 * x, 2.0 * y, 2.0 * z
+    twx, twy, twz = tx * w, ty * w, tz * w
+    txx, txy, txz = tx * x, ty * x, tz * x
+    tyy, tyz, tzz = ty * y, tz * y, tz * z
+    return np.array([[1.0 - (tyy + tzz), txy - twz, txz + twy], [txy + twz, 1.0 - (txx + tzz), tyz - twx],
+                     [txz - twy, tyz + twx, 1.0 - (txx + tyy)]])
+
+
+def _rot_to_quat(m):
+    """Eigen's Quaterniond(Matrix3d), as (x, y, z, w)."""
+    q = [0.0] * 4
+    t = m[0, 0] + m[1, 1] + m[2, 2]
+    if t > 0:
+        t = np.sqrt(t + 1.0); q[3] = 0.5 * t; t = 0.5 / t
+        q[0] = (m[2, 1] - m[1, 2]) * t; q[1] = (m[0, 2] - m[2, 0]) * t; q[2] = (m[1, 0] - m[0, 1]) * t
+    else:
+        i = 0
+        if m[1, 1] > m[0, 0]:
+            i = 1
+        if m[2, 2] > m[i, i]:
+            i = 2
+        j, k = (i + 1) % 3, (i + 2) % 3
+        t = np.sqrt(m[i, i] - m[j, j] - m[k, k] + 1.0); q[i] = 0.5 * t; t = 0.5 / t
+        q[3] = (m[k, j] - m[j, k]) * t; q[j] = (m[j, i] + m[i, j]) * t; q[k] = (m[k, i] + m[i, k]) * t
+    return np.array(q)
+
+
+def _mm3(a, b):
+    """3 x 3 product with Eigen's fixed-size reduction order c0 + (c1 + c2)."""
+    return np.array([[a[i, 0] * b[0, j] + (a[i, 1] * b[1, j] + a[i, 2] * b[2, j]) for j in range(3)] for i in range(3)])
+
+
+def _mv3(a, v):
+    return np.array([a[i, 0] * v[0] + (a[i, 1] * v[1] + a[i, 2] * v[2]) for i in range(3)])
+
+
+class CameraState:
+    """The p_state fields the camera updates read and write (srl_vio_state).  The constructor derives the camera poses as
+    lioOptimization::stateEstimation does before process (src/lioOptimization.cpp:1073-1075): q_world_camera =
+    Quaterniond(rotation.toRotationMatrix() * R_imu_camera), t_world_camera = rotation.toRotationMatrix() * t_imu_camera +
+    translation, then refreshPoseForProjection.  Quaternions are (x, y, z, w); R_imu_camera is (3, 3)."""
+
+    def __init__(self, rotation, translation, R_imu_camera, t_imu_camera, fx: float, fy: float, cx: float, cy: float,
+                 time_td: float = 0.0):
+        rq = np.asarray(rotation, np.float64).reshape(4)
+        tr = np.asarray(translation, np.float64).reshape(3)
+        ric = np.asarray(R_imu_camera, np.float64).reshape(3, 3)
+        tic = np.asarray(t_imu_camera, np.float64).reshape(3)
+        rw = _quat_to_rot(rq)
+        q_wc = _rot_to_quat(_mm3(rw, ric))
+        t_wc = _mv3(rw, tic) + tr
+        n2 = (q_wc[0] * q_wc[0] + q_wc[2] * q_wc[2]) + (q_wc[1] * q_wc[1] + q_wc[3] * q_wc[3])
+        q_cw = np.array([-q_wc[0] / n2, -q_wc[1] / n2, -q_wc[2] / n2, q_wc[3] / n2])   # Quaterniond::inverse
+        t_cw = _mv3(-_quat_to_rot(q_cw), t_wc)
+        c = capi.VioState()
+        c.rotation[:] = rq.tolist(); c.translation[:] = tr.tolist(); c.R_imu_camera[:] = ric.reshape(-1).tolist()
+        c.t_imu_camera[:] = tic.tolist()
+        c.fx, c.fy, c.cx, c.cy, c.time_td = float(fx), float(fy), float(cx), float(cy), float(time_td)
+        c.q_world_camera[:] = q_wc.tolist(); c.t_world_camera[:] = t_wc.tolist()
+        c.q_camera_world[:] = q_cw.tolist(); c.t_camera_world[:] = t_cw.tolist()
+        self.c = c
+
+    def __getattr__(self, name):
+        c = self.__dict__.get("c")
+        if c is None or name not in dict(capi.VioState._fields_):
+            raise AttributeError(name)
+        v = getattr(c, name)
+        if isinstance(v, float):
+            return v
+        a = np.array(v[:], np.float64)
+        return a.reshape(3, 3) if name == "R_imu_camera" else a
+
+    def camera(self, cols: int, rows: int, fov_margin: float) -> "capi.Camera":
+        """The srl_camera of this state for the renderer (renderPointsInRecentVoxel) and the selection (selectPointsForProjection)."""
+        c = self.c
+        return capi.Camera((C.c_double * 4)(*c.q_camera_world), (C.c_double * 3)(*c.t_camera_world), (C.c_double * 3)(*c.t_world_camera),
+                           c.fx, c.fy, c.cx, c.cy, float(fov_margin), int(cols), int(rows))
+
 
 __all__ = ["Context", "VoxelHashMap", "ColorVoxelMap", "Sweep", "EskfEstimator", "LioOptimization", "OptimizeSummary", "PlaneResiduals",
            "IcpParams", "r3live_params", "r3live_map_options", "r3live_compressed_map_options", "make_frame", "SrlError", "write_pcd_xyzrgb",
-           "LKOpticalFlowKernel", "tracker_lk_params", "ImageProcessing", "r3live_camera_params", "ntu_camera_params"]
+           "LKOpticalFlowKernel", "tracker_lk_params", "ImageProcessing", "CameraState", "r3live_camera_params", "ntu_camera_params"]
