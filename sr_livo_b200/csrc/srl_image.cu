@@ -1,7 +1,8 @@
 // srl_image.cu — the camera image preparation of imageProcessing::process (src/imageProcessing.cpp:91-125,166-200) on the device,
 // bit for bit OpenCV's:
 //   once per object (the first-image step, :93-104): the undistortion map of initUndistortRectifyMap(K, dist, I, K, size,
-//     CV_16SC2), kept in that format: map1 = (iu >> 5, iv >> 5) int16 pairs, map2 = (iv & 31) * 32 + (iu & 31), iu = cvRound(32 u)
+//     CV_16SC2), kept in that format: map1 = (iu >> 5, iv >> 5) saturated to int16 pairs, map2 = (iv & 31) * 32 + (iu & 31),
+//     iu = cvRound(32 u)
 //   per image (:120-125), three kernels after the upload:
 //     k_img_remap        remap INTER_LINEAR (BORDER_CONSTANT 0, per tap) of the BGR8 image, then from each undistorted pixel the
 //                        COLOR_RGB2GRAY grey (channel 0, B, weighted as R) and the COLOR_BGR2YCrCb planes; the undistorted image
@@ -36,6 +37,9 @@ __device__ __forceinline__ int cv_round(double v) {
     return (r >= -2147483648.0 && r <= 2147483647.0) ? (int)r : INT_MIN;
 }
 
+// saturate_cast<short>(int)
+__device__ __forceinline__ short sat_short(int v) { return (short)min(max(v, -32768), 32767); }
+
 struct MapArgs {
     double ir[9];                      // inv(K), row-major
     double fx, fy, u0, v0, k1, k2, p1, p2, k3;
@@ -61,7 +65,9 @@ __global__ void k_img_map(const __grid_constant__ MapArgs a) {
         const double xd = x * kr + a.p1 * _2xy + a.p2 * (r2 + 2 * x2);
         const double yd = y * kr + a.p1 * (r2 + 2 * y2) + a.p2 * _2xy;
         const int iu = cv_round((a.fx * xd + a.u0) * 32), iv = cv_round((a.fy * yd + a.v0) * 32);
-        m1[j] = make_short2((short)(iu >> 5), (short)(iv >> 5));
+        // saturate_cast<short> as OpenCV's vectorised pack: INT_MIN gives -32768, not the wrapped 0 that would sample a real
+        // pixel, and a coordinate past +-32767 px stays outside the image
+        m1[j] = make_short2(sat_short(iu >> 5), sat_short(iv >> 5));
         m2[j] = (uint16_t)((iv & 31) * 32 + (iu & 31));
     }
 }

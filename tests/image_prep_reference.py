@@ -55,16 +55,16 @@ def clahe_tiles(cols: int) -> int:
     return int(max(cols * 32.0 / 640, 4.0))
 
 
-def undistort_maps(K: np.ndarray, dist, out_cols: int, out_rows: int) -> tuple[np.ndarray, np.ndarray]:
-    """(map1 (rows, cols, 2) int16, map2 (rows, cols) uint16) of initUndistortRectifyMap with R = I and newK = K: per row,
-    _x/_y/_w start at i*ir[1] + ir[2], ... and step by += ir[0], ...; the rational model with k4..k6 = s1..s4 = 0 and no tilt."""
+def undistort_coords(K: np.ndarray, dist, out_cols: int, out_rows: int) -> tuple[np.ndarray, np.ndarray]:
+    """(32 u, 32 v) (rows, cols) float64 of initUndistortRectifyMap with R = I and newK = K, before cvRound: per row, _x/_y/_w
+    start at i*ir[1] + ir[2], ... and step by += ir[0], ...; the rational model with k4..k6 = s1..s4 = 0 and no tilt."""
     ir = inv3(K)
     fx, fy, u0, v0 = K[0, 0], K[1, 1], K[0, 2], K[1, 2]
     k1, k2, p1, p2, k3 = (float(v) for v in dist)
     i = np.arange(out_rows, dtype=np.float64)
     _x, _y, _w = i * ir[1] + ir[2], i * ir[4] + ir[5], i * ir[7] + ir[8]
-    iu = np.empty((out_rows, out_cols), np.int64)
-    iv = np.empty((out_rows, out_cols), np.int64)
+    u32 = np.empty((out_rows, out_cols), np.float64)
+    v32 = np.empty((out_rows, out_cols), np.float64)
     for j in range(out_cols):
         w = 1.0 / _w
         x, y = _x * w, _y * w
@@ -73,12 +73,28 @@ def undistort_maps(K: np.ndarray, dist, out_cols: int, out_rows: int) -> tuple[n
         kr = (1 + ((k3 * r2 + k2) * r2 + k1) * r2) / (1 + ((0.0 * r2 + 0.0) * r2 + 0.0) * r2)
         xd = x * kr + p1 * _2xy + p2 * (r2 + 2 * x2) + 0.0 * r2 + 0.0 * r2 * r2
         yd = y * kr + p1 * (r2 + 2 * y2) + p2 * _2xy + 0.0 * r2 + 0.0 * r2 * r2
-        iu[:, j] = _cv_round((fx * 1.0 * xd + u0) * 32)
-        iv[:, j] = _cv_round((fy * 1.0 * yd + v0) * 32)
+        u32[:, j] = (fx * 1.0 * xd + u0) * 32
+        v32[:, j] = (fy * 1.0 * yd + v0) * 32
         _x, _y, _w = _x + ir[0], _y + ir[3], _w + ir[6]
-    map1 = np.stack([(iu >> 5).astype(np.int16), (iv >> 5).astype(np.int16)], axis=-1)
+    return u32, v32
+
+
+def undistort_maps(K: np.ndarray, dist, out_cols: int, out_rows: int) -> tuple[np.ndarray, np.ndarray]:
+    """(map1 (rows, cols, 2) int16, map2 (rows, cols) uint16) of initUndistortRectifyMap(..., CV_16SC2) with R = I and newK = K:
+    iu = cvRound(32 u), map1 = (iu >> 5, iv >> 5) saturated to int16, map2 = (iv & 31) * 32 + (iu & 31)."""
+    u32, v32 = undistort_coords(K, dist, out_cols, out_rows)
+    iu, iv = _cv_round(u32), _cv_round(v32)
+    # saturate_cast<short>, as OpenCV's vectorised rows pack map1: an iu of INT_MIN (NaN or out of the int range) gives -32768,
+    # and a coordinate past +-32767 px stays outside the image instead of wrapping back into it
+    map1 = np.stack([np.clip(iu >> 5, -32768, 32767).astype(np.int16), np.clip(iv >> 5, -32768, 32767).astype(np.int16)], axis=-1)
     map2 = ((iv & 31) * 32 + (iu & 31)).astype(np.uint16)
     return map1, map2
+
+
+def saturated(map1: np.ndarray) -> np.ndarray:
+    """(rows, cols) bool: the map entries whose source coordinate saturated map1 in either component.  Every tap of such an
+    entry lies outside the image; a vectorised OpenCV may give their map2 a different last bit."""
+    return ((map1 == -32768) | (map1 == 32767)).any(axis=-1)
 
 
 def remap_bilinear(src: np.ndarray, map1: np.ndarray, map2: np.ndarray) -> np.ndarray:
@@ -130,9 +146,10 @@ def _reflect101(p: np.ndarray, n: int) -> np.ndarray:
         p = np.where(p < 0, -p, np.where(p >= n, 2 * n - p - 2, p))
 
 
-def clahe_luts(img: np.ndarray, clip: float, t: int) -> tuple[np.ndarray, int, int]:
-    """(lut (t, t, 256) uint8, tile width, tile height) of CLAHE's histogram pass.  A size that is not a multiple of the grid in
-    either dimension pads both, by t - size % t (a full t where it divides), with REFLECT_101, bottom and right."""
+def clahe_sums(img: np.ndarray, clip: float, t: int) -> tuple[np.ndarray, int, int]:
+    """(prefix sums (t * t, 256) int64 of the clipped and redistributed histograms, tile width, tile height) of CLAHE's
+    histogram pass.  A size that is not a multiple of the grid in either dimension pads both, by t - size % t (a full t where
+    it divides), with REFLECT_101, bottom and right."""
     h, w = img.shape
     if w % t == 0 and h % t == 0:
         ext = img
@@ -151,7 +168,13 @@ def clahe_luts(img: np.ndarray, clip: float, t: int) -> tuple[np.ndarray, int, i
     step = np.maximum(256 // np.maximum(residual, 1), 1)
     i = np.arange(256)[None, :]
     hist += ((residual[:, None] > 0) & (i % step[:, None] == 0) & (i // step[:, None] < residual[:, None])).astype(np.int64)
-    lut = np.rint(np.cumsum(hist, axis=1).astype(F32) * (F32(255) / F32(area)))
+    return np.cumsum(hist, axis=1), tw, th
+
+
+def clahe_luts(img: np.ndarray, clip: float, t: int) -> tuple[np.ndarray, int, int]:
+    """(lut (t, t, 256) uint8, tile width, tile height): cvRound((float)sum * (255.f / area)) of clahe_sums, clamped."""
+    sums, tw, th = clahe_sums(img, clip, t)
+    lut = np.rint(sums.astype(F32) * (F32(255) / F32(tw * th)))
     return np.clip(lut, 0, 255).astype(np.uint8).reshape(t, t, 256), tw, th
 
 
