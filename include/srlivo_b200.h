@@ -582,7 +582,8 @@ typedef struct srl_vio_state {   /* the p_state fields the two updates read and 
  * is map_tracker->number_of_new_visited_voxel: cam_measurement_weight = max(0.001, min(5.0 / n_new_visited, 0.01)).  *result
  * is the reference's return value; state and covariance are updated in place when it is 1.  n < 10: *result = 0 and nothing
  * changes.  ids, uv and velocity are host or device memory.  SRL_BAD_ARG (nothing written) for an id that names no stored
- * point; SRL_SINGULAR (nothing written) for a zero or NaN pivot of the update's 11 x 11 system. */
+ * point; SRL_SINGULAR (nothing written) for a zero or NaN pivot of the update's 11 x 11 system, which includes any NaN or
+ * +-inf component of uv or velocity (the reference writes a NaN state and covariance and returns 1 there). */
 int srl_image_vio_esikf(srl_image* img, srl_color_map* cm, srl_vio_state* state, const uint32_t* ids, const float* uv,
                         const double* velocity, size_t n, int32_t n_new_visited, int32_t* result);
 /* vioPhotometric on the prepared rgb_image `bgr` (BGR8, cols x rows, rows `pitch` bytes apart, host or device): each point with

@@ -27,12 +27,15 @@ def textured_image(rows, cols, seed):
     return np.ascontiguousarray(img)
 
 
-def make_state(rng, cam, scale=1.0, td=0.0, ric_angle=0.02):
+def make_state(rng, cam, scale=1.0, td=0.0, ric_angle=0.02, rotation=None, ric=None):
+    """rotation (x, y, z, w) and ric (3 x 3), when given, replace the seeded ones (the seeded draws are made either way)"""
     K = np.array(cam["camera_intrinsic"], np.float64).reshape(3, 3)
     fx, fy, cx, cy = K[0, 0] / scale, K[1, 1] / scale, K[0, 2] / scale, K[1, 2] / scale
     rot = _quat(rng, 0.7)
-    ric = lio._quat_to_rot(_quat(rng, ric_angle)) @ np.array([[0.0, 0.0, 1.0], [-1.0, 0.0, 0.0], [0.0, -1.0, 0.0]])
-    s = lio.CameraState(rot, rng.normal(size=3), ric, rng.normal(scale=0.05, size=3), fx, fy, cx, cy, td)
+    r_ic = lio._quat_to_rot(_quat(rng, ric_angle)) @ np.array([[0.0, 0.0, 1.0], [-1.0, 0.0, 0.0], [0.0, -1.0, 0.0]])
+    rot = rot if rotation is None else np.asarray(rotation, np.float64)
+    r_ic = r_ic if ric is None else np.asarray(ric, np.float64)
+    s = lio.CameraState(rot, rng.normal(size=3), r_ic, rng.normal(scale=0.05, size=3), fx, fy, cx, cy, td)
     return s
 
 
@@ -43,11 +46,11 @@ def state_array(s):
 
 
 def make_case(seed, camera="r3live", n=300, scale=1.0, td=0.002, outlier_px=3.0, colour_noise=6.0, n_low=0, n_new_visited=40,
-              pix_noise=0.6, margin=6.0, zmin=3.0, zmax=25.0, colour_at_projection=False):
+              pix_noise=0.6, margin=6.0, zmin=3.0, zmax=25.0, colour_at_projection=False, rotation=None, ric=None):
     rng = np.random.default_rng(seed)
     cam = CAMERAS[camera]
     cols, rows = int(cam["image_width"] / scale), int(cam["image_height"] / scale)
-    s = make_state(rng, cam, scale, td)
+    s = make_state(rng, cam, scale, td, rotation=rotation, ric=ric)
     st = state_array(s)
     Rcw = lio._quat_to_rot(st[31:35])
     tcw = st[35:38]
@@ -131,7 +134,9 @@ MARGIN = 1e-6
 
 def fragile(truth, esikf, n):
     """The decisions of one restated update that lie within MARGIN of their thresholds: the Huber test (residual norm vs 1),
-    so3ToQuat's small-angle branch (rotation step vs THETA_THRESHOLD), and the photometric break (acc_residual / n vs 10)."""
+    so3ToQuat's small-angle branch (rotation step vs THETA_THRESHOLD), rotationToSo3's (d_x's rotation vs THETA_THRESHOLD),
+    the photometric break (acc_residual / n vs 10), and the branches of Quaterniond(Matrix3d) (the trace vs 0, then the
+    diagonal comparisons), two of which give q and -q for the same rotation."""
     out = []
     # photometric residuals are differences of integers (a sampled BGR value and the short state): the squared norm is an
     # integer every form computes exactly, so that Huber test cannot round differently
@@ -142,21 +147,30 @@ def fragile(truth, esikf, n):
     for it, st in enumerate(truth.get("steps", [])):
         if abs(st - 1e-4) < MARGIN * 1e-4:
             out.append(("theta", it, st))
+    for it, st in enumerate(truth.get("dx_rot", [])):
+        if abs(st - 1e-4) < MARGIN * 1e-4:
+            out.append(("dtheta", it, st))
     if not esikf and truth["acc_history"]:
         r = float(truth["acc_history"][0]) / n
         if abs(r - 10.0) < MARGIN * 10.0:
             out.append(("break", 0, r))
+    for k, (role, t, m00, m11, m22) in enumerate(truth.get("rot2q", [])):
+        if abs(t) < MARGIN:
+            out.append(("rot2q trace", k, role, t))
+        elif t <= 0 and (abs(m22 - max(m00, m11)) < MARGIN or (m22 < max(m00, m11) and abs(m11 - m00) < MARGIN)):
+            out.append(("rot2q diagonal", k, role, (m00, m11, m22)))   # the comparison that picks the largest entry
     return out
 
 
 # ---- device scenes -----------------------------------------------------------------------------------------------------
-def device_scene(lio, ctx, camera="ntu", seed=501, n_usable=400, n_fresh=0, photometric_seed=950):
+def device_scene(lio, ctx, camera="ntu", seed=501, n_usable=400, n_fresh=0, photometric_seed=950, rotation=None, ric=None):
     """A colour map filled and coloured on the device as process fills it: n_usable points (depths 3-12 m) added and rendered
     three times (N_rgb = 3), then n_fresh points (depths 14-25 m, so in other voxels) added and rendered once (N_rgb = 1).
     Returns the handles, the state, and per selected point its id, gathered colour state, matched uv and velocity; img is the
-    image the photometric update samples (half the rendered scene, half an unrelated texture)."""
+    image the photometric update samples (half the rendered scene, half an unrelated texture).  rotation (the IMU's, x, y, z,
+    w) and ric (R_imu_camera), when given, replace the seeded ones."""
     cam = CAMERAS[camera]
-    c = make_case(seed, camera, n=n_usable, zmin=3.0, zmax=12.0)
+    c = make_case(seed, camera, n=n_usable, zmin=3.0, zmax=12.0, rotation=rotation, ric=ric)
     ip = lio.ImageProcessing(ctx, **cam)
     cols, rows = ip.output_size()
     cm = lio.ColorVoxelMap(ctx, 1.0, 20, 1 << 15, 0.05)

@@ -72,10 +72,16 @@ def q_to_R(q):
                       [2 * (x * z - y * w), 2 * (y * z + x * w), 1 - 2 * (x * x + y * y)]])
 
 
-def R_to_q(m):
+# R_to_q's branch inputs: while a list is set here, each call appends (role, trace, m00, m11, m22), the values as float64
+_BRANCH_LOG = None
+
+
+def R_to_q(m, role=None):
     """Eigen's Quaterniond(Matrix3d) (the branch by the trace, then by the largest diagonal entry)."""
     q = [mpf(0)] * 4
     t = m[0, 0] + m[1, 1] + m[2, 2]
+    if _BRANCH_LOG is not None:
+        _BRANCH_LOG.append((role, float(t), float(m[0, 0]), float(m[1, 1]), float(m[2, 2])))
     if t > 0:
         t = mp.sqrt(t + 1); q[3] = t / 2; t = mpf(1) / (2 * t)
         q[0] = (m[2, 1] - m[1, 2]) * t; q[1] = (m[0, 2] - m[2, 0]) * t; q[2] = (m[1, 0] - m[0, 1]) * t
@@ -117,8 +123,17 @@ def so3_to_quat(w):
     return qunit([u[0] * s, u[1] * s, u[2] * s, c])
 
 
+def rot2q_branch(t, m00, m11, m22):
+    """the branch R_to_q takes on these inputs: "trace", or "i=0" / "i=1" / "i=2" (the largest diagonal entry)"""
+    if t > 0:
+        return "trace"
+    d = [m00, m11, m22]
+    i = 1 if d[1] > d[0] else 0
+    return f"i={2 if d[2] > d[i] else i}"
+
+
 def rotation_to_so3(R):
-    R = q_to_R(qunit(R_to_q(R)))                 # normalizeR
+    R = q_to_R(qunit(R_to_q(R, "dq")))           # normalizeR
     th = mp.acos((R[0, 0] + R[1, 1] + R[2, 2] - 1) / 2)
     a = [R[2, 1] - R[1, 2], R[0, 2] - R[2, 0], R[1, 0] - R[0, 1]]
     if th < THETA:
@@ -149,13 +164,13 @@ class State:
         o = 1 if esikf else 0
         if esikf:
             self.td += d[0]
-        q = qunit(qmul(R_to_q(self.Ric), so3_to_quat([d[o], d[o + 1], d[o + 2]])))
+        q = qunit(qmul(R_to_q(self.Ric, "Ric"), so3_to_quat([d[o], d[o + 1], d[o + 2]])))
         self.Ric = q_to_R(q)
         self.tic = self.tic + mp.matrix([d[o + 3], d[o + 4], d[o + 5]])
         if esikf:
             self.fx += d[7]; self.fy += d[8]; self.cx += d[9]; self.cy += d[10]
         Rw = q_to_R(self.rotation)
-        self.q_wc = R_to_q(Rw * self.Ric)
+        self.q_wc = R_to_q(Rw * self.Ric, "Rwc")
         self.t_wc = Rw * self.tic + self.translation
         self.q_cw = qinv(self.q_wc)
         self.t_cw = -(q_to_R(self.q_cw) * self.t_wc)
@@ -179,16 +194,28 @@ def _solve(S, g, P, Jz, dx, w, D):
     KH = Ainv * S
     Kr = Ainv * g
     sol = -Kr - (mp.eye(D) - KH) * (Jz * dx)
-    return KH, sol
+    return KH, sol, M
 
 
-def vio_update(esikf, state, cov, xyz, uv, vel, rgb, cov_rgb, n_rgb, n_new_visited, img=None):
+def _f64(A):
+    return np.array([[float(A[r, c]) for c in range(A.cols)] for r in range(A.rows)])
+
+
+def vio_update(esikf, state, cov, xyz, uv, vel, rgb, cov_rgb, n_rgb, n_new_visited, img=None, mult=None):
     """One update on the exact inputs.  Returns dict(state (38 float64), cov (11 x 11 float64), result, iterations, used, acc,
     huber (per point, per iteration: True where the Huber branch scaled), residual_norms (per point, per iteration: what the Huber
     test compares with 1), projections (per iteration, float64 (n, 2)), acc_history (acc_residual per iteration, as the
     convergence tests read it), steps (the norm of each iteration's rotation step, which so3ToQuat compares with
-    THETA_THRESHOLD))."""
-    n = len(xyz)
+    THETA_THRESHOLD), dx_rot (per iteration, the norm of d_x's rotation, whose rotationToSo3 compares its angle with
+    THETA_THRESHOLD), systems (per iteration that solved: S, g and M = I + Pw S rounded to float64), rot2q (per R_to_q call in
+    order: (role, trace, m00, m11, m22), role "Ric" for R_imu_camera, "Rwc" for R_world R_imu_camera, "dq" for the step
+    rotation normalizeR converts)).
+
+    mult (optional, one positive int per point): point i stands for mult[i] copies of itself in the list, its rows, acc_residual
+    and used count added mult[i] times and n = sum(mult).  Exact here, so a list of repeated tiles costs what one tile costs."""
+    global _BRANCH_LOG
+    mult = None if mult is None else [int(m) for m in mult]
+    n = len(xyz) if mult is None else sum(mult)
     D = 11 if esikf else 6
     cov_in = np.array(cov, np.float64).reshape(11, 11)
     out = dict(state=np.array(state, np.float64).reshape(38).copy(), cov=cov_in.copy(), result=0, iterations=0, used=0, acc=0.0,
@@ -196,6 +223,15 @@ def vio_update(esikf, state, cov, xyz, uv, vel, rgb, cov_rgb, n_rgb, n_new_visit
     if n < MIN_POINTS:
         return out
     out["result"] = 1
+    _BRANCH_LOG = out["rot2q"] = []
+    try:
+        _iterate(out, esikf, state, cov_in, xyz, uv, vel, rgb, cov_rgb, n_rgb, n_new_visited, img, mult, n, D)
+    finally:
+        _BRANCH_LOG = None
+    return out
+
+
+def _iterate(out, esikf, state, cov_in, xyz, uv, vel, rgb, cov_rgb, n_rgb, n_new_visited, img, mult, n, D):
     st = State(state)
     o = 0 if esikf else 1
     P = mp.matrix([[mpf(float(cov_in[r + o, c + o])) for c in range(D)] for r in range(D)])
@@ -204,19 +240,22 @@ def vio_update(esikf, state, cov, xyz, uv, vel, rgb, cov_rgb, n_rgb, n_new_visit
     last = mpf("3e8")
     KH = sol = None
     for it in range(2):
-        d_so3 = rotation_to_so3(q_to_R(qmul(qinv(R_to_q(pred.Ric)), R_to_q(st.Ric))))
+        d_so3 = rotation_to_so3(q_to_R(qmul(qinv(R_to_q(pred.Ric, "Ric")), R_to_q(st.Ric, "Ric"))))
         d_p = st.tic - pred.tic
         if esikf:
             dx = mp.matrix([st.td - pred.td] + d_so3 + list(d_p) + [st.fx - pred.fx, st.fy - pred.fy, st.cx - pred.cx, st.cy - pred.cy])
         else:
             dx = mp.matrix(d_so3 + list(d_p))
+        out.setdefault("dx_rot", []).append(float(mp.sqrt(sum(c * c for c in d_so3))))
         Rcw = q_to_R(st.q_cw)
         S = mp.zeros(D, D); g = mp.zeros(D, 1)
         acc = mpf(0); used = 0
-        hub = np.zeros(n, bool); proj = np.full((n, 2), np.nan); rn = np.full(n, np.nan)
-        for i in range(n):
+        npt = len(xyz)
+        hub = np.zeros(npt, bool); proj = np.full((npt, 2), np.nan); rn = np.full(npt, np.nan)
+        for i in range(npt):
             if not esikf and n_rgb[i] < 3:
                 continue
+            m = 1 if mult is None else mult[i]
             pw = mp.matrix([mpf(float(np.float32(x))) for x in xyz[i]])
             pc = Rcw * pw + st.t_cw
             x, y, z = pc[0], pc[1], pc[2]
@@ -225,13 +264,13 @@ def vio_update(esikf, state, cov, xyz, uv, vel, rgb, cov_rgb, n_rgb, n_new_visit
             pv = st.fy * y / z + st.cy + st.td * v1
             proj[i] = (float(pu), float(pv))
             J = mp.matrix([[st.fx / z, 0, -(st.fx * x) / (z * z)], [0, st.fy / z, -(st.fy * y) / (z * z)]])
-            used += 1
+            used += m
             if esikf:
                 e = mp.matrix([pu - mpf(float(np.float32(uv[i][0]))), pv - mpf(float(np.float32(uv[i][1])))])
                 res = mp.sqrt(e[0] ** 2 + e[1] ** 2)
                 h = huber(res)
                 hub[i] = res >= 1; rn[i] = float(res)
-                acc += res
+                acc += res * m
                 H = mp.zeros(2, 11)
                 JS = J * skew(pc); JR = -J * st.Ric.T
                 for k in range(2):
@@ -241,7 +280,7 @@ def vio_update(esikf, state, cov, xyz, uv, vel, rgb, cov_rgb, n_rgb, n_new_visit
                         H[k, 4 + j] = JR[k, j] * h
                 H[0, 7] = x / z * h; H[0, 9] = h; H[1, 8] = y / z * h; H[1, 10] = h
                 r = e * h
-                S += H.T * H; g += H.T * r
+                S += H.T * H * m; g += H.T * r * m
             else:
                 col, cdx, cdy = get_rgb(img, float(pu), float(pv))
                 e = mp.matrix([mpf(float(col[c])) - int(rgb[i][c]) for c in range(3)])
@@ -250,7 +289,7 @@ def vio_update(esikf, state, cov, xyz, uv, vel, rgb, cov_rgb, n_rgb, n_new_visit
                 h = huber(nrm)
                 hub[i] = nrm >= 1; rn[i] = float(nrm)
                 r = e * h
-                acc += sum(r[c] * info[c] * r[c] for c in range(3))
+                acc += sum(r[c] * info[c] * r[c] for c in range(3)) * m
                 Jcu = mp.matrix([[mpf(float(cdx[c])), mpf(float(cdy[c]))] for c in range(3)])
                 Jc = Jcu * J
                 A1 = Jc * skew(pc) * h; A2 = -Jc * st.Ric.T * h
@@ -259,7 +298,7 @@ def vio_update(esikf, state, cov, xyz, uv, vel, rgb, cov_rgb, n_rgb, n_new_visit
                     for j in range(3):
                         H[k, j] = A1[k, j]; H[k, 3 + j] = A2[k, j]
                 Rinv = mp.diag(info)
-                S += H.T * Rinv * H; g += H.T * Rinv * r
+                S += H.T * Rinv * H * m; g += H.T * Rinv * r * m
         if esikf:
             acc = acc / n
         out["huber"].append(hub); out["projections"].append(proj); out["acc_history"].append(acc)
@@ -273,7 +312,8 @@ def vio_update(esikf, state, cov, xyz, uv, vel, rgb, cov_rgb, n_rgb, n_new_visit
         for a in range(3):
             for b in range(3):
                 Jz[so + a, so + b] = Js[a, b]
-        KH, sol = _solve(S, g, P, Jz, dx, w, D)
+        KH, sol, M = _solve(S, g, P, Jz, dx, w, D)
+        out.setdefault("systems", []).append(dict(S=_f64(S), g=_f64(g).reshape(D), M=_f64(M)))
         st.update([sol[k] for k in range(D)], esikf)
         out.setdefault("steps", []).append(float(mp.sqrt(sum(sol[so + k] ** 2 for k in range(3)))))
         out["iterations"] += 1
@@ -297,4 +337,3 @@ def vio_update(esikf, state, cov, xyz, uv, vel, rgb, cov_rgb, n_rgb, n_new_visit
                 cv[r + o, c + o] = float(Pn[r, c])
         out["cov"] = cv
     out["state"] = st.array()
-    return out
