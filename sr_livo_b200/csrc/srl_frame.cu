@@ -387,9 +387,20 @@ static int frame_reserve(srl_cloud_frame* f, size_t cap) {
     SRL_CUDA(ctx, cudaSetDevice(ctx->device));
     SRL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     SRL_CUDA(ctx, cudaMalloc(&g.mem, probe.used));
-    if (f->mem) cudaFree(f->mem);
     Carve c{static_cast<char*>(g.mem), 0};
     frame_layout(g, c, cap);
+    if (f->mem && f->n) {   // the frame moves with its block: a build refused after growing still leaves it as it was
+        const size_t n = f->n;
+        const cudaMemcpyKind dd = cudaMemcpyDeviceToDevice;
+        cudaStream_t st = ctx->stream;
+        SRL_CUDA(ctx, cudaMemcpyAsync(g.raw, f->raw, n * 24, dd, st)); SRL_CUDA(ctx, cudaMemcpyAsync(g.point, f->point, n * 24, dd, st));
+        SRL_CUDA(ctx, cudaMemcpyAsync(g.imu, f->imu, n * 24, dd, st)); SRL_CUDA(ctx, cudaMemcpyAsync(g.rel, f->rel, n * 8, dd, st));
+        SRL_CUDA(ctx, cudaMemcpyAsync(g.alpha, f->alpha, n * 8, dd, st)); SRL_CUDA(ctx, cudaMemcpyAsync(g.ts, f->ts, n * 8, dd, st));
+        SRL_CUDA(ctx, cudaMemcpyAsync(g.src, f->src, n * 4, dd, st));
+        SRL_CUDA(ctx, cudaStreamSynchronize(st));
+        g.n = n;
+    }
+    if (f->mem) cudaFree(f->mem);
     *f = g;
     return SRL_OK;
 }

@@ -121,6 +121,64 @@ def shuffle(n: int, words, pos: int = 0, rule: int = 0):
     return fisher_yates(j), pos
 
 
+def _mul128(w, r):
+    """(high, low) 64-bit halves of w * r, uint64 arrays, from 32-bit limbs."""
+    m32, s = np.uint64(0xFFFFFFFF), np.uint64(32)
+    a1, a0, b1, b0 = w >> s, w & m32, r >> s, r & m32
+    p00, p01, p10, p11 = a0 * b0, a0 * b1, a1 * b0, a1 * b1
+    mid = (p00 >> s) + (p01 & m32) + (p10 & m32)
+    return p11 + (p01 >> s) + (p10 >> s) + (mid >> s), (p00 & m32) | (mid << s)
+
+
+def _draw_try(w, r, rule: int):
+    """draw()'s one attempt on uint64 arrays: (accepted, value)."""
+    if rule == 0:
+        hi, lo = _mul128(w, r)
+        return ~((lo < r) & (lo < (np.uint64(0) - r) % r)), hi
+    scaling = np.uint64(MASK) // r
+    return w < r * scaling, w // scaling
+
+
+def shuffle_targets_fast(n: int, words, pos: int = 0, rule: int = 0):
+    """shuffle_targets on arrays: every draw at once on the words it would take without a rejection, then from each
+    rejected draw on again one word later.  (j, next word position, indices of the rejected draws; a draw rejected twice
+    is listed twice)."""
+    D = num_draws(n)
+    j = np.zeros(max(n, 1), np.int64)
+    if D == 0:
+        return j[:n], pos, []
+    d = np.arange(D, dtype=np.int64)
+    i = 2 * d + (1 if n % 2 else 0)
+    r = ((i + 1) * (i + 2)).astype(np.uint64)
+    if n % 2 == 0:
+        i[0], r[0] = 1, 2
+    x = np.zeros(D, np.uint64)
+    words = np.asarray(words, np.uint64)
+    rejected, start = [], 0
+    while start < D:
+        w0 = pos + start + len(rejected)
+        ok, val = _draw_try(words[w0:w0 + D - start], r[start:], rule)
+        bad = np.flatnonzero(~ok)
+        stop = D if bad.size == 0 else start + int(bad[0])
+        x[start:stop] = val[:stop - start]
+        if stop < D:
+            rejected.append(stop)
+        start = stop
+    b = (i + 2).astype(np.uint64)
+    pair = r != 2
+    j[i[pair]] = (x[pair] // b[pair]).astype(np.int64)
+    j[i[pair] + 1] = (x[pair] % b[pair]).astype(np.int64)
+    if not pair[0]:
+        j[1] = int(x[0])
+    return j, pos + D + len(rejected), rejected
+
+
+def shuffle_fast(n: int, words, pos: int = 0, rule: int = 0):
+    """shuffle() for frames of millions of points: (perm, next word position, rejected draws)."""
+    j, pos, rejected = shuffle_targets_fast(n, words, pos, rule)
+    return resolve(j), pos, rejected
+
+
 # ---- the oracle's buildFrame -------------------------------------------------------------------------------------------
 def make_point_timestamp(ts, begin, end, point_time_enable):
     """makePointTimestamp (:786-819): (kept indices, relative_time ms, alpha_time)."""
@@ -128,7 +186,8 @@ def make_point_timestamp(ts, begin, end, point_time_enable):
     keep = np.arange(ts.shape[0]) if point_time_enable else np.flatnonzero(~(ts > end) & ~(ts < begin))
     delta_t = end - begin
     rel = ts[keep] - begin
-    alpha = rel / delta_t
+    with np.errstate(divide="ignore", invalid="ignore"):   # delta_t 0: +-inf or NaN, as the reference divides
+        alpha = rel / delta_t
     rel = rel * 1000.0
     if point_time_enable:
         alpha = np.where(alpha > 1.0, 1.0 - 1e-5, alpha)
@@ -157,12 +216,13 @@ def build_frame(c: dict, rule: int = 0) -> dict:
     else:
         imu = O.distort_frame_by_imu(raw1, rel, c["states"], begin, R_il, t_il, imu_xyz_in=np.zeros((n1, 3)))[0] if n1 else np.zeros((0, 3))
     words = mt19937_64(2 * num_draws(n1) + 4096)
-    order, pos = shuffle(n1, words, 0, rule)
+    order, pos, rej1 = shuffle_fast(n1, words, 0, rule)
+    rej2 = []
     if c["voxel_size"] > 0:
         size = c["init_voxel_size"] if c["index_frame"] < c["init_num_frames"] else c["voxel_size"]
         sel = O.grid_sampling(raw1[order], size) if n1 else np.zeros(0, np.int64)
         order = order[sel]
-        perm, pos = shuffle(order.shape[0], words, pos, rule)
+        perm, pos, rej2 = shuffle_fast(order.shape[0], words, pos, rule)
         order = order[perm]
     imu_f = imu[order]
     raw_f = O.transform_all_imu_point(imu_f, c["states"][-1], R_il, t_il) if order.size else np.zeros((0, 3))
@@ -173,7 +233,8 @@ def build_frame(c: dict, rule: int = 0) -> dict:
         point = transform_point(raw_f, c["q_pred"], c["t_pred"], R_il, t_il)
         alpha_f = alpha[order]
     return dict(raw_point=raw_f, point=point, imu_point=imu_f, relative_time=rel[order], alpha_time=alpha_f, timestamp=ts1[order],
-                source_index=keep[order].astype(np.int32), engine_words=pos)
+                source_index=keep[order].astype(np.int32), engine_words=pos, n_timestamped=n1,
+                rejected=(rej1, rej2))
 
 
 # ---- cases --------------------------------------------------------------------------------------------------------------
