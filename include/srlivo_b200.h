@@ -226,6 +226,10 @@ int srl_sweep_upload(srl_sweep* sweep, const double* raw_xyz, size_t n);
 int srl_sweep_set_device(srl_sweep* sweep, const double* d_raw_xyz, size_t n);  /* device -> device copy */
 /* keypoints [begin, end) are this rank's shard (point-index sharding, SURVEY.md §8(e)); default whole sweep */
 int srl_sweep_set_shard(srl_sweep* sweep, size_t begin, size_t end);
+/* the sweep's Morton order as the passes read it (order[s] = the keypoint at sorted position s), copied to host memory
+ * after a synchronise of the ctx stream; an order already computed is copied as it is.  *n_out = the sweep's keypoints;
+ * order == NULL only counts; SRL_BAD_ARG when max_n < n. */
+int srl_sweep_download_order(srl_sweep* sweep, uint32_t* order, size_t max_n, int64_t* n_out);
 
 /* ---- one ESIKF pass: buildPlaneResiduals + H_x/h + HTH/HTh (src/optimize.cpp:18-131,160-170,235,239) */
 int srl_build_plane_residuals(srl_ctx* ctx, srl_map* map, srl_sweep* sweep, const srl_frame* frame,

@@ -129,7 +129,7 @@ EXPORTS = [
     "srl_last_error", "srl_ctx_synchronize", "srl_ctx_kernel_launches", "srl_ctx_set_timing", "srl_ctx_pass_time", "srl_ctx_set_option", "srl_ctx_get_counter", "srl_map_create", "srl_map_destroy",
     "srl_map_clear", "srl_map_stats", "srl_map_remove_far", "srl_map_upload", "srl_map_download", "srl_map_insert",
     "srl_map_insert_device", "srl_map_insert_sweep", "srl_sweep_create", "srl_sweep_destroy", "srl_sweep_upload", "srl_sweep_set_device",
-    "srl_sweep_set_shard", "srl_build_plane_residuals", "srl_build_plane_residuals_async", "srl_normal_eq_unpack",
+    "srl_sweep_set_shard", "srl_sweep_download_order", "srl_build_plane_residuals", "srl_build_plane_residuals_async", "srl_normal_eq_unpack",
     "srl_iekf_begin", "srl_iekf_step", "srl_update_iekf", "srl_comm_create", "srl_comm_destroy", "srl_comm_export", "srl_comm_connect",
     "srl_update_iekf_dist", "srl_optimize_host", "srl_optimize_host_dist", "srl_shard_range", "srl_sweep_transform_device",
     "srl_grid_sampling", "srl_eskf_observe", "srl_host_plane_fit", "srl_iekf_replay",
@@ -193,6 +193,7 @@ def lib():
     L.srl_sweep_upload.argtypes = [vp, vp, sz]
     L.srl_sweep_set_device.argtypes = [vp, vp, sz]
     L.srl_sweep_set_shard.argtypes = [vp, sz, sz]
+    L.srl_sweep_download_order.argtypes = [vp, vp, sz, C.POINTER(i64)]
     L.srl_build_plane_residuals.argtypes = [vp, vp, vp, C.POINTER(Frame), C.POINTER(IcpParams), C.POINTER(NormalEq),
                                             C.POINTER(DebugOut)]
     L.srl_build_plane_residuals_async.argtypes = [vp, vp, vp, C.POINTER(Frame), C.POINTER(IcpParams), vp]

@@ -532,6 +532,18 @@ int srl_sweep_set_shard(srl_sweep* s, size_t begin, size_t end) {
     s->shard_begin = begin; s->shard_end = end; s->flags_clean = false;
     return SRL_OK;
 }
+int srl_sweep_download_order(srl_sweep* s, uint32_t* order, size_t max_n, int64_t* n_out) {
+    if (!s) return SRL_BAD_ARG;
+    srl_ctx* ctx = s->ctx;
+    if (n_out) *n_out = (int64_t)s->n;
+    if (!order || s->n == 0) return SRL_OK;
+    if (max_n < s->n) return set_err(ctx, SRL_BAD_ARG, "srl_sweep_download_order: output too small");
+    SRL_CUDA(ctx, cudaSetDevice(ctx->device));
+    int rc;
+    if ((rc = ensure_order(ctx, s)) != SRL_OK) return rc;
+    SRL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return copy_to_host(ctx, order, s->d_order, s->n * sizeof(unsigned));
+}
 
 // ---- one pass ----------------------------------------------------------------------------------------------
 // The srl_last_error text of a failed pass or of a failed device-resident loop, the same on every entry point.

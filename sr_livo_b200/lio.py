@@ -443,6 +443,14 @@ class Sweep:
     def set_shard(self, begin: int, end: int):
         _check(self.ctx.h, lib().srl_sweep_set_shard(self.h, begin, end))
 
+    def order(self) -> np.ndarray:
+        """The Morton order the passes visit the keypoints in: (n,) uint32, entry s = the keypoint at sorted position s."""
+        n = C.c_int64(0)
+        _check(self.ctx.h, lib().srl_sweep_download_order(self.h, None, 0, C.byref(n)))
+        out = np.empty(n.value, np.uint32)
+        _check(self.ctx.h, lib().srl_sweep_download_order(self.h, ptr(out), out.size, C.byref(n)))
+        return out
+
 
 class CloudFrame:
     """The frame buildFrame hands to stateEstimation, resident in HBM (srl_cloud_frame), final frame order."""
