@@ -605,6 +605,68 @@ int srl_image_vio_last_summary(srl_image* img, int32_t which, int32_t* iteration
 /* device time of the last launch of each update (CUDA events around the kernel; inputs and the result copy excluded) */
 int srl_image_vio_last_times(srl_image* img, double* esikf_ms, double* photometric_ms);
 
+/* ---- row N9: the optical-flow tracker's bookkeeping around its Lucas-Kanade (DESIGN.md row N9): opticalFlowTracker's init /
+ * setTrackPoints (src/opticalFlowTracker.cpp:188-211), trackImage (:111-186, distance -20), removeOutlierUsingRansacPnp (:267-323,
+ * if_remove_ourlier 1) and updateAndAppendTrackPoints (:13-102).  The tracker keeps three point sets on the device, each sorted
+ * by colour-map point id (the reference's std::maps are ordered by rgbPoint*; DESIGN.md section 5):
+ *   last  = map_rgb_points_in_last_image_pose: ids + uv (float pairs)
+ *   match = what trackImage's Lucas-Kanade tracked (status set), in last order: ids, last uv, new uv; the list
+ *           findFundamentalMat is given, so a caller's fundamental-matrix RANSAC runs on it
+ *   cur   = map_rgb_points_in_cur_image_pose: ids, uv, image_velocity (double pairs)
+ * The two RANSACs stay with the caller: srl_flow_tracker_reject_matches takes findFundamentalMat's mask and
+ * srl_flow_tracker_remove_outliers solvePnPRansac's inliers.  rgbPoint::is_out_lier_count is kept in the colour map's per-point
+ * state (zero for a new point).  cm and lk must be created on ctx; the tracker calls lk for every image it tracks. */
+typedef struct srl_flow_tracker srl_flow_tracker;
+typedef struct srl_flow_tracker_sets_out {   /* device pointers, valid until the next call on the tracker */
+    int64_t n_match, n_cur, n_last;
+    const uint32_t* match_ids;
+    const float* match_last_uv;              /* n_match (x, y) pairs: the points findFundamentalMat's first argument holds */
+    const float* match_uv;                   /* n_match (x, y) pairs: its second */
+    const uint32_t* cur_ids;                 /* the ids, uv and velocity srl_image_vio_esikf / _photometric take */
+    const float* cur_uv;
+    const double* cur_velocity;
+    const uint32_t* last_ids;                /* the ids srl_color_map_gather_points takes */
+    const float* last_uv;
+    double last_image_time;
+} srl_flow_tracker_sets_out;
+/* maximum_tracked_points >= 1 (300 in the reference) */
+int srl_flow_tracker_create(srl_ctx* ctx, srl_color_map* cm, srl_lk* lk, int32_t maximum_tracked_points, srl_flow_tracker** out);
+void srl_flow_tracker_destroy(srl_flow_tracker* t);
+/* init: last = {ids[i] -> uv[i]} (a later duplicate id overwrites an earlier one), both image times = image_time, then the
+ * Lucas-Kanade call on gray (cols x rows, rows `pitch` bytes apart), which on lk's first image builds its pyramid only.  ids (n)
+ * and uv (n float pairs) are host or device memory.  An id that names no stored point, or an image lk refuses: SRL_BAD_ARG,
+ * and the tracker is not changed. */
+int srl_flow_tracker_init(srl_flow_tracker* t, const uint8_t* gray, int cols, int rows, size_t pitch, double image_time,
+                          const uint32_t* ids, const float* uv, size_t n);
+/* trackImage: cur and the match list are cleared; with fewer than 30 points in last only last_image_time = image_time (lk is not
+ * called, *lk_called = 0).  Otherwise Lucas-Kanade over last's uv, the matches in last order, and cur = the matches with
+ * if2dPointsAvailable(x, y, 1.0, 0.05) on a cols x rows image, with velocity (1e-3, 1e-3) when image_time - last_image_time <
+ * 1e-5, else (new - old) / dt in cv::Point2f arithmetic.  last is not changed.  lk_called may be NULL. */
+int srl_flow_tracker_track_image(srl_flow_tracker* t, const uint8_t* gray, int cols, int rows, size_t pitch, double image_time,
+                                 int32_t* lk_called);
+/* findFundamentalMat's status: one byte per match (n == n_match, host or device), non-zero = inlier; cur is rebuilt as the
+ * matches inside the margin whose byte is set.  mask NULL: every match is an inlier.  A length mismatch: SRL_BAD_ARG. */
+int srl_flow_tracker_reject_matches(srl_flow_tracker* t, const uint8_t* mask, size_t n);
+/* removeOutlierUsingRansacPnp: with fewer than 10 points in cur, *result = 0 and nothing changes.  Otherwise last and cur both
+ * become the entries of cur at the n indices `inliers` (host or device, in any order, repeats allowed), with cur's uv; inliers
+ * NULL: all of cur.  *result = 1.  An index outside [0, n_cur): SRL_BAD_ARG, nothing changed.  When the caller's
+ * solvePnPRansac fails or throws, the reference returns before this point: do not call it. */
+int srl_flow_tracker_remove_outliers(srl_flow_tracker* t, const int32_t* inliers, size_t n, int32_t* result);
+/* updateAndAppendTrackPoints(p_frame, map_tracker, mini_distance): cam is the image frame's camera after the updates (fov_margin
+ * as its state holds it, 0.005 in the reference); the reprojection threshold is 2 * cam->cols / 320.  Every entry of last is
+ * projected; one whose error exceeds the threshold twice in a row, or twice the threshold once, is erased (its count reset);
+ * the others keep their place and mark their pixel cell.  Then the candidates (n ids, host or device, the selection's order;
+ * refreshPointsForProjection's points_rgb_vec_for_projection) not in last whose projection succeeds and whose cell is free
+ * enter last with the projection as uv, until last holds maximum_tracked_points (one more can enter when it already did).
+ * SRL_BAD_ARG (nothing changed) for an id that names no stored point, mini_distance not finite or <= 0, cols or rows < 2, a
+ * fov_margin whose cell coordinates do not fit an int. */
+int srl_flow_tracker_update_and_append(srl_flow_tracker* t, const srl_camera* cam, double mini_distance, const uint32_t* candidates,
+                                       size_t n);
+/* the three sets' counts and device pointers */
+int srl_flow_tracker_sets(srl_flow_tracker* t, srl_flow_tracker_sets_out* out);
+/* test hook: is_out_lier_count of n point ids (host or device) into counts (n int16, host or device) */
+int srl_flow_tracker_outlier_counts(srl_flow_tracker* t, const uint32_t* ids, size_t n, int16_t* counts);
+
 /* eskfEstimator::observe (src/eskfEstimator.cpp:219-230) — host math, exported for parity tests */
 int srl_eskf_observe(srl_eskf_state* eskf, const double d_x[17]);
 

@@ -333,9 +333,56 @@ public:
         return ml;
     }
 
+    srl_lk* handle() { return lk_; }
+
 private:
     srl_ctx* ctx_ = nullptr;
     srl_lk* lk_ = nullptr;
+    void check(int rc, const char* what) {
+        if (rc != SRL_OK) throw std::runtime_error(std::string(what) + ": " + (ctx_ ? srl_last_error(ctx_) : "no context"));
+    }
+};
+
+// opticalFlowTracker's bookkeeping (src/opticalFlowTracker.cpp) on the GPU: last, the match list and cur kept on the device in
+// point-id order from one image to the next.  The caller's RANSACs plug in between: findFundamentalMat on matches() ->
+// rejectMatches(mask); solvePnPRansac on current() -> removeOutlierUsingRansacPnp(inliers).  Pointers are host or device
+// memory; the sets' pointers are device memory, valid until the next call.  Destroy before the map, the kernel and the context.
+class OpticalFlowTracker {
+public:
+    OpticalFlowTracker(srl_ctx* ctx, srl_color_map* cm, LKOpticalFlowKernel& lk, int maximum_tracked_points = 300) : ctx_(ctx) {
+        check(srl_flow_tracker_create(ctx, cm, lk.handle(), maximum_tracked_points, &t_), "srl_flow_tracker_create");
+    }
+    ~OpticalFlowTracker() { if (t_) srl_flow_tracker_destroy(t_); }
+    OpticalFlowTracker(const OpticalFlowTracker&) = delete;
+    OpticalFlowTracker& operator=(const OpticalFlowTracker&) = delete;
+
+    void init(const uint8_t* gray, int cols, int rows, size_t pitch, double time, const uint32_t* ids, const float* uv, size_t n) {
+        check(srl_flow_tracker_init(t_, gray, cols, rows, pitch, time, ids, uv, n), "srl_flow_tracker_init");
+    }
+    // returns whether Lucas-Kanade ran (30 points or more in last)
+    bool trackImage(const uint8_t* gray, int cols, int rows, size_t pitch, double time) {
+        int32_t called = 0;
+        check(srl_flow_tracker_track_image(t_, gray, cols, rows, pitch, time, &called), "srl_flow_tracker_track_image");
+        return called != 0;
+    }
+    void rejectMatches(const uint8_t* mask, size_t n) { check(srl_flow_tracker_reject_matches(t_, mask, n), "srl_flow_tracker_reject_matches"); }
+    bool removeOutlierUsingRansacPnp(const int32_t* inliers, size_t n) {
+        int32_t r = 0;
+        check(srl_flow_tracker_remove_outliers(t_, inliers, n, &r), "srl_flow_tracker_remove_outliers");
+        return r != 0;
+    }
+    void updateAndAppendTrackPoints(const srl_camera& cam, double mini_distance, const uint32_t* candidates, size_t n) {
+        check(srl_flow_tracker_update_and_append(t_, &cam, mini_distance, candidates, n), "srl_flow_tracker_update_and_append");
+    }
+    srl_flow_tracker_sets_out sets() {
+        srl_flow_tracker_sets_out s{};
+        check(srl_flow_tracker_sets(t_, &s), "srl_flow_tracker_sets");
+        return s;
+    }
+
+private:
+    srl_ctx* ctx_ = nullptr;
+    srl_flow_tracker* t_ = nullptr;
     void check(int rc, const char* what) {
         if (rc != SRL_OK) throw std::runtime_error(std::string(what) + ": " + (ctx_ ? srl_last_error(ctx_) : "no context"));
     }

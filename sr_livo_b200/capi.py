@@ -97,6 +97,13 @@ class ProjectionParams(C.Structure):
                 ("maximum_depth", C.c_double)]
 
 
+class FlowTrackerSets(C.Structure):
+    """srl_flow_tracker_sets_out: the optical-flow tracker's set counts and device pointers."""
+    _fields_ = [("n_match", C.c_int64), ("n_cur", C.c_int64), ("n_last", C.c_int64), ("match_ids", C.c_void_p),
+                ("match_last_uv", C.c_void_p), ("match_uv", C.c_void_p), ("cur_ids", C.c_void_p), ("cur_uv", C.c_void_p),
+                ("cur_velocity", C.c_void_p), ("last_ids", C.c_void_p), ("last_uv", C.c_void_p), ("last_image_time", C.c_double)]
+
+
 class BuildFrameParams(C.Structure):
     """srl_build_frame_params: buildFrame's inputs (src/lioOptimization.cpp:821-893)."""
     _fields_ = [("timestamp_begin", C.c_double), ("timestamp_offset", C.c_double), ("point_time_enable", C.c_int32),
@@ -143,6 +150,9 @@ EXPORTS = [
     "srl_lk_create", "srl_lk_destroy", "srl_lk_track_image", "srl_lk_info", "srl_lk_download_level", "srl_lk_last_times",
     "srl_image_create", "srl_image_destroy", "srl_image_process", "srl_image_info", "srl_image_download_maps", "srl_image_last_times",
     "srl_image_vio_esikf", "srl_image_vio_photometric", "srl_image_covariance", "srl_image_vio_last_summary", "srl_image_vio_last_times",
+    "srl_flow_tracker_create", "srl_flow_tracker_destroy", "srl_flow_tracker_init", "srl_flow_tracker_track_image",
+    "srl_flow_tracker_reject_matches", "srl_flow_tracker_remove_outliers", "srl_flow_tracker_update_and_append", "srl_flow_tracker_sets",
+    "srl_flow_tracker_outlier_counts",
 ]
 
 _lib = None
@@ -258,6 +268,16 @@ def lib():
     L.srl_image_covariance.argtypes = [vp, vp, vp]
     L.srl_image_vio_last_summary.argtypes = [vp, i32, C.POINTER(i32), C.POINTER(i32), C.POINTER(dbl)]
     L.srl_image_vio_last_times.argtypes = [vp, C.POINTER(dbl), C.POINTER(dbl)]
+    L.srl_flow_tracker_create.argtypes = [vp, vp, vp, i32, C.POINTER(vp)]
+    L.srl_flow_tracker_destroy.argtypes = [vp]
+    L.srl_flow_tracker_destroy.restype = None
+    L.srl_flow_tracker_init.argtypes = [vp, vp, C.c_int, C.c_int, sz, dbl, vp, vp, sz]
+    L.srl_flow_tracker_track_image.argtypes = [vp, vp, C.c_int, C.c_int, sz, dbl, C.POINTER(i32)]
+    L.srl_flow_tracker_reject_matches.argtypes = [vp, vp, sz]
+    L.srl_flow_tracker_remove_outliers.argtypes = [vp, vp, sz, C.POINTER(i32)]
+    L.srl_flow_tracker_update_and_append.argtypes = [vp, C.POINTER(Camera), dbl, vp, sz]
+    L.srl_flow_tracker_sets.argtypes = [vp, C.POINTER(FlowTrackerSets)]
+    L.srl_flow_tracker_outlier_counts.argtypes = [vp, vp, sz, vp]
     L.srl_cloud_frame_create.argtypes = [vp, sz, C.POINTER(vp)]
     L.srl_cloud_frame_destroy.argtypes = [vp]
     L.srl_cloud_frame_destroy.restype = None

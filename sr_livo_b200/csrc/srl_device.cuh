@@ -22,7 +22,9 @@ constexpr int kMetaKeyLo = 0 * 4 + 3, kMetaKeyHi = 1 * 4 + 3, kMetaCount = 2 * 4
 
 struct ColorPoint {            // colour state of one stored point of a colour map (rgbPoint minus position), index = block * block_pts + i
     short rgb[3]; short n_rgb;
-    float cov[3]; float pad;
+    float cov[3];
+    short outlier_count;       // rgbPoint::is_out_lier_count, the optical-flow tracker's (srl_flow_tracker.cu)
+    short pad;
     double obs_dist, last_obs;
 };
 

@@ -346,6 +346,34 @@ __device__ __forceinline__ void sub_pixel_bgr(const unsigned char* __restrict__ 
 }
 #endif
 
+// An srl_camera as the projection kernels read it (camera_constants)
+struct CamConst { double R[9], t_cw[3], t_wc[3], fx, fy, cx, cy, fov; int cols, rows; };
+CamConst camera_constants(const srl_camera* cam);
+// The cell coordinates of one image axis for cells of min_dis pixels over the FoV window of `fov`: the axis offset and its
+// bit count (srl_map.cu).  False when they do not fit an int.
+bool cell_axis(double fov, int size, double min_dis, int& offset, int& bits);
+#if defined(__CUDACC__)
+// cloudFrame::project3dPointInThisImage with scale 1 (src/lioOptimization.cpp:142-198) of a stored position widened to double:
+// project3dTo2d (reject pcz < 0.001), then if2dPointsAvailable with the frame's own fov_margin.  Products and sums rounded one
+// by one like the host code.  The renderer, the tracker's selection and the optical-flow tracker project through it.
+// *z_ok (may be null) tells whether project3dTo2d got as far as writing u and v.
+__device__ __forceinline__ bool project_in_image(const CamConst& c, double px, double py, double pz, double& u, double& v,
+                                                 bool* z_ok = nullptr) {
+    double cxm, cym, czm;
+    matvec3_exact(c.R, px, py, pz, cxm, cym, czm);
+    const double pcx = __dadd_rn(cxm, c.t_cw[0]), pcy = __dadd_rn(cym, c.t_cw[1]), pcz = __dadd_rn(czm, c.t_cw[2]);
+    if (z_ok) *z_ok = !(pcz < 0.001);
+    if (pcz < 0.001) return false;
+    u = __dadd_rn(__ddiv_rn(__dmul_rn(pcx, c.fx), pcz), c.cx);
+    v = __dadd_rn(__ddiv_rn(__dmul_rn(pcy, c.fy), pcz), c.cy);
+    return (u >= __dadd_rn(__dmul_rn(c.fov, (double)c.cols), 1.0)) && (ceil(u) < __dmul_rn(__dsub_rn(1.0, c.fov), (double)c.cols)) &&
+           (v >= __dadd_rn(__dmul_rn(c.fov, (double)c.rows), 1.0)) && (ceil(v) < __dmul_rn(__dsub_rn(1.0, c.fov), (double)c.rows));
+}
+// The pixel cell of a projected coordinate (src/rgbMapTracker.cpp:116-117, src/opticalFlowTracker.cpp:29-30): std::round (half
+// away from zero), times min_dis, the double truncated to int
+__device__ __forceinline__ int projection_cell(double x, double min_dis) { return (int)__dmul_rn(round(__ddiv_rn(x, min_dis)), min_dis); }
+#endif
+
 // A colour map's stored points as the camera updates read them (srl_map.cu owns the map): position of point id in
 // blocks[(id / block_pts) * 4 * block_pts + 4 * (id % block_pts)], colour state in cpts[id]; an id is valid when its block is
 // below n_voxels and its index below the block's count.
@@ -357,6 +385,9 @@ struct ColorMapView {
 };
 ColorMapView color_map_view(const srl_color_map* cm);
 srl_ctx* color_map_ctx(const srl_color_map* cm);
+// The colour states of a colour map for the one writer outside srl_map.cu: the optical-flow tracker's is_out_lier_count
+ColorPoint* color_map_states(srl_color_map* cm);
+srl_ctx* lk_ctx(const srl_lk* lk);
 
 // Which compiled instance of each pass kernel a ctx launches, and the state of its sweep-order sort.  Filled once by
 // srl_ctx_create (defaults, then the SRL_* environment variables), changed by srl_ctx_set_option.

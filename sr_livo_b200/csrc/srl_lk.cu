@@ -306,6 +306,7 @@ struct srl_lk {
     cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};   // call start, pyramid built, points tracked
     bool timed = false;
 };
+srl_ctx* srl::lk_ctx(const srl_lk* lk) { return lk->ctx; }
 
 namespace {
 

@@ -297,7 +297,7 @@ __global__ void k_color_seg_process(Slot* slots, float* blocks, ColorPoint* cpts
         const unsigned int i = idx[j];
         bp[4 * count] = fxyz[3 * (size_t)i]; bp[4 * count + 1] = fxyz[3 * (size_t)i + 1]; bp[4 * count + 2] = fxyz[3 * (size_t)i + 2];
         ColorPoint cp;                                            // rgbPoint::reset() (src/cloudMap.cpp:12-19)
-        cp.rgb[0] = cp.rgb[1] = cp.rgb[2] = 0; cp.n_rgb = 0; cp.cov[0] = cp.cov[1] = cp.cov[2] = 0.f; cp.pad = 0.f; cp.obs_dist = 0.0; cp.last_obs = 0.0;
+        cp.rgb[0] = cp.rgb[1] = cp.rgb[2] = 0; cp.n_rgb = 0; cp.cov[0] = cp.cov[1] = cp.cov[2] = 0.f; cp.outlier_count = 0; cp.pad = 0; cp.obs_dist = 0.0; cp.last_obs = 0.0;
         cpts[(size_t)blk * block_pts + count] = cp;
         accept_id[i] = blk * (unsigned)block_pts + (unsigned)count;
         ++count; ++added;
@@ -356,20 +356,6 @@ __global__ void k_color_emit_rgb(Slot* fine, unsigned int fmask, const unsigned 
     slot_claim(fine, fmask, k, x, y, z, (unsigned)pos, 1u);       // hashmap_3d_points.insert (:481, :506)
 }
 
-struct CamConst { double R[9], t_cw[3], t_wc[3], fx, fy, cx, cy, fov; int cols, rows; };
-// cloudFrame::project3dPointInThisImage with scale 1 (src/lioOptimization.cpp:142-198) of a stored position widened to double:
-// project3dTo2d (reject pcz < 0.001), then if2dPointsAvailable with the frame's own fov_margin.  Products and sums rounded one
-// by one like the host code.  The renderer and the tracker's selection both project through it.
-__device__ __forceinline__ bool project_in_image(const CamConst& c, double px, double py, double pz, double& u, double& v) {
-    double cxm, cym, czm;
-    matvec3_exact(c.R, px, py, pz, cxm, cym, czm);
-    const double pcx = __dadd_rn(cxm, c.t_cw[0]), pcy = __dadd_rn(cym, c.t_cw[1]), pcz = __dadd_rn(czm, c.t_cw[2]);
-    if (pcz < 0.001) return false;
-    u = __dadd_rn(__ddiv_rn(__dmul_rn(pcx, c.fx), pcz), c.cx);
-    v = __dadd_rn(__ddiv_rn(__dmul_rn(pcy, c.fy), pcz), c.cy);
-    return (u >= __dadd_rn(__dmul_rn(c.fov, (double)c.cols), 1.0)) && (ceil(u) < __dmul_rn(__dsub_rn(1.0, c.fov), (double)c.cols)) &&
-           (v >= __dadd_rn(__dmul_rn(c.fov, (double)c.rows), 1.0)) && (ceil(v) < __dmul_rn(__dsub_rn(1.0, c.fov), (double)c.rows));
-}
 // (point_world - t_world_camera).norm(), the 3-term sum as c0 + (c1 + c2) (DESIGN.md section 2)
 __device__ __forceinline__ double camera_distance(const CamConst& c, double px, double py, double pz) {
     const double dx = __dsub_rn(px, c.t_wc[0]), dy = __dsub_rn(py, c.t_wc[1]), dz = __dsub_rn(pz, c.t_wc[2]);
@@ -514,9 +500,7 @@ __global__ void k_proj_candidates(const Slot* slots, unsigned int mask, const fl
         d = camera_distance(c, px, py, pz);                         // :97
         double u, v;
         if (!(d > max_depth) && !(d < min_depth) && project_in_image(c, px, py, pz, u, v)) {   // :99-114
-            // :116-117: std::round (half away from zero), times minimum_dis, the double truncated to int
-            const int cu = (int)__dmul_rn(round(__ddiv_rn(u, min_dis)), min_dis);
-            const int cv = (int)__dmul_rn(round(__ddiv_rn(v, min_dis)), min_dis);
+            const int cu = projection_cell(u, min_dis), cv = projection_cell(v, min_dis);   // :116-117
             k = ((unsigned long long)(unsigned)(cu - u0) << bits_v) | (unsigned long long)(unsigned)(cv - v0);
             uv[j] = make_float2(__double2float_rn(u), __double2float_rn(v));   // cv::Point2f(u_f, v_f)
         }
@@ -773,8 +757,8 @@ int srl::check_lio_map(srl_ctx* ctx, const srl_map* m) {
 }
 
 // ---- N4: colour map host side ---------------------------------------------------------------------------------------
-// the renderer's and the selection's projection constants of a camera
-static CamConst camera_constants(const srl_camera* cam) {
+// the projection constants of a camera (renderer, selection, optical-flow tracker)
+CamConst srl::camera_constants(const srl_camera* cam) {
     CamConst c;
     quat_to_rot(cam->q_camera_world, c.R);
     for (int i = 0; i < 3; ++i) { c.t_cw[i] = cam->t_camera_world[i]; c.t_wc[i] = cam->t_world_camera[i]; }
@@ -808,6 +792,7 @@ ColorMapView srl::color_map_view(const srl_color_map* cm) {
     return ColorMapView{cm->vox->d_blocks, cm->d_cpts, cm->vox->block_pts, (long long)cm->vox->n_voxels};
 }
 srl_ctx* srl::color_map_ctx(const srl_color_map* cm) { return cm->ctx; }
+ColorPoint* srl::color_map_states(srl_color_map* cm) { return cm->d_cpts; }
 
 // the colour state of committed_voxels voxels (called by map_grow before the blocks grow)
 static int color_map_grow_voxels(srl_color_map* cm, size_t committed_voxels) {
@@ -1725,7 +1710,7 @@ int srl_color_map_export(srl_color_map* cm, int32_t min_views, int32_t order, fl
 // |x| <= a = max(|lo|, |hi|), and the cell std::round(x / d) * d lies within 2a + 1 of zero (it is 0, or |x / d| >= 1/2 and
 // |round(x / d)| <= 2 |x / d|).  The axis is offset by -b (b = ceil(2a) + 2) and takes `bits` bits, with 2^bits > 2b + 1 so that
 // an all-ones field never comes from a cell.  False when b does not fit an int or x / d can overflow.
-static bool cell_axis(double fov, int size, double min_dis, int& offset, int& bits) {
+bool srl::cell_axis(double fov, int size, double min_dis, int& offset, int& bits) {
     const double lo = fov * (double)size + 1.0, hi = (1.0 - fov) * (double)size;
     const double a = std::max(std::fabs(lo), std::fabs(hi));
     if (!(a < 1e9) || !(a / min_dis < 1e300)) return false;

@@ -14,6 +14,7 @@ Names and argument meaning follow the reference so the parity tests read like it
   rgbMapTracker::selectPointsForProjection src/rgbMapTracker.cpp:45     -> ColorVoxelMap.selectPointsForProjection / gatherPoints
   LKOpticalFlowKernel::trackImage       src/lkpyramid.cpp:755           -> LKOpticalFlowKernel.trackImage
   imageProcessing::process (:91-125)    src/imageProcessing.cpp:91      -> ImageProcessing.process
+  opticalFlowTracker                    src/opticalFlowTracker.cpp      -> OpticalFlowTracker
 
 Error behaviour: optimizeSummary.success=false <-> OptimizeSummary.success False (SRL_TOO_FEW_RESIDUALS);
 the reference's `throw std::runtime_error("error")` on NaN planarity <-> RuntimeError; everything else raises
@@ -1045,6 +1046,157 @@ class ImageProcessing:
         return a.value, b.value
 
 
+def _gray_2d(gray):
+    """(address, rows, cols, row pitch in bytes) of a 2-D uint8 image with unit column stride; rows may be padded."""
+    if _is_tensor(gray):
+        if str(gray.dtype) != "torch.uint8" or gray.dim() != 2 or gray.stride(1) != 1:
+            raise TypeError("expected a 2-D torch.uint8 image with unit column stride")
+        return gray.data_ptr(), gray.shape[0], gray.shape[1], gray.stride(0)
+    if not (isinstance(gray, np.ndarray) and gray.dtype == np.uint8 and gray.ndim == 2 and gray.strides[1] == 1):
+        raise TypeError("expected a 2-D uint8 array with unit column stride")
+    return gray.ctypes.data, gray.shape[0], gray.shape[1], gray.strides[0]
+
+
+class _DeviceArray:
+    """A view of device memory for torch.as_tensor (the CUDA array interface): no copy."""
+
+    def __init__(self, p, shape, typestr):
+        self.__cuda_array_interface__ = dict(shape=shape, typestr=typestr, data=(p, False), version=3, strides=None)
+
+
+_NO_INLIERS = np.zeros(1, np.int32)
+
+
+class OpticalFlowTracker:
+    """opticalFlowTracker (src/opticalFlowTracker.cpp, srl_flow_tracker_*): the tracked point sets of the camera frame kept on the
+    device from one image to the next, in colour-map point id order.  lk is the LKOpticalFlowKernel it tracks with
+    (LKOpticalFlowKernel(ctx, **tracker_lk_params()) as the reference's constructor makes it); cmap holds the points.
+
+    Per image, as imageProcessing::process calls it: trackImage(gray, t) -> (caller's findFundamentalMat on matches(),
+    rejectMatches(mask)) -> (caller's solvePnPRansac on current(), removeOutlierUsingRansacPnp(inliers)) -> the camera updates on
+    current(device=True) -> render -> refresh selection -> updateAndAppendTrackPoints(camera, selected ids, 40 / scale).
+    Point lists are numpy arrays or torch tensors, host or CUDA; the set accessors return numpy copies, or with device=True
+    torch views of the tracker's own memory, valid until its next call."""
+
+    def __init__(self, ctx: Context, cmap: "ColorVoxelMap", lk: "LKOpticalFlowKernel", maximum_tracked_points: int = 300):
+        self.ctx, self.cmap, self.lk = ctx, cmap, lk
+        h = C.c_void_p()
+        _check(ctx.h, lib().srl_flow_tracker_create(ctx.h, cmap.h, lk.h, int(maximum_tracked_points), C.byref(h)))
+        self.h = h
+
+    def close(self):
+        if getattr(self, "h", None):
+            lib().srl_flow_tracker_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def init(self, gray, image_time: float, ids, uv) -> None:
+        """init / setTrackPoints (:188-211): last = {ids[i]: uv[i]}, both image times = image_time, and the Lucas-Kanade call
+        on gray (its first image: the pyramid only).  ids: uint32 point ids (int32 tensors hold their bits); uv: (n, 2) float32."""
+        p_img, rows, cols, pitch = _gray_2d(gray)
+        p_ids, n = _ids_addr(ids)
+        p_uv, n_uv = _addr(uv, np.float32, 2)
+        if n_uv != n:
+            raise ValueError("ids and uv must hold the same number of points")
+        _check(self.ctx.h, lib().srl_flow_tracker_init(self.h, C.c_void_p(p_img), int(cols), int(rows), int(pitch), float(image_time),
+                                                       C.c_void_p(p_ids), C.c_void_p(p_uv), n))
+
+    def trackImage(self, gray, image_time: float) -> bool:
+        """trackImage(p_frame, -20) (:111-186) on gray_image at time_sweep_end; returns whether Lucas-Kanade ran (not below 30
+        tracked points)."""
+        p_img, rows, cols, pitch = _gray_2d(gray)
+        called = C.c_int32(0)
+        _check(self.ctx.h, lib().srl_flow_tracker_track_image(self.h, C.c_void_p(p_img), int(cols), int(rows), int(pitch), float(image_time),
+                                                              C.byref(called)))
+        return bool(called.value)
+
+    def rejectMatches(self, mask=None) -> None:
+        """findFundamentalMat's status over matches() (one uint8 per match, non-zero = inlier); None = all inliers."""
+        if mask is None:
+            _check(self.ctx.h, lib().srl_flow_tracker_reject_matches(self.h, None, 0))
+            return
+        if not _is_tensor(mask):
+            mask = np.ascontiguousarray(mask, np.uint8).reshape(-1)
+        p, n = _addr(mask, np.uint8, 1)
+        _check(self.ctx.h, lib().srl_flow_tracker_reject_matches(self.h, C.c_void_p(p), n))
+
+    def removeOutlierUsingRansacPnp(self, inliers=None) -> bool:
+        """removeOutlierUsingRansacPnp(p_frame, 1) (:267-323) with solvePnPRansac's inlier indices into current() (int32, any
+        order, repeats allowed); None = all.  False (nothing changed) below 10 current points."""
+        r = C.c_int32(0)
+        if inliers is None:
+            _check(self.ctx.h, lib().srl_flow_tracker_remove_outliers(self.h, None, 0, C.byref(r)))
+            return bool(r.value)
+        if not _is_tensor(inliers):
+            inliers = np.ascontiguousarray(inliers, np.int32).reshape(-1)
+        p, n = _addr(inliers, np.int32, 1)
+        if n == 0:
+            p = _NO_INLIERS.ctypes.data          # an empty list is zero inliers, which a NULL pointer would not say
+        _check(self.ctx.h, lib().srl_flow_tracker_remove_outliers(self.h, C.c_void_p(p), n, C.byref(r)))
+        return bool(r.value)
+
+    def updateAndAppendTrackPoints(self, camera: "capi.Camera", candidates, mini_distance: float) -> None:
+        """updateAndAppendTrackPoints(p_frame, map_tracker, mini_distance) (:13-102): camera is the frame's after the updates
+        (fov_margin 0.005), candidates the refresh selection's point ids in its order (points_rgb_vec_for_projection)."""
+        p, n = _ids_addr(candidates)
+        _check(self.ctx.h, lib().srl_flow_tracker_update_and_append(self.h, C.byref(camera), float(mini_distance), C.c_void_p(p), n))
+
+    def _sets(self) -> "capi.FlowTrackerSets":
+        s = capi.FlowTrackerSets()
+        _check(self.ctx.h, lib().srl_flow_tracker_sets(self.h, C.byref(s)))
+        return s
+
+    def counts(self) -> dict:
+        s = self._sets()
+        return dict(match=s.n_match, cur=s.n_cur, last=s.n_last)
+
+    def _arrays(self, device, spec):
+        import torch
+        out = []
+        for p, n, w, ts in spec:
+            shape = (n,) if w == 1 else (n, w)
+            if n == 0:
+                t = torch.empty(shape, dtype={"<i4": torch.int32, "<f4": torch.float32, "<f8": torch.float64}[ts],
+                                device=f"cuda:{self.ctx.device}")
+            else:
+                t = torch.as_tensor(_DeviceArray(p, shape, ts), device=f"cuda:{self.ctx.device}")
+            out.append(t if device else (t.cpu().numpy().view(np.uint32) if ts == "<i4" else t.cpu().numpy()))
+        return tuple(out)
+
+    def matches(self, device: bool = False):
+        """(ids, last uv (n, 2) float32, new uv (n, 2) float32): what trackImage's Lucas-Kanade tracked, in last order — the two
+        point lists findFundamentalMat is given.  ids are uint32 (numpy) or int32 holding their bits (device)."""
+        s = self._sets()
+        return self._arrays(device, [(s.match_ids, s.n_match, 1, "<i4"), (s.match_last_uv, s.n_match, 2, "<f4"),
+                                     (s.match_uv, s.n_match, 2, "<f4")])
+
+    def current(self, device: bool = False):
+        """(ids, uv (n, 2) float32, velocity (n, 2) float64): map_rgb_points_in_cur_image_pose and the points' image_velocity, what
+        vioEsikf / vioPhotometric take."""
+        s = self._sets()
+        return self._arrays(device, [(s.cur_ids, s.n_cur, 1, "<i4"), (s.cur_uv, s.n_cur, 2, "<f4"), (s.cur_velocity, s.n_cur, 2, "<f8")])
+
+    def last(self, device: bool = False):
+        """(ids, uv (n, 2) float32): map_rgb_points_in_last_image_pose."""
+        s = self._sets()
+        return self._arrays(device, [(s.last_ids, s.n_last, 1, "<i4"), (s.last_uv, s.n_last, 2, "<f4")])
+
+    def lastImageTime(self) -> float:
+        return self._sets().last_image_time
+
+    def outlierCounts(self, ids) -> np.ndarray:
+        """Test hook: rgbPoint::is_out_lier_count of each point id, int16."""
+        ids = np.ascontiguousarray(ids, np.uint32).reshape(-1)
+        out = np.zeros(ids.size, np.int16)
+        _check(self.ctx.h, lib().srl_flow_tracker_outlier_counts(self.h, ptr(ids), ids.size, ptr(out)))
+        return out
+
+
 def _quat_to_rot(q):
     """Eigen's Quaterniond::toRotationMatrix, q = (x, y, z, w)."""
     x, y, z, w = (float(v) for v in q)
@@ -1129,4 +1281,4 @@ class CameraState:
 
 __all__ = ["Context", "VoxelHashMap", "ColorVoxelMap", "Sweep", "EskfEstimator", "LioOptimization", "OptimizeSummary", "PlaneResiduals",
            "IcpParams", "r3live_params", "r3live_map_options", "r3live_compressed_map_options", "make_frame", "SrlError", "write_pcd_xyzrgb",
-           "LKOpticalFlowKernel", "tracker_lk_params", "ImageProcessing", "CameraState", "r3live_camera_params", "ntu_camera_params"]
+           "LKOpticalFlowKernel", "tracker_lk_params", "OpticalFlowTracker", "ImageProcessing", "CameraState", "r3live_camera_params", "ntu_camera_params"]
