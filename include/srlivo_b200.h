@@ -498,7 +498,7 @@ int srl_color_map_select_for_projection(srl_color_map* cm, const srl_camera* cam
                                         uint32_t* point_ids, float* xyz, float* uv, size_t max_points, int64_t* n_out);
 /* the per-point state the tracker reads, by point id (opticalFlowTracker.cpp:25,75,226,280 read positions;
  * imageProcessing.cpp:465-478 colour, N_rgb and covariance): xyz n*3 floats, rgb n*3 shorts (the BGR state as stored),
- * n_rgb n shorts, cov n*3 floats (0 before the first observation), key_index n*4 shorts (voxel key x, y, z, index in block).
+ * n_rgb n shorts, cov n*3 floats (0 while N_rgb == 0; a wrapped, negative N_rgb reports it), key_index n*4 shorts (voxel key x, y, z, index in block).
  * point_ids and every output are host or device memory; any output may be NULL.  An id that names no stored point returns
  * SRL_BAD_ARG and writes nothing. */
 int srl_color_map_gather_points(srl_color_map* cm, const uint32_t* point_ids, size_t n, float* xyz, int16_t* rgb,

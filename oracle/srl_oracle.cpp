@@ -1502,7 +1502,7 @@ int64_t orc_color_snapshot(void* cm_, int32_t cap, int16_t* keys, int32_t* count
             for (int a = 0; a < 3; ++a) {
                 xyz[e * 3 + a] = p ? p->position[a] : 0.f;
                 rgb[e * 3 + a] = p ? p->rgb[a] : (short)0;
-                cov[e * 3 + a] = (p && p->N_rgb > 0) ? p->cov_rgb[a] : 0.f;   // cov_rgb is uninitialised before the first observation
+                cov[e * 3 + a] = (p && p->N_rgb != 0) ? p->cov_rgb[a] : 0.f;   // cov_rgb is uninitialised before the first view; a wrapped (negative) N_rgb has one
             }
             n_rgb[e] = p ? p->N_rgb : (short)0;
             obs_dist[e] = p ? p->observe_distance : 0.0;

@@ -249,7 +249,7 @@ int64_t ref_map_snapshot(void* ctx, int32_t which, int32_t cap, int16_t* keys, i
             for (int a = 0; a < 3; ++a) {
                 xyz[e * 3 + a] = p ? p->position(a) : 0.f;
                 if (rgb) rgb[e * 3 + a] = p ? p->rgb[a] : (short)0;
-                if (cov) cov[e * 3 + a] = (p && p->N_rgb > 0) ? p->cov_rgb(a) : 0.f;
+                if (cov) cov[e * 3 + a] = (p && p->N_rgb != 0) ? p->cov_rgb(a) : 0.f;
             }
             if (n_rgb) n_rgb[e] = p ? p->N_rgb : (short)0;
             if (obs_dist) obs_dist[e] = p ? p->observe_distance : 0.0;

@@ -123,7 +123,7 @@ int32_t orc_color_gather(void* cm_, const int16_t* key_index, int64_t n, float* 
         for (int a = 0; a < 3; ++a) {
             xyz[3 * i + a] = p.position[a];
             rgb[3 * i + a] = p.rgb[a];
-            cov[3 * i + a] = p.N_rgb > 0 ? p.cov_rgb[a] : 0.f;   // cov_rgb is uninitialised before the first observation
+            cov[3 * i + a] = p.N_rgb != 0 ? p.cov_rgb[a] : 0.f;   // cov_rgb is uninitialised before the first view; a wrapped (negative) N_rgb has one
         }
         n_rgb[i] = p.N_rgb;
     }

@@ -445,7 +445,7 @@ __global__ void k_color_download(const ColorPoint* __restrict__ cpts, const floa
     const int cnt = (int)reinterpret_cast<const unsigned int*>(blocks + (size_t)v * (4 * block_pts))[kMetaCount];
     const bool on = i < cnt;
     const ColorPoint cp = cpts[(size_t)v * block_pts + i];
-    for (int a = 0; a < 3; ++a) { rgb[3 * e + a] = on ? cp.rgb[a] : (short)0; cov[3 * e + a] = (on && cp.n_rgb > 0) ? cp.cov[a] : 0.f; }
+    for (int a = 0; a < 3; ++a) { rgb[3 * e + a] = on ? cp.rgb[a] : (short)0; cov[3 * e + a] = (on && cp.n_rgb != 0) ? cp.cov[a] : 0.f; }
     n_rgb[e] = on ? cp.n_rgb : (short)0;
     obs_dist[e] = on ? cp.obs_dist : 0.0;
     last_obs[e] = on ? cp.last_obs : 0.0;
@@ -567,7 +567,8 @@ __global__ void k_color_check_ids(const unsigned int* __restrict__ ids, long lon
     const unsigned b = __ballot_sync(0xffffffffu, bad);
     if ((threadIdx.x & 31) == 0 && b) atomicAdd(n_bad, (unsigned long long)__popc(b));
 }
-// position, BGR state, N_rgb and covariance of each id (cov 0 before the first observation, like srl_color_map_download_state)
+// position, BGR state, N_rgb and covariance of each id (cov 0 while N_rgb == 0, like srl_color_map_download_state: a
+// wrapped, negative N_rgb has a covariance)
 __global__ void k_color_gather(const unsigned int* __restrict__ ids, long long n, const float* __restrict__ blocks, int block_pts,
                                const ColorPoint* __restrict__ cpts, float* xyz, short* rgb, short* n_rgb, float* cov) {
     const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -581,7 +582,7 @@ __global__ void k_color_gather(const unsigned int* __restrict__ ids, long long n
     const ColorPoint cp = cpts[id];
     if (rgb) { rgb[3 * t] = cp.rgb[0]; rgb[3 * t + 1] = cp.rgb[1]; rgb[3 * t + 2] = cp.rgb[2]; }
     if (n_rgb) n_rgb[t] = cp.n_rgb;
-    if (cov) for (int a = 0; a < 3; ++a) cov[3 * t + a] = cp.n_rgb > 0 ? cp.cov[a] : 0.f;
+    if (cov) for (int a = 0; a < 3; ++a) cov[3 * t + a] = cp.n_rgb != 0 ? cp.cov[a] : 0.f;
 }
 
 __global__ void k_gather_points(const double* __restrict__ xyz, const unsigned int* __restrict__ sel, int m, double* out) {
