@@ -667,6 +667,62 @@ int srl_flow_tracker_sets(srl_flow_tracker* t, srl_flow_tracker_sets_out* out);
 /* test hook: is_out_lier_count of n point ids (host or device) into counts (n int16, host or device) */
 int srl_flow_tracker_outlier_counts(srl_flow_tracker* t, const uint32_t* ids, size_t n, int16_t* counts);
 
+/* ---- row N10: cloudProcessing (src/cloudProcessing.cpp) and the point pops of getMeasurements (src/lioOptimization.cpp:719-723,
+ * 759-763).  The handlers decode a sensor message as it comes off the wire, order its points as libstdc++'s std::sort does
+ * (the order of equal keys included), filter them as the reference does and append them to a device-resident point_buffer:
+ * raw xyz (3 doubles), relative_time (ms) and timestamp (s) per point.  srl_lidar_cut pops the queue's front while its
+ * timestamp is below t and hands out device pointers that srl_build_frame takes as they are.  Message buffers are host or
+ * device memory (detected per pointer).  Each handler call and each cut reads back once.  Where the reference is undefined:
+ * a Livox message with no point left appends nothing and keeps last_end_time; a ring >= n_scans on the yaw path, or a NaN
+ * sort key (a NaN time field, NaN xyz on the yaw path), is SRL_BAD_ARG with nothing appended and no state changed. */
+typedef struct srl_lidar srl_lidar;
+typedef struct srl_lidar_params {   /* lioOptimization::readParameters' lidar_parameter / common values */
+    int32_t lidar_type;             /* 1 LIVOX, 2 VELO, 3 OUST, 4 ROBO (include/cloudProcessing.h LID_TYPE) */
+    int32_t n_scans;                /* N_SCANS */
+    int32_t scan_rate;              /* SCAN_RATE (Hz) */
+    int32_t time_unit;              /* 0 SEC, 1 MS, 2 US, 3 NS */
+    double blind;                   /* m */
+    int32_t point_filter_num;       /* >= 1 */
+    int32_t reserved;
+} srl_lidar_params;
+typedef struct srl_cloud2_layout {  /* PointCloud2: point_step and the byte offsets msg->fields gives (pcl::fromROSMsg by name) */
+    uint32_t point_step;
+    int32_t off_x, off_y, off_z;    /* float32 */
+    int32_t off_time;               /* VELO "time" float32, OUST "t" uint32, ROBO "timestamp" float64 */
+    int32_t off_ring;               /* "ring": OUST uint8, VELO / ROBO uint16; < 0: absent (ring 0, as a robosense point's default) */
+    uint32_t width;                 /* msg->width: points per row */
+    uint32_t row_step;              /* msg->row_step: bytes from one row to the next; 0: rows packed (width * point_step) */
+} srl_cloud2_layout;
+typedef struct srl_lidar_info {
+    double last_end_time;           /* -1 before the first message */
+    int32_t given_offset_time;      /* isPointTimeEnable(): set by the PointCloud2 handlers, false at creation */
+    int32_t sweep_id;               /* process() calls that decoded a message */
+    double sweep_interval;          /* getSweepInterval() = 1 / scan_rate */
+    int64_t size;                   /* points queued */
+    double front_timestamp, back_timestamp;   /* NaN when the queue is empty */
+    int64_t capacity;               /* points the queue holds before it grows */
+} srl_lidar_info;
+/* initial_capacity: points reserved up front; the queue grows on demand */
+int srl_lidar_create(srl_ctx* ctx, const srl_lidar_params* params, size_t initial_capacity, srl_lidar** out);
+void srl_lidar_destroy(srl_lidar* l);
+/* livoxHandler: n CustomPoint records `stride` (>= 19) bytes apart, packed as the ROS message (offset_time u32 @0, x y z f32 @4,
+ * @8, @12, reflectivity @16, tag @17, line @18; no alignment needed).  *appended may be NULL. */
+int srl_lidar_livox(srl_lidar* l, const uint8_t* records, size_t n, size_t stride, double stamp, int64_t* appended);
+/* process: the handler of params->lidar_type (VELO, OUST, ROBO; SRL_BAD_ARG for LIVOX) over n = width * height points of
+ * layout->point_step bytes, row r at data + r * row_step (row_step 0: rows packed).  SRL_BAD_ARG for a field outside point_step,
+ * row_step below width * point_step, or n not a multiple of width (width 0 takes one row of n points). */
+int srl_lidar_process(srl_lidar* l, const uint8_t* data, size_t n, const srl_cloud2_layout* layout, double stamp, int64_t* appended);
+/* pop while the queue is not empty and front().timestamp < t.  *raw_xyz / *timestamp: the popped points in the queue's device
+ * memory (count x 3 and count doubles), valid until the next handler call on l (which may move the queue); either may be NULL.
+ * A handle is not thread-safe: calls on one srl_lidar (and the srl_build_frame that reads a cut's pointers) must not overlap. */
+int srl_lidar_cut(srl_lidar* l, double t, int64_t* count, const double** raw_xyz, const double** timestamp);
+int srl_lidar_info_get(srl_lidar* l, srl_lidar_info* info);
+/* host copies of the whole queue, front first; any pointer may be NULL */
+int srl_lidar_download(srl_lidar* l, double* raw_xyz, double* relative_time, double* timestamp);
+/* the device std::sort alone, for tests: perm_out[p] = the index of the key that ends at p (host, n); keys host or device;
+ * *heapsorts = segments the depth limit handed to the heapsort fallback (may be NULL).  NaN keys: SRL_BAD_ARG. */
+int srl_lidar_sort_replay(srl_ctx* ctx, const double* keys, size_t n, int32_t* perm_out, int32_t* heapsorts);
+
 /* eskfEstimator::observe (src/eskfEstimator.cpp:219-230) — host math, exported for parity tests */
 int srl_eskf_observe(srl_eskf_state* eskf, const double d_x[17]);
 

@@ -456,4 +456,76 @@ private:
     }
 };
 
+// cloudProcessing (include/cloudProcessing.h, src/cloudProcessing.cpp) on the GPU with its point_buffer kept on the device: the
+// constructor takes what lioOptimization::readParameters sets (setLidarType, setNumScans, setScanRate, setTimeUnit, setBlind,
+// setPointFilterNum); livoxHandler / process mirror the reference's handlers over the message as it comes off the wire (Livox
+// CustomPoint records, PointCloud2 data with the layout msg->fields gives); cut() is getMeasurements' pop loop (front timestamp
+// below t) and hands out device pointers that LioBackend::buildFrame / srl_build_frame take as they are, valid until the next
+// handler call.  Message pointers take host or device memory.  Not thread-safe: serialise handler calls against cut() and the
+// buildFrame that reads its pointers.  Destroy before the context.
+class cloudProcessing {
+public:
+    cloudProcessing(srl_ctx* ctx, int lidar_type, int N_SCANS, int SCAN_RATE, int time_unit, double blind, int point_filter_num,
+                    size_t initial_capacity = size_t(1) << 18)
+        : ctx_(ctx) {
+        const srl_lidar_params p{lidar_type, N_SCANS, SCAN_RATE, time_unit, blind, point_filter_num, 0};
+        check(srl_lidar_create(ctx, &p, initial_capacity, &l_), "srl_lidar_create");
+        lidar_type_ = lidar_type;
+    }
+    ~cloudProcessing() { if (l_) srl_lidar_destroy(l_); }
+    cloudProcessing(const cloudProcessing&) = delete;
+    cloudProcessing& operator=(const cloudProcessing&) = delete;
+
+    // livoxHandler(msg, point_buffer): msg->points as n records `stride` bytes apart (19: the packed ROS layout); returns the
+    // points appended
+    int64_t livoxHandler(const uint8_t* records, size_t n, double stamp, size_t stride = 19) {
+        int64_t k = 0;
+        check(srl_lidar_livox(l_, records, n, stride, stamp, &k), "srl_lidar_livox");
+        return k;
+    }
+    // process(msg, point_buffer): msg->data of n = width * height points
+    int64_t process(const uint8_t* data, size_t n, const srl_cloud2_layout& layout, double stamp) {
+        int64_t k = 0;
+        check(srl_lidar_process(l_, data, n, &layout, stamp, &k), "srl_lidar_process");
+        return k;
+    }
+    int getLidarType() const { return lidar_type_; }
+    double getSweepInterval() { return info().sweep_interval; }
+    bool isPointTimeEnable() { return info().given_offset_time != 0; }
+
+    // getMeasurements' pops: while the queue is not empty and front().timestamp < t; returns the count, *raw_xyz / *timestamp
+    // point at the popped points on the device (either may be null)
+    int64_t cut(double t, const double** raw_xyz = nullptr, const double** timestamp = nullptr) {
+        int64_t k = 0;
+        check(srl_lidar_cut(l_, t, &k, raw_xyz, timestamp), "srl_lidar_cut");
+        return k;
+    }
+    // what the branches of getMeasurements read of point_buffer (host copies, no device access)
+    size_t size() { return (size_t)info().size; }
+    bool empty() { return size() == 0; }
+    double frontTimestamp() { return info().front_timestamp; }
+    double backTimestamp() { return info().back_timestamp; }
+    // host copies of the whole queue, front first
+    void download(std::vector<double>& raw_xyz, std::vector<double>& relative_time, std::vector<double>& timestamp) {
+        const size_t n = size();
+        raw_xyz.resize(3 * n);
+        relative_time.resize(n);
+        timestamp.resize(n);
+        check(srl_lidar_download(l_, raw_xyz.data(), relative_time.data(), timestamp.data()), "srl_lidar_download");
+    }
+    srl_lidar_info info() {
+        srl_lidar_info i{};
+        check(srl_lidar_info_get(l_, &i), "srl_lidar_info_get");
+        return i;
+    }
+
+private:
+    srl_ctx* ctx_ = nullptr;
+    srl_lidar* l_ = nullptr;
+    int lidar_type_ = 0;
+    void check(int rc, const char* what) {
+        if (rc != SRL_OK) throw std::runtime_error(std::string(what) + ": " + (ctx_ ? srl_last_error(ctx_) : "no context"));
+    }
+};
+
 }  // namespace srl

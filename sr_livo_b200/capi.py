@@ -126,6 +126,23 @@ class CloudFramePtrs(C.Structure):
                 ("alpha_time", C.c_void_p), ("timestamp", C.c_void_p), ("source_index", C.c_void_p)]
 
 
+class LidarParams(C.Structure):
+    """srl_lidar_params: cloudProcessing's configuration (lidar_parameter / common in the reference's yaml)."""
+    _fields_ = [("lidar_type", C.c_int32), ("n_scans", C.c_int32), ("scan_rate", C.c_int32), ("time_unit", C.c_int32),
+                ("blind", C.c_double), ("point_filter_num", C.c_int32), ("reserved", C.c_int32)]
+
+
+class Cloud2Layout(C.Structure):
+    _fields_ = [("point_step", C.c_uint32), ("off_x", C.c_int32), ("off_y", C.c_int32), ("off_z", C.c_int32),
+                ("off_time", C.c_int32), ("off_ring", C.c_int32), ("width", C.c_uint32), ("row_step", C.c_uint32)]
+
+
+class LidarInfo(C.Structure):
+    _fields_ = [("last_end_time", C.c_double), ("given_offset_time", C.c_int32), ("sweep_id", C.c_int32),
+                ("sweep_interval", C.c_double), ("size", C.c_int64), ("front_timestamp", C.c_double),
+                ("back_timestamp", C.c_double), ("capacity", C.c_int64)]
+
+
 class IekfIter(C.Structure):
     _fields_ = [("predict", EskfState), ("pass_index", C.c_int32), ("max_num_iter", C.c_int32)]
 
@@ -153,6 +170,8 @@ EXPORTS = [
     "srl_flow_tracker_create", "srl_flow_tracker_destroy", "srl_flow_tracker_init", "srl_flow_tracker_track_image",
     "srl_flow_tracker_reject_matches", "srl_flow_tracker_remove_outliers", "srl_flow_tracker_update_and_append", "srl_flow_tracker_sets",
     "srl_flow_tracker_outlier_counts",
+    "srl_lidar_create", "srl_lidar_destroy", "srl_lidar_livox", "srl_lidar_process", "srl_lidar_cut", "srl_lidar_info_get",
+    "srl_lidar_download", "srl_lidar_sort_replay",
 ]
 
 _lib = None
@@ -278,6 +297,15 @@ def lib():
     L.srl_flow_tracker_update_and_append.argtypes = [vp, C.POINTER(Camera), dbl, vp, sz]
     L.srl_flow_tracker_sets.argtypes = [vp, C.POINTER(FlowTrackerSets)]
     L.srl_flow_tracker_outlier_counts.argtypes = [vp, vp, sz, vp]
+    L.srl_lidar_create.argtypes = [vp, C.POINTER(LidarParams), sz, C.POINTER(vp)]
+    L.srl_lidar_destroy.argtypes = [vp]
+    L.srl_lidar_destroy.restype = None
+    L.srl_lidar_livox.argtypes = [vp, vp, sz, sz, dbl, C.POINTER(i64)]
+    L.srl_lidar_process.argtypes = [vp, vp, sz, C.POINTER(Cloud2Layout), dbl, C.POINTER(i64)]
+    L.srl_lidar_cut.argtypes = [vp, dbl, C.POINTER(i64), C.POINTER(vp), C.POINTER(vp)]
+    L.srl_lidar_info_get.argtypes = [vp, C.POINTER(LidarInfo)]
+    L.srl_lidar_download.argtypes = [vp, vp, vp, vp]
+    L.srl_lidar_sort_replay.argtypes = [vp, vp, sz, vp, C.POINTER(i32)]
     L.srl_cloud_frame_create.argtypes = [vp, sz, C.POINTER(vp)]
     L.srl_cloud_frame_destroy.argtypes = [vp]
     L.srl_cloud_frame_destroy.restype = None

@@ -15,6 +15,7 @@ Names and argument meaning follow the reference so the parity tests read like it
   LKOpticalFlowKernel::trackImage       src/lkpyramid.cpp:755           -> LKOpticalFlowKernel.trackImage
   imageProcessing::process (:91-125)    src/imageProcessing.cpp:91      -> ImageProcessing.process
   opticalFlowTracker                    src/opticalFlowTracker.cpp      -> OpticalFlowTracker
+  cloudProcessing + getMeasurements' pops src/cloudProcessing.cpp        -> CloudProcessing
 
 Error behaviour: optimizeSummary.success=false <-> OptimizeSummary.success False (SRL_TOO_FEW_RESIDUALS);
 the reference's `throw std::runtime_error("error")` on NaN planarity <-> RuntimeError; everything else raises
@@ -615,12 +616,16 @@ class LioOptimization:
                    q_pred=None, t_pred=None, point_time_enable: bool = True, motion_compensation: int = 1, init_num_frames: int = 20,
                    init_voxel_size: float = 0.2, voxel_size: float = 0.5, prev_time_sweep_end: float = 0.0,
                    frame: "CloudFrame | None" = None) -> CloudFrame:
-        """buildFrame over a cut sweep given as host arrays (raw_xyz n*3, timestamp n; capi.lib().srl_build_frame takes device
-        pointers too).  imu_states: a list of capi.ImuState.  motion_compensation: 0 IMU, 1 CONSTANT_VELOCITY.  Returns the
+        """buildFrame over a cut sweep: raw_xyz n*3 and timestamp n as host arrays, or torch tensors (host or CUDA, read in place;
+        CloudProcessing.cut(t, device=True) gives such views).  imu_states: a list of capi.ImuState.  motion_compensation: 0 IMU, 1 CONSTANT_VELOCITY.  Returns the
         device-resident frame (into `frame` when given), with the cloudFrame scalars in frame.info (capi.BuildFrameInfo)."""
-        raw = f64(raw_xyz).reshape(-1, 3)
-        ts = f64(timestamp).reshape(-1)
-        assert ts.shape[0] == raw.shape[0]
+        if _is_tensor(raw_xyz):   # e.g. CloudProcessing.cut(t, device=True): the device buffers are read in place
+            (p_raw, n), (p_ts, n_ts) = _addr(raw_xyz, np.float64, 3), _addr(timestamp, np.float64, 1)
+        else:
+            raw = f64(raw_xyz).reshape(-1, 3)
+            ts = f64(timestamp).reshape(-1)
+            (p_raw, n), (p_ts, n_ts) = (raw.ctypes.data, raw.shape[0]), (ts.ctypes.data, ts.shape[0])
+        assert n_ts == n
         states = (capi.ImuState * len(imu_states))(*imu_states)
         p = capi.BuildFrameParams()
         p.timestamp_begin, p.timestamp_offset = float(timestamp_begin), float(timestamp_offset)
@@ -631,9 +636,9 @@ class LioOptimization:
         for name, val in (("R_il", f64(self.R_imu_lidar).reshape(9)), ("t_il", f64(self.t_imu_lidar)),
                           ("q_pred", f64([0, 0, 0, 1] if q_pred is None else q_pred)), ("t_pred", f64(np.zeros(3) if t_pred is None else t_pred))):
             getattr(p, name)[:] = list(val)
-        frame = frame if frame is not None else CloudFrame(self.ctx, max(raw.shape[0], 1))
+        frame = frame if frame is not None else CloudFrame(self.ctx, max(n, 1))
         info = capi.BuildFrameInfo()
-        _check(self.ctx.h, lib().srl_build_frame(self.ctx.h, ptr(raw), ptr(ts), raw.shape[0], states, len(imu_states), C.byref(p),
+        _check(self.ctx.h, lib().srl_build_frame(self.ctx.h, C.c_void_p(p_raw), C.c_void_p(p_ts), n, states, len(imu_states), C.byref(p),
                                                  frame.h, C.byref(info)))
         frame.info = info
         return frame
@@ -1279,6 +1284,117 @@ class CameraState:
                            c.fx, c.fy, c.cx, c.cy, float(fov_margin), int(cols), int(rows))
 
 
+def r3live_lidar_params(**kw) -> dict:
+    """config/r3live.yaml: Livox, 6 lines, 10 Hz, ns, blind 0.1 m, point_filter_num 4"""
+    return dict(dict(lidar_type=1, n_scans=6, scan_rate=10, time_unit=3, blind=0.1, point_filter_num=4), **kw)
+
+
+def ntu_lidar_params(**kw) -> dict:
+    """config/ntu.yaml: Ouster, 16 rings, 20 Hz, ns, blind 4 m, point_filter_num 4"""
+    return dict(dict(lidar_type=3, n_scans=16, scan_rate=20, time_unit=3, blind=4.0, point_filter_num=4), **kw)
+
+
+class CloudProcessing:
+    """cloudProcessing (src/cloudProcessing.cpp, srl_lidar_*) with its point_buffer kept on the device.  Messages are byte buffers
+    as they come off the wire: numpy arrays (a structured array is taken as its bytes) or torch uint8 tensors, host or CUDA.
+
+    livoxHandler(records, stamp): CustomMsg points, `stride` bytes apart (19 for the packed ROS layout).
+    process(data, layout, stamp): PointCloud2 data; layout = dict(point_step, x, y, z, time, ring) byte offsets (msg->fields),
+    and for rows padded past width * point_step also width and row_step (msg->width, msg->row_step).
+    cut(t): getMeasurements' pops (front().timestamp < t) as (count, raw_xyz, timestamp) torch views of the queue's memory
+    (device=True, valid until the next handler call) or numpy copies; the views go to srl_build_frame as they are:
+        n, xyz, ts = cp.cut(t, device=True)
+        frame = lio_opt.buildFrame(xyz, ts, states, ..., point_time_enable=cp.isPointTimeEnable())"""
+
+    def __init__(self, ctx: Context, lidar_type: int, n_scans: int, scan_rate: int, time_unit: int, blind: float,
+                 point_filter_num: int, capacity: int = 1 << 18):
+        self.ctx = ctx
+        self.params = capi.LidarParams(int(lidar_type), int(n_scans), int(scan_rate), int(time_unit), float(blind),
+                                       int(point_filter_num), 0)
+        h = C.c_void_p()
+        _check(ctx.h, lib().srl_lidar_create(ctx.h, C.byref(self.params), int(capacity), C.byref(h)))
+        self.h = h
+
+    def close(self):
+        if getattr(self, "h", None):
+            lib().srl_lidar_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    @staticmethod
+    def _bytes(a):
+        if _is_tensor(a):
+            if not a.is_contiguous():
+                raise TypeError("expected a contiguous tensor")
+            return a.data_ptr(), a.numel() * a.element_size()
+        a = np.ascontiguousarray(a)
+        return a.ctypes.data, a.nbytes
+
+    def livoxHandler(self, records, stamp: float, stride: int = 19) -> int:
+        p, nbytes = self._bytes(records)
+        n = C.c_int64(0)
+        _check(self.ctx.h, lib().srl_lidar_livox(self.h, C.c_void_p(p), nbytes // stride, stride, float(stamp), C.byref(n)))
+        return n.value
+
+    def process(self, data, layout: dict, stamp: float) -> int:
+        p, nbytes = self._bytes(data)
+        y = capi.Cloud2Layout(int(layout["point_step"]), int(layout["x"]), int(layout["y"]), int(layout["z"]), int(layout["time"]),
+                              int(layout.get("ring", -1)), int(layout.get("width", 0)), int(layout.get("row_step", 0)))
+        n_pts = (nbytes // y.row_step) * y.width if y.row_step else nbytes // y.point_step
+        n = C.c_int64(0)
+        _check(self.ctx.h, lib().srl_lidar_process(self.h, C.c_void_p(p), n_pts, C.byref(y), float(stamp), C.byref(n)))
+        return n.value
+
+    def cut(self, t: float, device: bool = False):
+        n, xyz, ts = C.c_int64(0), C.c_void_p(), C.c_void_p()
+        _check(self.ctx.h, lib().srl_lidar_cut(self.h, float(t), C.byref(n), C.byref(xyz), C.byref(ts)))
+        k = n.value
+        import torch
+        dev = torch.device("cuda", self.ctx.device)
+        xyz_t = torch.as_tensor(_DeviceArray(xyz.value or 0, (k, 3), "<f8"), device=dev)
+        ts_t = torch.as_tensor(_DeviceArray(ts.value or 0, (k,), "<f8"), device=dev)
+        if device:
+            return k, xyz_t, ts_t
+        return k, xyz_t.cpu().numpy(), ts_t.cpu().numpy()
+
+    def info(self) -> "capi.LidarInfo":
+        i = capi.LidarInfo()
+        _check(self.ctx.h, lib().srl_lidar_info_get(self.h, C.byref(i)))
+        return i
+
+    def isPointTimeEnable(self) -> bool:
+        return bool(self.info().given_offset_time)
+
+    def getSweepInterval(self) -> float:
+        return self.info().sweep_interval
+
+    def queue(self):
+        """the whole point_buffer, front first: (raw_xyz n x 3, relative_time, timestamp) numpy copies"""
+        n = self.info().size
+        xyz, rel, ts = np.empty((n, 3)), np.empty(n), np.empty(n)
+        _check(self.ctx.h, lib().srl_lidar_download(self.h, ptr(xyz), ptr(rel), ptr(ts)))
+        return xyz, rel, ts
+
+
+def device_sort_permutation(ctx: Context, keys, return_heapsorts: bool = False):
+    """The device std::sort's permutation of float64 keys (host or CUDA): perm[p] = the index of the key that ends at p."""
+    if _is_tensor(keys):
+        p, n = keys.data_ptr(), keys.numel()
+    else:
+        keys = f64(keys).reshape(-1)
+        p, n = keys.ctypes.data, keys.size
+    perm = np.empty(n, np.int32)
+    h = C.c_int32(0)
+    _check(ctx.h, lib().srl_lidar_sort_replay(ctx.h, C.c_void_p(p), n, ptr(perm), C.byref(h)))
+    return (perm, h.value) if return_heapsorts else perm
+
+
 __all__ = ["Context", "VoxelHashMap", "ColorVoxelMap", "Sweep", "EskfEstimator", "LioOptimization", "OptimizeSummary", "PlaneResiduals",
            "IcpParams", "r3live_params", "r3live_map_options", "r3live_compressed_map_options", "make_frame", "SrlError", "write_pcd_xyzrgb",
-           "LKOpticalFlowKernel", "tracker_lk_params", "OpticalFlowTracker", "ImageProcessing", "CameraState", "r3live_camera_params", "ntu_camera_params"]
+           "LKOpticalFlowKernel", "tracker_lk_params", "OpticalFlowTracker", "ImageProcessing", "CameraState", "r3live_camera_params", "ntu_camera_params",
+           "CloudProcessing", "r3live_lidar_params", "ntu_lidar_params", "device_sort_permutation"]
