@@ -315,10 +315,6 @@ def lib():
     L.srl_cloud_frame_download.argtypes = [vp] + [vp] * 7
     L.srl_build_frame.argtypes = [vp, vp, vp, sz, vp, sz, C.POINTER(BuildFrameParams), vp, C.POINTER(BuildFrameInfo)]
     L.srl_shuffle_replay.argtypes = [vp, vp, sz, sz, i32, vp, C.POINTER(sz), C.POINTER(C.c_uint64)]
-    for name in EXPORTS:
-        fn = getattr(L, name)
-        if fn.restype is C.c_int and name not in ("srl_abi_version",):
-            fn.restype = C.c_int
     _lib = L
     return L
 

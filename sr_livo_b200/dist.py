@@ -12,6 +12,7 @@ import numpy as np
 
 from . import capi
 from .capi import IcpParams, IekfIter, NormalEq, SrlError, lib, ptr
+from .lio import _check
 
 
 def shard_range(n: int, rank: int, world: int) -> tuple[int, int]:
@@ -39,9 +40,7 @@ def allreduce_block(block, group=None):
 def unpack_block(block64: np.ndarray) -> NormalEq:
     ne = NormalEq()
     b = np.ascontiguousarray(block64, np.float64)
-    rc = lib().srl_normal_eq_unpack(ptr(b), C.byref(ne))
-    if rc != capi.SRL_OK:
-        raise SrlError(rc, "srl_normal_eq_unpack")
+    _check(None, lib().srl_normal_eq_unpack(ptr(b), C.byref(ne)), what="srl_normal_eq_unpack")
     return ne
 
 
@@ -50,9 +49,7 @@ def iekf_loop(pass_fn, eskf_c, frame_q: np.ndarray, frame_t: np.ndarray, prm: Ic
     pass_fn(frame_q, frame_t) -> torch tensor of 32 doubles holding THIS rank's partial sums
     (device tensor filled asynchronously is fine).  Returns dict(success, passes, converged, trace)."""
     it = IekfIter()
-    rc = lib().srl_iekf_begin(C.byref(eskf_c), C.byref(prm), C.byref(it))
-    if rc != capi.SRL_OK:
-        raise SrlError(rc, "srl_iekf_begin")
+    _check(None, lib().srl_iekf_begin(C.byref(eskf_c), C.byref(prm), C.byref(it)), what="srl_iekf_begin")
     passes = 0
     trace = []
     success = True
@@ -73,10 +70,8 @@ def iekf_loop(pass_fn, eskf_c, frame_q: np.ndarray, frame_t: np.ndarray, prm: Ic
         d_x = np.zeros(17)
         done = C.c_int32(0)
         div = C.c_int32(0)
-        rc = lib().srl_iekf_step(C.byref(it), C.byref(ne), C.byref(prm), C.byref(eskf_c), ptr(frame_q), ptr(frame_t),
-                                 ptr(d_x), C.byref(done), C.byref(div))
-        if rc != capi.SRL_OK:
-            raise SrlError(rc, "srl_iekf_step")
+        _check(None, lib().srl_iekf_step(C.byref(it), C.byref(ne), C.byref(prm), C.byref(eskf_c), ptr(frame_q), ptr(frame_t),
+                                         ptr(d_x), C.byref(done), C.byref(div)), what="srl_iekf_step")
         if len(trace) < max_trace:
             trace.append(np.concatenate([d_x, frame_t, frame_q]))
         if done.value:
@@ -102,19 +97,13 @@ class DistributedLio:
         if native and world > 1:
             import torch.distributed as tdist
             h = C.c_void_p()
-            rc = lib().srl_comm_create(lio_opt.ctx.h, rank, world, C.byref(h))
-            if rc != capi.SRL_OK:
-                raise SrlError(rc, "srl_comm_create")
+            _check(None, lib().srl_comm_create(lio_opt.ctx.h, rank, world, C.byref(h)), what="srl_comm_create")
             mine = np.zeros(64, np.uint8)
-            rc = lib().srl_comm_export(h, ptr(mine))
-            if rc != capi.SRL_OK:
-                raise SrlError(rc, lib().srl_last_error(lio_opt.ctx.h).decode())
+            _check(lio_opt.ctx.h, lib().srl_comm_export(h, ptr(mine)))
             gathered = [None] * world
             tdist.all_gather_object(gathered, mine.tobytes(), group=group)
             allh = np.frombuffer(b"".join(gathered), np.uint8).copy()
-            rc = lib().srl_comm_connect(h, ptr(allh))
-            if rc != capi.SRL_OK:
-                raise SrlError(rc, lib().srl_last_error(lio_opt.ctx.h).decode())
+            _check(lio_opt.ctx.h, lib().srl_comm_connect(h, ptr(allh)))
             tdist.barrier(group=group)
             self.comm = h
             # every rank must run the same form of the loop (the device-resident and the host-driven form agree to rounding,
@@ -170,10 +159,8 @@ class DistributedLio:
 
         def fn(frame_q, frame_t):
             fr = make_frame(frame_q, frame_t, t_last, self.L.R_imu_lidar, self.L.t_imu_lidar)
-            rc = lib().srl_build_plane_residuals_async(self.L.ctx.h, self.L.voxel_map.h, self.L.sweep.h, C.byref(fr),
-                                                       C.byref(prm), C.c_void_p(self.block.data_ptr()))
-            if rc != capi.SRL_OK:
-                raise SrlError(rc, lib().srl_last_error(self.L.ctx.h).decode())
+            _check(self.L.ctx.h, lib().srl_build_plane_residuals_async(self.L.ctx.h, self.L.voxel_map.h, self.L.sweep.h, C.byref(fr),
+                                                                       C.byref(prm), C.c_void_p(self.block.data_ptr())))
             # the pass ran on the ctx stream, the all-reduce and the D2H read run on torch's current stream: order them
             self.L.ctx.synchronize()
             return self.block

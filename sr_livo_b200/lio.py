@@ -24,7 +24,9 @@ SrlError.  No CPU fallback exists: without the CUDA library/GPU every call fails
 from __future__ import annotations
 
 import ctypes as C
+import math
 from dataclasses import dataclass, field
+from types import SimpleNamespace
 
 import numpy as np
 
@@ -35,33 +37,86 @@ from .capi import (DebugOut, EskfState, Frame, IcpParams, IekfSummary, NormalEq,
 NS = capi.NS
 
 
-def _check(ctx, rc, ok=(capi.SRL_OK,)):
+def _check(ctx, rc, ok=(capi.SRL_OK,), what=""):
+    """Raise SrlError unless rc is in `ok`, with ctx's last error message (or `what` for a call that takes no ctx)."""
     if rc not in ok:
-        raise SrlError(rc, lib().srl_last_error(ctx).decode() if ctx else "")
+        raise SrlError(rc, lib().srl_last_error(ctx).decode() if ctx else what)
     return rc
 
 
-def _is_tensor(a) -> bool:
-    return type(a).__module__.split(".")[0] == "torch"
+def _buffer(a, dtype, width=1, *, convert=False, image=False):
+    """The one rule by which a caller's buffer reaches the C ABI, which tells host from device memory per pointer.
 
+    `a` is a numpy array or a torch tensor on the host or a CUDA device.  A tensor must have exactly `dtype` (an int32 tensor
+    also stands for uint32 point ids: torch has no uint32 arithmetic) and is never copied.  A numpy array must have exactly
+    `dtype`, unless convert=True: then any array-like is copied as C-contiguous `dtype` when it is not so already, and must
+    hold whole rows.  dtype None takes any dtype and counts bytes.
 
-def _addr(a, dtype, width):
-    """(address, rows) of a C-contiguous buffer of `width` elements of `dtype` per row: a numpy array (host) or a torch tensor
-    (host or CUDA; the C ABI tells host from device per pointer)."""
-    if _is_tensor(a):
-        if str(a.dtype) != "torch." + np.dtype(dtype).name or not a.is_contiguous():
-            raise TypeError(f"expected a contiguous torch.{np.dtype(dtype).name} tensor")
-        return a.data_ptr(), a.numel() // width
-    if not (isinstance(a, np.ndarray) and a.dtype == dtype and a.flags.c_contiguous):
-        raise TypeError(f"expected a C-contiguous {np.dtype(dtype).name} array")
-    return a.ctypes.data, a.size // width
+    A row buffer is C-contiguous with `width` values per row: returns (a, address, rows).  An image (image=True) is
+    (rows, cols), or (rows, cols, width) for width > 1, with contiguous pixels and a row pitch of at least one row of
+    pixels, padding allowed: returns (a, address, rows, cols, pitch in bytes).  `a` is the converted copy when one was made,
+    which the caller keeps alive across the C call."""
+    name = "any" if dtype is None else np.dtype(dtype).name
+    if type(a).__module__.split(".")[0] == "torch":
+        got = str(a.dtype).replace("torch.", "")
+        if dtype is not None and got != name and (name, got) != ("uint32", "int32"):
+            raise TypeError(f"expected a torch.{name} tensor, got torch.{got}")
+        p, shape, strides, item, contiguous = a.data_ptr(), tuple(a.shape), a.stride(), a.element_size(), a.is_contiguous()
+    else:
+        if convert:
+            a = np.ascontiguousarray(a, dtype)
+            if a.size % width:
+                raise ValueError(f"expected whole rows of {width} values, got {a.size}")
+        if not isinstance(a, np.ndarray) or (dtype is not None and a.dtype != dtype):
+            raise TypeError(f"expected a numpy {name} array or a torch tensor, got {type(a).__name__} {getattr(a, 'dtype', '')}")
+        p, shape, item, contiguous = a.ctypes.data, a.shape, a.itemsize, a.flags.c_contiguous
+        strides = tuple(s // item for s in a.strides)
+    if image:
+        pixel = (width,) if width > 1 else ()
+        if (len(shape) != 2 + len(pixel) or tuple(shape[2:]) != pixel or tuple(strides[1:]) != pixel[::-1] + (1,)
+                or strides[0] < shape[1] * width):
+            raise TypeError(f"expected a (rows, cols{', %d' % width if pixel else ''}) image with contiguous pixels and rows at "
+                            f"least cols pixels apart in address order, got shape {tuple(shape)} and strides {tuple(strides)}")
+        return a, p, shape[0], shape[1], strides[0] * item
+    if not contiguous:
+        raise TypeError("expected a C-contiguous buffer")
+    return a, p, math.prod(shape) * item // (width * (1 if dtype is None else item))
 
 
 def _empty_like_input(a, rows, width, dtype):
-    if _is_tensor(a):
-        import torch
-        return torch.empty((rows, width), dtype=getattr(torch, np.dtype(dtype).name), device=a.device)
-    return np.empty((rows, width), dtype)
+    if isinstance(a, np.ndarray):
+        return np.empty((rows, width), dtype)
+    import torch
+    return torch.empty((rows, width), dtype=getattr(torch, np.dtype(dtype).name), device=a.device)
+
+
+def _device_view(ctx, p, rows, width, dtype):
+    """A torch view of `rows` x `width` values of `dtype` at address p of ctx's device (memory the library owns): no copy."""
+    import torch
+    shape = (rows,) if width == 1 else (rows, width)
+    dev = torch.device("cuda", ctx.device)
+    if rows == 0:
+        return torch.empty(shape, dtype=getattr(torch, np.dtype(dtype).name), device=dev)
+    view = dict(shape=shape, typestr=np.dtype(dtype).str, data=(p, False), version=3, strides=None)
+    return torch.as_tensor(SimpleNamespace(__cuda_array_interface__=view), device=dev)
+
+
+class _Handle:
+    """Owns the C handle `h`.  close() releases it once with the `_destroy` call, and does nothing on an object whose
+    constructor failed before it had one; __del__ closes and swallows errors."""
+    _destroy = ""
+    h = None
+
+    def close(self):
+        if self.h:
+            getattr(lib(), self._destroy)(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 def write_pcd_xyzrgb(path: str, xyz, rgb) -> None:
@@ -83,8 +138,10 @@ def write_pcd_xyzrgb(path: str, xyz, rgb) -> None:
         f.write(rec.tobytes())
 
 
-class Context:
+class Context(_Handle):
     """srl_ctx: one per host thread / GPU. `stream` may be a raw cudaStream_t (e.g. torch's current stream)."""
+
+    _destroy = "srl_ctx_destroy"
 
     def __init__(self, device: int = 0, stream: int | None = None):
         h = C.c_void_p()
@@ -93,17 +150,6 @@ class Context:
             raise SrlError(rc, "srl_ctx_create failed: no usable CUDA device (this path has no CPU fallback)")
         self.h = h
         self.device = device
-
-    def close(self):
-        if getattr(self, "h", None):
-            lib().srl_ctx_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     def synchronize(self):
         _check(self.h, lib().srl_ctx_synchronize(self.h))
@@ -130,11 +176,13 @@ class Context:
         return ms.value, n.value
 
 
-class VoxelHashMap:
+class VoxelHashMap(_Handle):
     """HBM-resident voxelHashMap (include/cloudMap.h:171).
 
     max_voxels is the limit (SRL_MAP_FULL past it); initial_voxels (None = max_voxels) is what is committed at creation,
     and the map grows from there on demand, doubling, up to max_voxels."""
+
+    _destroy = "srl_map_destroy"
 
     def __init__(self, ctx: Context, voxel_size: float = 1.0, max_num_points_in_voxel: int = 20,
                  max_voxels: int = 1 << 20, initial_voxels: int | None = None):
@@ -151,17 +199,6 @@ class VoxelHashMap:
         v = [C.c_size_t(0) for _ in range(3)]
         _check(self.ctx.h, lib().srl_map_capacity(self.h, *[C.byref(x) for x in v]))
         return dict(zip(("committed_voxels", "slot_capacity", "committed_bytes"), [x.value for x in v]))
-
-    def close(self):
-        if getattr(self, "h", None):
-            lib().srl_map_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     def clear(self):
         _check(self.ctx.h, lib().srl_map_clear(self.h))
@@ -210,11 +247,9 @@ class VoxelHashMap:
         """insert + the cloud addPointsToMap publishes (srl_map_insert_published): (points stored, xyzi) with xyzi the first
         n_published rows of `out` (n x 4 float32: x, y, z, intensity, sweep order).  xyz_world is an (n, 3) float64 numpy array
         or torch tensor (host or CUDA); out, when not given, is allocated like the input."""
-        if not _is_tensor(xyz_world):
-            xyz_world = f64(xyz_world).reshape(-1, 3)
-        p_in, n = _addr(xyz_world, np.float64, 3)
+        xyz_world, p_in, n = _buffer(xyz_world, np.float64, 3, convert=True)
         out = _empty_like_input(xyz_world, n, 4, np.float32) if out is None else out
-        p_out, max_out = _addr(out, np.float32, 4)
+        _, p_out, max_out = _buffer(out, np.float32, 4)
         added, n_pub = C.c_int64(0), C.c_int64(0)
         _check(self.ctx.h, lib().srl_map_insert_published(self.h, C.c_void_p(p_in), n, min_distance_points, min_num_points, float(translation_z),
                                                           C.c_void_p(p_out), max_out, C.byref(added), C.byref(n_pub)))
@@ -231,7 +266,7 @@ def r3live_compressed_map_options() -> dict:
     return dict(size_voxel_map=0.1, max_num_points_in_voxel=100, min_distance_points=0.01, add_point_step=1, pub_point_minimum_views=3)
 
 
-class ColorVoxelMap:
+class ColorVoxelMap(_Handle):
     """color_voxel_map + hashmap_3d_points + rgb_points_vec + voxels_recent_visited (include/lioOptimization.h:275-291,
     include/rgbMapTracker.h:38), fed by the colour branch of addPointsToMap and coloured by renderPointsInRecentVoxel.
 
@@ -241,6 +276,8 @@ class ColorVoxelMap:
     there on demand, so a long run needs no guess of its size: initial_voxels=4096, max_voxels=1 << 20.
     The yaml values: ColorVoxelMap(ctx, o["size_voxel_map"], o["max_num_points_in_voxel"], max_voxels, o["min_distance_points"])
     with o = r3live_map_options(), and addPoints(..., add_point_step=o["add_point_step"])."""
+
+    _destroy = "srl_color_map_destroy"
 
     def __init__(self, ctx: Context, voxel_size: float = 1.0, max_num_points_in_voxel: int = 20, max_voxels: int = 1 << 16,
                  min_distance_points: float = 0.15, initial_voxels: int | None = None):
@@ -257,17 +294,6 @@ class ColorVoxelMap:
         _check(self.ctx.h, lib().srl_color_map_capacity(self.h, *[C.byref(x) for x in v]))
         return dict(zip(("committed_voxels", "fine_capacity", "committed_rgb_points", "committed_bytes"), [x.value for x in v]))
 
-    def close(self):
-        if getattr(self, "h", None):
-            lib().srl_color_map_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
     def stats(self) -> dict:
         v = [C.c_int64(0) for _ in range(5)]
         _check(self.ctx.h, lib().srl_color_map_stats(self.h, *[C.byref(x) for x in v]))
@@ -277,9 +303,7 @@ class ColorVoxelMap:
                   to_rendering: bool = True) -> int:
         """the loop of src/lioOptimization.cpp:533-551 over the registered frame: an (n, 3) float64 numpy array or torch tensor
         (host or CUDA).  Returns the number of points stored."""
-        if not _is_tensor(xyz_world):
-            xyz_world = f64(xyz_world).reshape(-1, 3)
-        p, n = _addr(xyz_world, np.float64, 3)
+        xyz_world, p, n = _buffer(xyz_world, np.float64, 3, convert=True)
         stored = C.c_int64(0)
         _check(self.ctx.h, lib().srl_color_map_add_points(self.h, C.c_void_p(p), n, add_point_step, time_sweep_end, time_last_process,
                                                           1 if to_rendering else 0, C.byref(stored)))
@@ -291,13 +315,9 @@ class ColorVoxelMap:
         render_point_count.  camera.fov_margin must be >= 0 (SRL_BAD_ARG otherwise, NaN included, and the map is untouched):
         a negative margin would sample outside the image, which the reference leaves undefined.  The selection
         (selectPointsForProjection) still takes negative margins."""
-        if _is_tensor(image_bgr):
-            assert tuple(image_bgr.shape) == (camera.rows, camera.cols, 3)
-            p_img, _ = _addr(image_bgr, np.uint8, 3)
-        else:
-            img = np.ascontiguousarray(image_bgr, np.uint8)
-            assert img.shape == (camera.rows, camera.cols, 3)
-            p_img = img.ctypes.data
+        if tuple(np.shape(image_bgr)) != (camera.rows, camera.cols, 3):
+            raise ValueError(f"expected a ({camera.rows}, {camera.cols}, 3) image, got {tuple(np.shape(image_bgr))}")
+        image_bgr, p_img, _ = _buffer(image_bgr, np.uint8, 3, convert=True)
         n = C.c_int64(0)
         _check(self.ctx.h, lib().srl_color_map_render_recent(self.h, C.byref(camera), C.c_void_p(p_img), float(obs_time), C.byref(n)))
         return n.value
@@ -312,8 +332,8 @@ class ColorVoxelMap:
         if xyz is None:
             _check(self.ctx.h, lib().srl_color_map_export(self.h, int(min_views), int(order), None, None, 0, C.byref(n)))
             xyz, rgb = np.empty((n.value, 3), np.float32), np.empty((n.value, 3), np.uint8)
-        p_xyz, cap = _addr(xyz, np.float32, 3)
-        p_rgb, cap_rgb = _addr(rgb, np.uint8, 3)
+        _, p_xyz, cap = _buffer(xyz, np.float32, 3)
+        _, p_rgb, cap_rgb = _buffer(rgb, np.uint8, 3)
         _check(self.ctx.h, lib().srl_color_map_export(self.h, int(min_views), int(order), C.c_void_p(p_xyz), C.c_void_p(p_rgb),
                                                       min(cap, cap_rgb), C.byref(n)))
         return xyz[:n.value], rgb[:n.value]
@@ -358,10 +378,7 @@ class ColorVoxelMap:
             if a is None:
                 addrs.append(None)
                 continue
-            if _is_tensor(a) and str(a.dtype) == "torch.int32" and dt == np.uint32:
-                p, rows = a.data_ptr(), a.numel()          # torch has no uint32 of its own: int32 holds the ids' bits
-            else:
-                p, rows = _addr(a, dt, w)
+            _, p, rows = _buffer(a, dt, w)
             addrs.append(C.c_void_p(p))
             caps.append(rows)
         _check(self.ctx.h, lib().srl_color_map_select_for_projection(self.h, C.byref(camera), C.byref(prm), addrs[0], addrs[1], addrs[2],
@@ -381,13 +398,7 @@ class ColorVoxelMap:
         """srl_color_map_gather_points: the state of each point id as numpy arrays — xyz (n, 3) float32, rgb (n, 3) int16 (the BGR
         state), n_rgb (n,) int16, cov (n, 3) float32, key_index (n, 4) int16 (voxel key, index in block).  ids: a uint32 numpy array
         or a torch tensor (host or CUDA; int32 holds the ids' bits).  An id that names no stored point raises SrlError."""
-        if _is_tensor(ids):
-            p, n = ids.data_ptr(), ids.numel()
-            if ids.element_size() != 4 or not ids.is_contiguous():
-                raise TypeError("expected a contiguous 32-bit tensor of point ids")
-        else:
-            ids = np.ascontiguousarray(ids, np.uint32).reshape(-1)
-            p, n = ids.ctypes.data, ids.size
+        ids, p, n = _buffer(ids, np.uint32, convert=True)
         out = dict(xyz=np.empty((n, 3), np.float32), rgb=np.empty((n, 3), np.int16), n_rgb=np.empty(n, np.int16),
                    cov=np.empty((n, 3), np.float32), key_index=np.empty((n, 4), np.int16))
         _check(self.ctx.h, lib().srl_color_map_gather_points(self.h, C.c_void_p(p), n, *[ptr(out[k]) for k in ("xyz", "rgb", "n_rgb", "cov",
@@ -411,8 +422,10 @@ class ColorVoxelMap:
         return out
 
 
-class Sweep:
+class Sweep(_Handle):
     """The keypoints of one reconstructed sweep, resident in HBM (raw LiDAR-frame points, FP64)."""
+
+    _destroy = "srl_sweep_destroy"
 
     def __init__(self, ctx: Context, capacity: int):
         self.ctx = ctx
@@ -421,17 +434,6 @@ class Sweep:
         h = C.c_void_p()
         _check(ctx.h, lib().srl_sweep_create(ctx.h, capacity, C.byref(h)))
         self.h = h
-
-    def close(self):
-        if getattr(self, "h", None):
-            lib().srl_sweep_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     def upload(self, raw_xyz):
         raw = f64(raw_xyz).reshape(-1, 3)
@@ -454,9 +456,10 @@ class Sweep:
         return out
 
 
-class CloudFrame:
+class CloudFrame(_Handle):
     """The frame buildFrame hands to stateEstimation, resident in HBM (srl_cloud_frame), final frame order."""
 
+    _destroy = "srl_cloud_frame_destroy"
     FIELDS = (("raw_point", 3, np.float64), ("point", 3, np.float64), ("imu_point", 3, np.float64), ("relative_time", 1, np.float64),
               ("alpha_time", 1, np.float64), ("timestamp", 1, np.float64), ("source_index", 1, np.int32))
 
@@ -466,17 +469,6 @@ class CloudFrame:
         h = C.c_void_p()
         _check(ctx.h, lib().srl_cloud_frame_create(ctx.h, capacity, C.byref(h)))
         self.h = h
-
-    def close(self):
-        if getattr(self, "h", None):
-            lib().srl_cloud_frame_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     def __len__(self) -> int:
         return int(lib().srl_cloud_frame_size(self.h))
@@ -516,9 +508,7 @@ class EskfEstimator:
         """eskfEstimator::observe (src/eskfEstimator.cpp:219-230)."""
         s = self.to_c()
         d = f64(d_x)
-        rc = lib().srl_eskf_observe(C.byref(s), ptr(d))
-        if rc != capi.SRL_OK:
-            raise SrlError(rc, "srl_eskf_observe")
+        _check(None, lib().srl_eskf_observe(C.byref(s), ptr(d)), what="srl_eskf_observe")
         return EskfEstimator.from_c(s)
 
 
@@ -604,7 +594,7 @@ class LioOptimization:
         q, t = f64(frame_q), f64(frame_t)
         R, ti = f64(self.R_imu_lidar).reshape(9), f64(self.t_imu_lidar)
         out = np.empty((self.sweep.n, 4), np.float32) if out is None else out
-        p_out, max_out = _addr(out, np.float32, 4)
+        _, p_out, max_out = _buffer(out, np.float32, 4)
         added, n_pub = C.c_int64(0), C.c_int64(0)
         _check(self.ctx.h, lib().srl_map_insert_sweep_published(self.voxel_map.h, self.sweep.h, ptr(q), ptr(t), ptr(R), ptr(ti),
                                                                 min_distance_points, min_num_points, C.c_void_p(p_out), max_out,
@@ -619,13 +609,10 @@ class LioOptimization:
         """buildFrame over a cut sweep: raw_xyz n*3 and timestamp n as host arrays, or torch tensors (host or CUDA, read in place;
         CloudProcessing.cut(t, device=True) gives such views).  imu_states: a list of capi.ImuState.  motion_compensation: 0 IMU, 1 CONSTANT_VELOCITY.  Returns the
         device-resident frame (into `frame` when given), with the cloudFrame scalars in frame.info (capi.BuildFrameInfo)."""
-        if _is_tensor(raw_xyz):   # e.g. CloudProcessing.cut(t, device=True): the device buffers are read in place
-            (p_raw, n), (p_ts, n_ts) = _addr(raw_xyz, np.float64, 3), _addr(timestamp, np.float64, 1)
-        else:
-            raw = f64(raw_xyz).reshape(-1, 3)
-            ts = f64(timestamp).reshape(-1)
-            (p_raw, n), (p_ts, n_ts) = (raw.ctypes.data, raw.shape[0]), (ts.ctypes.data, ts.shape[0])
-        assert n_ts == n
+        raw_xyz, p_raw, n = _buffer(raw_xyz, np.float64, 3, convert=True)
+        timestamp, p_ts, n_ts = _buffer(timestamp, np.float64, convert=True)
+        if n_ts != n:
+            raise ValueError(f"raw_xyz holds {n} points and timestamp {n_ts}")
         states = (capi.ImuState * len(imu_states))(*imu_states)
         p = capi.BuildFrameParams()
         p.timestamp_begin, p.timestamp_offset = float(timestamp_begin), float(timestamp_offset)
@@ -802,10 +789,12 @@ def tracker_lk_params() -> dict:
     return dict(win_size=(21, 21), max_level=3, criteria=(COUNT | EPS, 10, 0.05), flags=8, min_eig_threshold=1e-4)
 
 
-class LKOpticalFlowKernel:
+class LKOpticalFlowKernel(_Handle):
     """LKOpticalFlowKernel (include/lkpyramid.h:65-131, srl_lk_*): the optical-flow tracker's pyramidal Lucas-Kanade on the GPU, bit
     for bit the reference.  criteria = (type, max_count, epsilon) as cv::TermCriteria; the defaults are the reference's own
     constructor defaults.  Each image's pyramid stays on the device as the previous image of the next call."""
+
+    _destroy = "srl_lk_destroy"
 
     def __init__(self, ctx: Context, win_size=(21, 21), max_level: int = 3, criteria=(COUNT | EPS, 30, 0.01), flags: int = 0,
                  min_eig_threshold: float = 1e-4):
@@ -817,40 +806,22 @@ class LKOpticalFlowKernel:
         _check(ctx.h, lib().srl_lk_create(ctx.h, C.byref(self.params), C.byref(h)))
         self.h = h
 
-    def close(self):
-        if getattr(self, "h", None):
-            lib().srl_lk_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
     def trackImage(self, gray, last_pts, out=None):
         """trackImage (src/lkpyramid.cpp:755-795): (curr_pts (n, 2) float32, status (n,) uint8, n_tracked).  gray: (rows, cols) uint8
         with unit column stride (a numpy array or a torch tensor, host or CUDA; rows may be padded); last_pts: (n, 2) float32 (the
         selection's uv as it comes).  out = (curr_pts, status) buffers receive the result; without it they are made on last_pts'
         side (numpy, or a torch tensor on its device), status filled with ones.  The first image only builds its pyramid:
         curr_pts = last_pts, status as it was, n_tracked 0."""
-        if _is_tensor(gray):
-            if str(gray.dtype) != "torch.uint8" or gray.dim() != 2 or gray.stride(1) != 1:
-                raise TypeError("expected a 2-D torch.uint8 image with unit column stride")
-            p_img, rows, cols, pitch = gray.data_ptr(), gray.shape[0], gray.shape[1], gray.stride(0)
-        else:
-            if not (isinstance(gray, np.ndarray) and gray.dtype == np.uint8 and gray.ndim == 2 and gray.strides[1] == 1):
-                raise TypeError("expected a 2-D uint8 array with unit column stride")
-            p_img, rows, cols, pitch = gray.ctypes.data, gray.shape[0], gray.shape[1], gray.strides[0]
-        p_last, n = _addr(last_pts, np.float32, 2)
+        _, p_img, rows, cols, pitch = _buffer(gray, np.uint8, image=True)
+        _, p_last, n = _buffer(last_pts, np.float32, 2)
         if out is None:
             curr = _empty_like_input(last_pts, n, 2, np.float32)
             status = _empty_like_input(last_pts, n, 1, np.uint8).reshape(-1)
             status[:] = 1
         else:
             curr, status = out
-        p_curr, n_curr = _addr(curr, np.float32, 2)
-        p_st, n_st = _addr(status, np.uint8, 1)
+        _, p_curr, n_curr = _buffer(curr, np.float32, 2)
+        _, p_st, n_st = _buffer(status, np.uint8)
         if n_curr < n or n_st < n:
             raise ValueError("out buffers hold fewer points than last_pts")
         k = C.c_int64(0)
@@ -894,33 +865,14 @@ def ntu_camera_params() -> dict:
                 camera_dist_coeffs=[-0.2881, 0.0746, 7.7845e-04, -2.2779e-04, 0.0])
 
 
-def _image_2d(img, what):
-    """(address, rows, cols, row pitch in bytes) of a (rows, cols, 3) uint8 image with contiguous pixels; rows may be padded."""
-    if _is_tensor(img):
-        if str(img.dtype) != "torch.uint8" or img.dim() != 3 or img.shape[2] != 3 or img.stride(2) != 1 or img.stride(1) != 3:
-            raise TypeError(f"{what}: expected a (rows, cols, 3) torch.uint8 image with contiguous pixels")
-        return img.data_ptr(), img.shape[0], img.shape[1], img.stride(0)
-    if not (isinstance(img, np.ndarray) and img.dtype == np.uint8 and img.ndim == 3 and img.shape[2] == 3 and img.strides[2] == 1
-            and img.strides[1] == 3):
-        raise TypeError(f"{what}: expected a (rows, cols, 3) uint8 array with contiguous pixels")
-    return img.ctypes.data, img.shape[0], img.shape[1], img.strides[0]
-
-
-def _ids_addr(ids):
-    """(address, n) of point ids: a uint32 numpy array or a contiguous 32-bit torch tensor (int32 holds the ids' bits)."""
-    if _is_tensor(ids):
-        if ids.element_size() != 4 or not ids.is_contiguous() or ids.is_floating_point():
-            raise TypeError("expected a contiguous 32-bit integer tensor of point ids")
-        return ids.data_ptr(), ids.numel()
-    return _addr(ids, np.uint32, 1)
-
-
-class ImageProcessing:
+class ImageProcessing(_Handle):
     """The image preparation of imageProcessing::process (src/imageProcessing.cpp:91-125,166-200, srl_image_*) on the GPU, bit for
     bit OpenCV's: undistortion (initUndistortRectifyMap CV_16SC2 + remap INTER_LINEAR), COLOR_RGB2GRAY and CLAHE clip 3 for
     gray_image, BGR2YCrCb, CLAHE clip 1 on Y and YCrCb2BGR for rgb_image.  Construction is the first-image step for inputs of
     cols x rows (the yaml's size unless given): the scale factor, the scaled intrinsics (camera_intrinsic()) and the map.
     ImageProcessing(ctx, **r3live_camera_params())."""
+
+    _destroy = "srl_image_destroy"
 
     def __init__(self, ctx: Context, image_width: int, image_height: int, camera_intrinsic, camera_dist_coeffs, cols: int | None = None,
                  rows: int | None = None):
@@ -934,17 +886,6 @@ class ImageProcessing:
         h = C.c_void_p()
         _check(ctx.h, lib().srl_image_create(ctx.h, C.byref(self.params), self.input_size[0], self.input_size[1], C.byref(h)))
         self.h = h
-
-    def close(self):
-        if getattr(self, "h", None):
-            lib().srl_image_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     def _info(self):
         c, r, t, s, k = C.c_int32(0), C.c_int32(0), C.c_int32(0), C.c_double(0), np.zeros(9, np.float64)
@@ -971,14 +912,14 @@ class ImageProcessing:
         """process:120-125 for one (rows, cols, 3) BGR8 image (numpy or torch, host or CUDA; rows may be padded, as a ROS step is):
         (rgb_image (out_rows, out_cols, 3) BGR8, gray_image (out_rows, out_cols)).  out = (rgb, gray) buffers (contiguous, numpy or
         torch, host or CUDA) receive them; without it numpy arrays are returned."""
-        p_img, rows, cols, pitch = _image_2d(image_bgr, "image_bgr")
+        _, p_img, rows, cols, pitch = _buffer(image_bgr, np.uint8, 3, image=True)
         oc, orows = self.output_size()
         if out is None:
             rgb, gray = np.empty((orows, oc, 3), np.uint8), np.empty((orows, oc), np.uint8)
         else:
             rgb, gray = out
-        p_rgb, n_rgb = _addr(rgb, np.uint8, 3)
-        p_gray, n_gray = _addr(gray, np.uint8, 1)
+        _, p_rgb, n_rgb = _buffer(rgb, np.uint8, 3)
+        _, p_gray, n_gray = _buffer(gray, np.uint8)
         if n_rgb < oc * orows or n_gray < oc * orows:
             raise ValueError(f"out buffers must hold {orows} x {oc} pixels")
         _check(self.ctx.h, lib().srl_image_process(self.h, C.c_void_p(p_img), int(cols), int(rows), int(pitch), C.c_void_p(p_rgb),
@@ -1014,9 +955,9 @@ class ImageProcessing:
         as it is), velocity (n, 2) float64 image velocities; numpy arrays or torch tensors, host or CUDA.  n_new_visited is the
         colour map's stats()["recent"] after the rendering insert.  Updates `state` and the covariance in place; returns the reference's
         result."""
-        p_ids, n = _ids_addr(ids)
-        p_uv, n_uv = _addr(uv, np.float32, 2)
-        p_vel, n_vel = _addr(velocity, np.float64, 2)
+        _, p_ids, n = _buffer(ids, np.uint32)
+        _, p_uv, n_uv = _buffer(uv, np.float32, 2)
+        _, p_vel, n_vel = _buffer(velocity, np.float64, 2)
         if n_uv != n or n_vel != n:
             raise ValueError("ids, uv and velocity must hold the same number of points")
         r = C.c_int32(0)
@@ -1027,11 +968,11 @@ class ImageProcessing:
     def vioPhotometric(self, cmap: "ColorVoxelMap", state: "CameraState", ids, velocity, n_new_visited: int, rgb_image) -> bool:
         """imageProcessing::vioPhotometric (:402-552, srl_image_vio_photometric) on the prepared rgb_image ((out_rows, out_cols,
         3) BGR8, process()'s rgb output; numpy or torch, host or CUDA, rows may be padded); ids and velocity as for vioEsikf."""
-        p_ids, n = _ids_addr(ids)
-        p_vel, n_vel = _addr(velocity, np.float64, 2)
+        _, p_ids, n = _buffer(ids, np.uint32)
+        _, p_vel, n_vel = _buffer(velocity, np.float64, 2)
         if n_vel != n:
             raise ValueError("ids and velocity must hold the same number of points")
-        p_img, rows, cols, pitch = _image_2d(rgb_image, "rgb_image")
+        _, p_img, rows, cols, pitch = _buffer(rgb_image, np.uint8, 3, image=True)
         r = C.c_int32(0)
         _check(self.ctx.h, lib().srl_image_vio_photometric(self.h, cmap.h, C.byref(state.c), C.c_void_p(p_ids), C.c_void_p(p_vel), n,
                                                            int(n_new_visited), C.c_void_p(p_img), int(cols), int(rows), int(pitch),
@@ -1051,28 +992,10 @@ class ImageProcessing:
         return a.value, b.value
 
 
-def _gray_2d(gray):
-    """(address, rows, cols, row pitch in bytes) of a 2-D uint8 image with unit column stride; rows may be padded."""
-    if _is_tensor(gray):
-        if str(gray.dtype) != "torch.uint8" or gray.dim() != 2 or gray.stride(1) != 1:
-            raise TypeError("expected a 2-D torch.uint8 image with unit column stride")
-        return gray.data_ptr(), gray.shape[0], gray.shape[1], gray.stride(0)
-    if not (isinstance(gray, np.ndarray) and gray.dtype == np.uint8 and gray.ndim == 2 and gray.strides[1] == 1):
-        raise TypeError("expected a 2-D uint8 array with unit column stride")
-    return gray.ctypes.data, gray.shape[0], gray.shape[1], gray.strides[0]
-
-
-class _DeviceArray:
-    """A view of device memory for torch.as_tensor (the CUDA array interface): no copy."""
-
-    def __init__(self, p, shape, typestr):
-        self.__cuda_array_interface__ = dict(shape=shape, typestr=typestr, data=(p, False), version=3, strides=None)
-
-
 _NO_INLIERS = np.zeros(1, np.int32)
 
 
-class OpticalFlowTracker:
+class OpticalFlowTracker(_Handle):
     """opticalFlowTracker (src/opticalFlowTracker.cpp, srl_flow_tracker_*): the tracked point sets of the camera frame kept on the
     device from one image to the next, in colour-map point id order.  lk is the LKOpticalFlowKernel it tracks with
     (LKOpticalFlowKernel(ctx, **tracker_lk_params()) as the reference's constructor makes it); cmap holds the points.
@@ -1083,29 +1006,20 @@ class OpticalFlowTracker:
     Point lists are numpy arrays or torch tensors, host or CUDA; the set accessors return numpy copies, or with device=True
     torch views of the tracker's own memory, valid until its next call."""
 
+    _destroy = "srl_flow_tracker_destroy"
+
     def __init__(self, ctx: Context, cmap: "ColorVoxelMap", lk: "LKOpticalFlowKernel", maximum_tracked_points: int = 300):
         self.ctx, self.cmap, self.lk = ctx, cmap, lk
         h = C.c_void_p()
         _check(ctx.h, lib().srl_flow_tracker_create(ctx.h, cmap.h, lk.h, int(maximum_tracked_points), C.byref(h)))
         self.h = h
 
-    def close(self):
-        if getattr(self, "h", None):
-            lib().srl_flow_tracker_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
     def init(self, gray, image_time: float, ids, uv) -> None:
         """init / setTrackPoints (:188-211): last = {ids[i]: uv[i]}, both image times = image_time, and the Lucas-Kanade call
         on gray (its first image: the pyramid only).  ids: uint32 point ids (int32 tensors hold their bits); uv: (n, 2) float32."""
-        p_img, rows, cols, pitch = _gray_2d(gray)
-        p_ids, n = _ids_addr(ids)
-        p_uv, n_uv = _addr(uv, np.float32, 2)
+        _, p_img, rows, cols, pitch = _buffer(gray, np.uint8, image=True)
+        _, p_ids, n = _buffer(ids, np.uint32)
+        _, p_uv, n_uv = _buffer(uv, np.float32, 2)
         if n_uv != n:
             raise ValueError("ids and uv must hold the same number of points")
         _check(self.ctx.h, lib().srl_flow_tracker_init(self.h, C.c_void_p(p_img), int(cols), int(rows), int(pitch), float(image_time),
@@ -1114,7 +1028,7 @@ class OpticalFlowTracker:
     def trackImage(self, gray, image_time: float) -> bool:
         """trackImage(p_frame, -20) (:111-186) on gray_image at time_sweep_end; returns whether Lucas-Kanade ran (not below 30
         tracked points)."""
-        p_img, rows, cols, pitch = _gray_2d(gray)
+        _, p_img, rows, cols, pitch = _buffer(gray, np.uint8, image=True)
         called = C.c_int32(0)
         _check(self.ctx.h, lib().srl_flow_tracker_track_image(self.h, C.c_void_p(p_img), int(cols), int(rows), int(pitch), float(image_time),
                                                               C.byref(called)))
@@ -1125,9 +1039,7 @@ class OpticalFlowTracker:
         if mask is None:
             _check(self.ctx.h, lib().srl_flow_tracker_reject_matches(self.h, None, 0))
             return
-        if not _is_tensor(mask):
-            mask = np.ascontiguousarray(mask, np.uint8).reshape(-1)
-        p, n = _addr(mask, np.uint8, 1)
+        mask, p, n = _buffer(mask, np.uint8, convert=True)
         _check(self.ctx.h, lib().srl_flow_tracker_reject_matches(self.h, C.c_void_p(p), n))
 
     def removeOutlierUsingRansacPnp(self, inliers=None) -> bool:
@@ -1137,18 +1049,15 @@ class OpticalFlowTracker:
         if inliers is None:
             _check(self.ctx.h, lib().srl_flow_tracker_remove_outliers(self.h, None, 0, C.byref(r)))
             return bool(r.value)
-        if not _is_tensor(inliers):
-            inliers = np.ascontiguousarray(inliers, np.int32).reshape(-1)
-        p, n = _addr(inliers, np.int32, 1)
-        if n == 0:
-            p = _NO_INLIERS.ctypes.data          # an empty list is zero inliers, which a NULL pointer would not say
-        _check(self.ctx.h, lib().srl_flow_tracker_remove_outliers(self.h, C.c_void_p(p), n, C.byref(r)))
+        inliers, p, n = _buffer(inliers, np.int32, convert=True)
+        p = C.c_void_p(p) if n else ptr(_NO_INLIERS)   # an empty list is zero inliers, which a NULL pointer would not say
+        _check(self.ctx.h, lib().srl_flow_tracker_remove_outliers(self.h, p, n, C.byref(r)))
         return bool(r.value)
 
     def updateAndAppendTrackPoints(self, camera: "capi.Camera", candidates, mini_distance: float) -> None:
         """updateAndAppendTrackPoints(p_frame, map_tracker, mini_distance) (:13-102): camera is the frame's after the updates
         (fov_margin 0.005), candidates the refresh selection's point ids in its order (points_rgb_vec_for_projection)."""
-        p, n = _ids_addr(candidates)
+        _, p, n = _buffer(candidates, np.uint32)
         _check(self.ctx.h, lib().srl_flow_tracker_update_and_append(self.h, C.byref(camera), float(mini_distance), C.c_void_p(p), n))
 
     def _sets(self) -> "capi.FlowTrackerSets":
@@ -1161,35 +1070,29 @@ class OpticalFlowTracker:
         return dict(match=s.n_match, cur=s.n_cur, last=s.n_last)
 
     def _arrays(self, device, spec):
-        import torch
         out = []
-        for p, n, w, ts in spec:
-            shape = (n,) if w == 1 else (n, w)
-            if n == 0:
-                t = torch.empty(shape, dtype={"<i4": torch.int32, "<f4": torch.float32, "<f8": torch.float64}[ts],
-                                device=f"cuda:{self.ctx.device}")
-            else:
-                t = torch.as_tensor(_DeviceArray(p, shape, ts), device=f"cuda:{self.ctx.device}")
-            out.append(t if device else (t.cpu().numpy().view(np.uint32) if ts == "<i4" else t.cpu().numpy()))
+        for p, n, w, dt in spec:
+            t = _device_view(self.ctx, p, n, w, dt)
+            out.append(t if device else (t.cpu().numpy().view(np.uint32) if dt == np.int32 else t.cpu().numpy()))
         return tuple(out)
 
     def matches(self, device: bool = False):
         """(ids, last uv (n, 2) float32, new uv (n, 2) float32): what trackImage's Lucas-Kanade tracked, in last order — the two
         point lists findFundamentalMat is given.  ids are uint32 (numpy) or int32 holding their bits (device)."""
         s = self._sets()
-        return self._arrays(device, [(s.match_ids, s.n_match, 1, "<i4"), (s.match_last_uv, s.n_match, 2, "<f4"),
-                                     (s.match_uv, s.n_match, 2, "<f4")])
+        return self._arrays(device, [(s.match_ids, s.n_match, 1, np.int32), (s.match_last_uv, s.n_match, 2, np.float32),
+                                     (s.match_uv, s.n_match, 2, np.float32)])
 
     def current(self, device: bool = False):
         """(ids, uv (n, 2) float32, velocity (n, 2) float64): map_rgb_points_in_cur_image_pose and the points' image_velocity, what
         vioEsikf / vioPhotometric take."""
         s = self._sets()
-        return self._arrays(device, [(s.cur_ids, s.n_cur, 1, "<i4"), (s.cur_uv, s.n_cur, 2, "<f4"), (s.cur_velocity, s.n_cur, 2, "<f8")])
+        return self._arrays(device, [(s.cur_ids, s.n_cur, 1, np.int32), (s.cur_uv, s.n_cur, 2, np.float32), (s.cur_velocity, s.n_cur, 2, np.float64)])
 
     def last(self, device: bool = False):
         """(ids, uv (n, 2) float32): map_rgb_points_in_last_image_pose."""
         s = self._sets()
-        return self._arrays(device, [(s.last_ids, s.n_last, 1, "<i4"), (s.last_uv, s.n_last, 2, "<f4")])
+        return self._arrays(device, [(s.last_ids, s.n_last, 1, np.int32), (s.last_uv, s.n_last, 2, np.float32)])
 
     def lastImageTime(self) -> float:
         return self._sets().last_image_time
@@ -1294,7 +1197,7 @@ def ntu_lidar_params(**kw) -> dict:
     return dict(dict(lidar_type=3, n_scans=16, scan_rate=20, time_unit=3, blind=4.0, point_filter_num=4), **kw)
 
 
-class CloudProcessing:
+class CloudProcessing(_Handle):
     """cloudProcessing (src/cloudProcessing.cpp, srl_lidar_*) with its point_buffer kept on the device.  Messages are byte buffers
     as they come off the wire: numpy arrays (a structured array is taken as its bytes) or torch uint8 tensors, host or CUDA.
 
@@ -1306,6 +1209,8 @@ class CloudProcessing:
         n, xyz, ts = cp.cut(t, device=True)
         frame = lio_opt.buildFrame(xyz, ts, states, ..., point_time_enable=cp.isPointTimeEnable())"""
 
+    _destroy = "srl_lidar_destroy"
+
     def __init__(self, ctx: Context, lidar_type: int, n_scans: int, scan_rate: int, time_unit: int, blind: float,
                  point_filter_num: int, capacity: int = 1 << 18):
         self.ctx = ctx
@@ -1315,34 +1220,14 @@ class CloudProcessing:
         _check(ctx.h, lib().srl_lidar_create(ctx.h, C.byref(self.params), int(capacity), C.byref(h)))
         self.h = h
 
-    def close(self):
-        if getattr(self, "h", None):
-            lib().srl_lidar_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    @staticmethod
-    def _bytes(a):
-        if _is_tensor(a):
-            if not a.is_contiguous():
-                raise TypeError("expected a contiguous tensor")
-            return a.data_ptr(), a.numel() * a.element_size()
-        a = np.ascontiguousarray(a)
-        return a.ctypes.data, a.nbytes
-
     def livoxHandler(self, records, stamp: float, stride: int = 19) -> int:
-        p, nbytes = self._bytes(records)
+        records, p, nbytes = _buffer(records, None, convert=True)
         n = C.c_int64(0)
         _check(self.ctx.h, lib().srl_lidar_livox(self.h, C.c_void_p(p), nbytes // stride, stride, float(stamp), C.byref(n)))
         return n.value
 
     def process(self, data, layout: dict, stamp: float) -> int:
-        p, nbytes = self._bytes(data)
+        data, p, nbytes = _buffer(data, None, convert=True)
         y = capi.Cloud2Layout(int(layout["point_step"]), int(layout["x"]), int(layout["y"]), int(layout["z"]), int(layout["time"]),
                               int(layout.get("ring", -1)), int(layout.get("width", 0)), int(layout.get("row_step", 0)))
         n_pts = (nbytes // y.row_step) * y.width if y.row_step else nbytes // y.point_step
@@ -1354,10 +1239,7 @@ class CloudProcessing:
         n, xyz, ts = C.c_int64(0), C.c_void_p(), C.c_void_p()
         _check(self.ctx.h, lib().srl_lidar_cut(self.h, float(t), C.byref(n), C.byref(xyz), C.byref(ts)))
         k = n.value
-        import torch
-        dev = torch.device("cuda", self.ctx.device)
-        xyz_t = torch.as_tensor(_DeviceArray(xyz.value or 0, (k, 3), "<f8"), device=dev)
-        ts_t = torch.as_tensor(_DeviceArray(ts.value or 0, (k,), "<f8"), device=dev)
+        xyz_t, ts_t = _device_view(self.ctx, xyz.value, k, 3, np.float64), _device_view(self.ctx, ts.value, k, 1, np.float64)
         if device:
             return k, xyz_t, ts_t
         return k, xyz_t.cpu().numpy(), ts_t.cpu().numpy()
@@ -1383,11 +1265,7 @@ class CloudProcessing:
 
 def device_sort_permutation(ctx: Context, keys, return_heapsorts: bool = False):
     """The device std::sort's permutation of float64 keys (host or CUDA): perm[p] = the index of the key that ends at p."""
-    if _is_tensor(keys):
-        p, n = keys.data_ptr(), keys.numel()
-    else:
-        keys = f64(keys).reshape(-1)
-        p, n = keys.ctypes.data, keys.size
+    keys, p, n = _buffer(keys, np.float64, convert=True)
     perm = np.empty(n, np.int32)
     h = C.c_int32(0)
     _check(ctx.h, lib().srl_lidar_sort_replay(ctx.h, C.c_void_p(p), n, ptr(perm), C.byref(h)))

@@ -31,21 +31,34 @@ def test_library_exports_every_symbol_the_header_declares():
         assert re.search(rf"\bT {name}\b", out), f"{name} is not an exported text symbol"
 
 
+# every ctypes mirror of a header struct (a mismatch in a size or a field offset would silently corrupt every call)
+STRUCTS = dict(IcpParams="srl_icp_params", EskfState="srl_eskf_state", Frame="srl_frame", NormalEq="srl_normal_eq",
+               DebugOut="srl_debug_out", IekfSummary="srl_iekf_summary", ImuState="srl_imu_state", Camera="srl_camera",
+               LkParams="srl_lk_params", ImageParams="srl_image_params", VioState="srl_vio_state",
+               ProjectionParams="srl_projection_params", FlowTrackerSets="srl_flow_tracker_sets_out",
+               BuildFrameParams="srl_build_frame_params", BuildFrameInfo="srl_build_frame_info", CloudFramePtrs="srl_cloud_frame_ptrs",
+               LidarParams="srl_lidar_params", Cloud2Layout="srl_cloud2_layout", LidarInfo="srl_lidar_info", IekfIter="srl_iekf_iter")
+
+
 def test_struct_layouts_match_the_header():
-    # sizes the C compiler gives the structs (a mismatch here would silently corrupt every call)
-    src = r'''
-    #include <stdio.h>
-    #include "srlivo_b200.h"
-    int main(){ printf("%zu %zu %zu %zu %zu %zu %zu\n", sizeof(srl_icp_params), sizeof(srl_eskf_state), sizeof(srl_frame),
-        sizeof(srl_normal_eq), sizeof(srl_debug_out), sizeof(srl_iekf_summary), sizeof(srl_iekf_iter)); return 0; }'''
+    mirrors = {n for n, v in vars(capi).items() if isinstance(v, type) and issubclass(v, C.Structure)}
+    assert mirrors == set(STRUCTS), mirrors ^ set(STRUCTS)
+    lines, py = [], []
+    for name, c_name in STRUCTS.items():
+        t = getattr(capi, name)
+        lines.append(f'printf("%zu\\n", sizeof({c_name}));')
+        py.append((name, "sizeof", C.sizeof(t)))
+        for field, _ in t._fields_:
+            lines.append(f'printf("%zu\\n", offsetof({c_name}, {field}));')
+            py.append((name, field, getattr(t, field).offset))
+    src = "#include <stddef.h>\n#include <stdio.h>\n#include \"srlivo_b200.h\"\nint main(void){\n" + "\n".join(lines) + "\nreturn 0; }\n"
     import tempfile
     with tempfile.TemporaryDirectory() as d:
         open(os.path.join(d, "t.c"), "w").write(src)
         subprocess.check_call(["gcc", "-I", os.path.join(ROOT, "include"), "-o", os.path.join(d, "t"), os.path.join(d, "t.c")])
-        sizes = [int(x) for x in subprocess.check_output([os.path.join(d, "t")]).split()]
-    py = [C.sizeof(t) for t in (capi.IcpParams, capi.EskfState, capi.Frame, capi.NormalEq, capi.DebugOut,
-                                capi.IekfSummary, capi.IekfIter)]
-    assert sizes == py
+        got = [int(x) for x in subprocess.check_output([os.path.join(d, "t")]).split()]
+    assert len(got) == len(py)
+    assert [(n, f, v) for (n, f, _), v in zip(py, got)] == py
 
 
 def test_no_cpu_fallback_without_a_gpu():
