@@ -126,6 +126,8 @@ const char* srl_build_info(void);
 /* stream == NULL: the library creates its own non-blocking stream; otherwise a cudaStream_t to run on
  * (pass cudaStreamLegacy = (void*)1 for the legacy default stream, whose handle is NULL) */
 int srl_ctx_create(int device, void* cuda_stream, srl_ctx** out);
+/* Every handle created on a ctx records the ctx's device and may be destroyed before or after the ctx: no srl_*_destroy
+ * reads the ctx.  A handle outliving its ctx can only be destroyed; every other call on it needs the ctx. */
 void srl_ctx_destroy(srl_ctx* ctx);
 const char* srl_last_error(const srl_ctx* ctx);
 int srl_ctx_synchronize(srl_ctx* ctx);

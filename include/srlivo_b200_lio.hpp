@@ -292,7 +292,7 @@ private:
 // LKOpticalFlowKernel (include/lkpyramid.h:65-131) on the GPU, bit for bit: the constructor takes the reference's arguments
 // and defaults (criteria = (type, max_count, epsilon) of cv::TermCriteria, SRL_LK_COUNT | SRL_LK_EPS), trackImage mirrors
 // src/lkpyramid.cpp:755.  Points are (x, y) float pairs, the layout of std::vector<cv::Point2f>; every pointer overload takes
-// host or device memory.  The kernel must be destroyed before its context.
+// host or device memory.  It may be destroyed before or after its context.
 class LKOpticalFlowKernel {
 public:
     LKOpticalFlowKernel(srl_ctx* ctx, int win_w = 21, int win_h = 21, int maxLevel = 3, int criteria_type = SRL_LK_COUNT | SRL_LK_EPS,
@@ -390,8 +390,8 @@ private:
 
 // The image preparation of imageProcessing::process (src/imageProcessing.cpp:91-125) on the GPU, bit for bit OpenCV's: the
 // constructor is the first-image step for inputs of cols x rows, process() turns one BGR8 image into rgb_image (BGR8) and
-// gray_image.  Every pointer takes host or device memory; outputs are contiguous, outputSize() in pixels.  The object must be
-// destroyed before its context.
+// gray_image.  Every pointer takes host or device memory; outputs are contiguous, outputSize() in pixels.  The object may be
+// destroyed before or after its context.
 class ImageProcessing {
 public:
     ImageProcessing(srl_ctx* ctx, int image_width, int image_height, const std::array<double, 9>& camera_intrinsic,
@@ -462,7 +462,7 @@ private:
 // CustomPoint records, PointCloud2 data with the layout msg->fields gives); cut() is getMeasurements' pop loop (front timestamp
 // below t) and hands out device pointers that LioBackend::buildFrame / srl_build_frame take as they are, valid until the next
 // handler call.  Message pointers take host or device memory.  Not thread-safe: serialise handler calls against cut() and the
-// buildFrame that reads its pointers.  Destroy before the context.
+// buildFrame that reads its pointers.  It may be destroyed before or after its context.
 class cloudProcessing {
 public:
     cloudProcessing(srl_ctx* ctx, int lidar_type, int N_SCANS, int SCAN_RATE, int time_unit, double blind, int point_filter_num,

@@ -300,24 +300,17 @@ __global__ void k_ft_counts(const unsigned* __restrict__ ids, int n, const Color
     if (k < n) out[k] = cpts[ids[k]].outlier_count;
 }
 
-// A device array that grows by reallocation, keeping its first `keep` elements
-template <class T> struct DevBuf {
-    T* p = nullptr;
-    size_t cap = 0;
-};
-template <class T> int grow(srl_ctx* ctx, DevBuf<T>& b, size_t n, size_t keep) {
-    if (n <= b.cap) return SRL_OK;
-    size_t cap = std::max<size_t>(b.cap * 2, 256);
+// room for n elements in a device array that grows by reallocation, keeping its first `keep` elements
+template <class T> int grow(srl_ctx* ctx, DevArray<T>& b, size_t n, size_t keep) {
+    if (n <= b.size()) return SRL_OK;
+    size_t cap = std::max<size_t>(b.size() * 2, 256);
     while (cap < n) cap *= 2;
-    T* p = nullptr;
-    SRL_CUDA(ctx, cudaMalloc(&p, cap * sizeof(T)));
-    if (keep) SRL_CUDA(ctx, cudaMemcpyAsync(p, b.p, keep * sizeof(T), cudaMemcpyDeviceToDevice, ctx->stream));
-    if (b.p) SRL_CUDA(ctx, cudaFree(b.p));                 // waits for the copy
-    b.p = p;
-    b.cap = cap;
+    DevArray<T> p;
+    SRL_CUDA(ctx, p.alloc(cap));
+    if (keep) SRL_CUDA(ctx, cudaMemcpyAsync(p, b, keep * sizeof(T), cudaMemcpyDeviceToDevice, ctx->stream));
+    b = std::move(p);                                      // cudaFree of the old array waits for the copy
     return SRL_OK;
 }
-template <class T> void release(DevBuf<T>& b) { if (b.p) cudaFree(b.p); b.p = nullptr; b.cap = 0; }
 
 }  // namespace
 
@@ -330,12 +323,12 @@ struct srl_flow_tracker {
     double last_time = 0.0;
     bool have_time = false;
     int64_t n_last = 0, n_match = 0, n_cur = 0;
-    DevBuf<unsigned> last_ids, m_ids, c_ids, new_ids;
-    DevBuf<float2> last_uv, m_last, m_uv, c_uv, lk_uv, new_uv;     // new_*: init's set until its Lucas-Kanade call succeeded
-    DevBuf<double2> m_vel, c_vel;
-    DevBuf<unsigned char> m_in, lk_status;
-    long long* d_counts = nullptr;          // device [0, 4)
-    long long* h_counts = nullptr;          // pinned [0, 4)
+    DevArray<unsigned> last_ids, m_ids, c_ids, new_ids;
+    DevArray<float2> last_uv, m_last, m_uv, c_uv, lk_uv, new_uv;   // new_*: init's set until its Lucas-Kanade call succeeded
+    DevArray<double2> m_vel, c_vel;
+    DevArray<unsigned char> m_in, lk_status;
+    DevArray<long long> d_counts;           // [0, 4)
+    PinnedArray<long long> h_counts;        // [0, 4)
 };
 
 namespace {
@@ -371,7 +364,7 @@ int ensure_last(srl_flow_tracker* t, size_t n) {
 // Lucas-Kanade over n points' uv into lk_uv / lk_status
 int run_lk(srl_flow_tracker* t, const uint8_t* gray, int cols, int rows, size_t pitch, const float2* uv, int64_t n, int64_t* n_tracked) {
     return srl_lk_track_image(t->lk, gray, cols, rows, pitch, reinterpret_cast<const float*>(uv), (size_t)n,
-                              reinterpret_cast<float*>(t->lk_uv.p), t->lk_status.p, n_tracked);
+                              reinterpret_cast<float*>(t->lk_uv.get()), t->lk_status, n_tracked);
 }
 }  // namespace
 
@@ -385,23 +378,18 @@ int srl_flow_tracker_create(srl_ctx* ctx, srl_color_map* cm, srl_lk* lk, int32_t
         return set_err(ctx, SRL_BAD_ARG, "srl_flow_tracker_create: the colour map and the Lucas-Kanade tracker must use this ctx");
     if (maximum_tracked_points < 1) return set_err(ctx, SRL_BAD_ARG, "srl_flow_tracker_create: maximum_tracked_points must be >= 1");
     SRL_CUDA(ctx, cudaSetDevice(ctx->device));
-    srl_flow_tracker* t = new srl_flow_tracker();
+    std::unique_ptr<srl_flow_tracker> t(new srl_flow_tracker());
     t->ctx = ctx; t->device = ctx->device; t->cm = cm; t->lk = lk; t->max_points = maximum_tracked_points;
-    cudaError_t e = cudaMalloc(&t->d_counts, 4 * sizeof(long long));
-    if (e == cudaSuccess) e = cudaMallocHost(&t->h_counts, 4 * sizeof(long long));
-    if (e != cudaSuccess) { srl_flow_tracker_destroy(t); return cuda_fail(ctx, e, "srl_flow_tracker_create"); }
-    *out = t;
+    cudaError_t e = t->d_counts.alloc(4);
+    if (e == cudaSuccess) e = t->h_counts.alloc(4);
+    if (e != cudaSuccess) return cuda_fail(ctx, e, "srl_flow_tracker_create");
+    *out = t.release();
     return SRL_OK;
 }
 
 void srl_flow_tracker_destroy(srl_flow_tracker* t) {
     if (!t) return;
     cudaSetDevice(t->device);
-    release(t->last_ids); release(t->m_ids); release(t->c_ids); release(t->new_ids); release(t->new_uv);
-    release(t->last_uv); release(t->m_last); release(t->m_uv); release(t->c_uv); release(t->lk_uv);
-    release(t->m_vel); release(t->c_vel); release(t->m_in); release(t->lk_status);
-    if (t->d_counts) cudaFree(t->d_counts);
-    if (t->h_counts) cudaFreeHost(t->h_counts);
     delete t;
 }
 
@@ -442,14 +430,14 @@ int srl_flow_tracker_init(srl_flow_tracker* t, const uint8_t* gray, int cols, in
         SRL_CUDA(ctx, cub::DeviceRadixSort::SortPairs(d_tmp, tmp_sort, keys_a, keys_b, vals_a, vals_b, nn, 0, 32, st));   // stable
         // setTrackPoints (:205-208): map[id] = uv in input order, so a later duplicate overwrites an earlier one
         k_ft_unique<<<1, kSetThreads, 0, st>>>(nn, keys_b, vals_b, true, reinterpret_cast<const float2*>(s_uv.d), nullptr, nn,
-                                               t->new_ids.p, t->new_uv.p, nullptr, t->d_counts);
+                                               t->new_ids, t->new_uv, nullptr, t->d_counts);
         SRL_CUDA(ctx, cudaGetLastError());
         ctx->launches += 3;
         if ((rc = read_counts(t, 1)) != SRL_OK) return rc;
         n_new = t->h_counts[0];
     }
     int64_t k = 0;
-    if ((rc = run_lk(t, gray, cols, rows, pitch, t->new_uv.p, n_new, &k)) != SRL_OK) return rc;   // :196: on the first image, the pyramid only
+    if ((rc = run_lk(t, gray, cols, rows, pitch, t->new_uv, n_new, &k)) != SRL_OK) return rc;   // :196: on the first image, the pyramid only
     std::swap(t->last_ids, t->new_ids);
     std::swap(t->last_uv, t->new_uv);
     t->n_last = n_new;
@@ -475,12 +463,12 @@ int srl_flow_tracker_track_image(srl_flow_tracker* t, const uint8_t* gray, int c
         return SRL_OK;
     }
     int64_t tracked = 0;
-    int rc = run_lk(t, gray, cols, rows, pitch, t->last_uv.p, t->n_last, &tracked);
+    int rc = run_lk(t, gray, cols, rows, pitch, t->last_uv, t->n_last, &tracked);
     if (rc != SRL_OK) return rc;
     if (lk_called) *lk_called = 1;
-    k_ft_track<<<1, kSetThreads, 0, ctx->stream>>>((int)t->n_last, t->last_ids.p, t->last_uv.p, t->lk_uv.p, t->lk_status.p, dt, cols, rows,
-                                                   t->m_ids.p, t->m_last.p, t->m_uv.p, t->m_vel.p, t->m_in.p, nullptr, t->c_ids.p, t->c_uv.p,
-                                                   t->c_vel.p, t->d_counts);
+    k_ft_track<<<1, kSetThreads, 0, ctx->stream>>>((int)t->n_last, t->last_ids, t->last_uv, t->lk_uv, t->lk_status, dt, cols, rows,
+                                                   t->m_ids, t->m_last, t->m_uv, t->m_vel, t->m_in, nullptr, t->c_ids, t->c_uv,
+                                                   t->c_vel, t->d_counts);
     SRL_CUDA(ctx, cudaGetLastError());
     ctx->launches += 1;
     if ((rc = read_counts(t, 2)) != SRL_OK) return rc;
@@ -500,8 +488,8 @@ int srl_flow_tracker_reject_matches(srl_flow_tracker* t, const uint8_t* mask, si
     Staged<const unsigned char> s_mask(mask);
     int rc = carve_scratch(ctx, [&](Carve& c) { s_mask.place(c, n); });
     if (rc != SRL_OK || (rc = s_mask.upload(ctx, mask ? n : 0)) != SRL_OK) return rc;
-    k_ft_track<<<1, kSetThreads, 0, ctx->stream>>>((int)t->n_match, nullptr, nullptr, nullptr, nullptr, 0.0, 0, 0, t->m_ids.p, t->m_last.p,
-                                                   t->m_uv.p, t->m_vel.p, t->m_in.p, s_mask.d, t->c_ids.p, t->c_uv.p, t->c_vel.p,
+    k_ft_track<<<1, kSetThreads, 0, ctx->stream>>>((int)t->n_match, nullptr, nullptr, nullptr, nullptr, 0.0, 0, 0, t->m_ids, t->m_last,
+                                                   t->m_uv, t->m_vel, t->m_in, s_mask.d, t->c_ids, t->c_uv, t->c_vel,
                                                    t->d_counts);
     SRL_CUDA(ctx, cudaGetLastError());
     ctx->launches += 1;
@@ -523,8 +511,8 @@ int srl_flow_tracker_remove_outliers(srl_flow_tracker* t, const int32_t* inliers
     if (!inliers) {                                                // every entry of cur is an inlier: last = cur
         int rc = ensure_last(t, nc);
         if (rc != SRL_OK) return rc;
-        SRL_CUDA(ctx, cudaMemcpyAsync(t->last_ids.p, t->c_ids.p, nc * sizeof(unsigned), cudaMemcpyDeviceToDevice, st));
-        SRL_CUDA(ctx, cudaMemcpyAsync(t->last_uv.p, t->c_uv.p, nc * sizeof(float2), cudaMemcpyDeviceToDevice, st));
+        SRL_CUDA(ctx, cudaMemcpyAsync(t->last_ids, t->c_ids, nc * sizeof(unsigned), cudaMemcpyDeviceToDevice, st));
+        SRL_CUDA(ctx, cudaMemcpyAsync(t->last_uv, t->c_uv, nc * sizeof(float2), cudaMemcpyDeviceToDevice, st));
         SRL_CUDA(ctx, cudaStreamSynchronize(st));
         t->n_last = t->n_cur;
         *result = 1;
@@ -548,11 +536,11 @@ int srl_flow_tracker_remove_outliers(srl_flow_tracker* t, const int32_t* inliers
     if (rc != SRL_OK || (rc = s_in.upload(ctx, n)) != SRL_OK) return rc;
     long long uniq = 0;
     if (n) {
-        k_ft_pairs<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(nullptr, reinterpret_cast<const int*>(s_in.d), nn, t->c_ids.p, (int)nc, keys_a, vals_a);
+        k_ft_pairs<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(nullptr, reinterpret_cast<const int*>(s_in.d), nn, t->c_ids, (int)nc, keys_a, vals_a);
         SRL_CUDA(ctx, cudaGetLastError());
         SRL_CUDA(ctx, cub::DeviceRadixSort::SortPairs(d_tmp, tmp_sort, keys_a, keys_b, vals_a, vals_b, nn, 0, 32, st));
         // :310-317: both maps take the inliers with their current uv; std::map sorts them and drops repeats
-        k_ft_unique<<<1, kSetThreads, 0, st>>>(nn, keys_b, vals_b, false, t->c_uv.p, t->c_vel.p, (int)nc, o_ids, o_uv, o_vel, t->d_counts);
+        k_ft_unique<<<1, kSetThreads, 0, st>>>(nn, keys_b, vals_b, false, t->c_uv, t->c_vel, (int)nc, o_ids, o_uv, o_vel, t->d_counts);
         SRL_CUDA(ctx, cudaGetLastError());
         ctx->launches += 3;
         if ((rc = read_counts(t, 2)) != SRL_OK) return rc;
@@ -562,11 +550,11 @@ int srl_flow_tracker_remove_outliers(srl_flow_tracker* t, const int32_t* inliers
     if ((rc = ensure_last(t, (size_t)uniq)) != SRL_OK) return rc;
     if (uniq) {
         const size_t u = (size_t)uniq;
-        SRL_CUDA(ctx, cudaMemcpyAsync(t->last_ids.p, o_ids, u * sizeof(unsigned), cudaMemcpyDeviceToDevice, st));
-        SRL_CUDA(ctx, cudaMemcpyAsync(t->last_uv.p, o_uv, u * sizeof(float2), cudaMemcpyDeviceToDevice, st));
-        SRL_CUDA(ctx, cudaMemcpyAsync(t->c_ids.p, o_ids, u * sizeof(unsigned), cudaMemcpyDeviceToDevice, st));
-        SRL_CUDA(ctx, cudaMemcpyAsync(t->c_uv.p, o_uv, u * sizeof(float2), cudaMemcpyDeviceToDevice, st));
-        SRL_CUDA(ctx, cudaMemcpyAsync(t->c_vel.p, o_vel, u * sizeof(double2), cudaMemcpyDeviceToDevice, st));
+        SRL_CUDA(ctx, cudaMemcpyAsync(t->last_ids, o_ids, u * sizeof(unsigned), cudaMemcpyDeviceToDevice, st));
+        SRL_CUDA(ctx, cudaMemcpyAsync(t->last_uv, o_uv, u * sizeof(float2), cudaMemcpyDeviceToDevice, st));
+        SRL_CUDA(ctx, cudaMemcpyAsync(t->c_ids, o_ids, u * sizeof(unsigned), cudaMemcpyDeviceToDevice, st));
+        SRL_CUDA(ctx, cudaMemcpyAsync(t->c_uv, o_uv, u * sizeof(float2), cudaMemcpyDeviceToDevice, st));
+        SRL_CUDA(ctx, cudaMemcpyAsync(t->c_vel, o_vel, u * sizeof(double2), cudaMemcpyDeviceToDevice, st));
         SRL_CUDA(ctx, cudaStreamSynchronize(st));
     }
     t->n_last = t->n_cur = uniq;
@@ -626,7 +614,7 @@ int srl_flow_tracker_update_and_append(srl_flow_tracker* t, const srl_camera* ca
     const ColorMapView mv = color_map_view(t->cm);
     const double thr = 2.0 * (double)cam->cols / 320.0;            // :18
     SRL_CUDA(ctx, cudaMemsetAsync(t->d_counts, 0, 2 * sizeof(long long), st));
-    k_ft_loop1<<<1, kSetThreads, 0, st>>>(nl, t->last_ids.p, t->last_uv.p, mv, color_map_states(t->cm), cc, mini_distance, u0, v0, bits_v,
+    k_ft_loop1<<<1, kSetThreads, 0, st>>>(nl, t->last_ids, t->last_uv, mv, color_map_states(t->cm), cc, mini_distance, u0, v0, bits_v,
                                           none, thr, proj, s_ids, s_uv, keys_a, ranks_a, t->d_counts);
     SRL_CUDA(ctx, cudaGetLastError());
     int launches = 1;
@@ -649,7 +637,7 @@ int srl_flow_tracker_update_and_append(srl_flow_tracker* t, const srl_camera* ca
     const int bound = nl + n_ins;
     if (bound) {
         k_ft_merge<<<(unsigned)((bound + 255) / 256), 256, 0, st>>>(s_ids, s_uv, mc ? i_ids_b : nullptr, mc ? i_uv_b : nullptr, t->d_counts,
-                                                                    bound, t->last_ids.p, t->last_uv.p);
+                                                                    bound, t->last_ids, t->last_uv);
         SRL_CUDA(ctx, cudaGetLastError());
         ++launches;
     }
@@ -662,14 +650,14 @@ int srl_flow_tracker_update_and_append(srl_flow_tracker* t, const srl_camera* ca
 int srl_flow_tracker_sets(srl_flow_tracker* t, srl_flow_tracker_sets_out* out) {
     if (!t || !out) return SRL_BAD_ARG;
     out->n_match = t->n_match; out->n_cur = t->n_cur; out->n_last = t->n_last;
-    out->match_ids = t->m_ids.p;
-    out->match_last_uv = reinterpret_cast<const float*>(t->m_last.p);
-    out->match_uv = reinterpret_cast<const float*>(t->m_uv.p);
-    out->cur_ids = t->c_ids.p;
-    out->cur_uv = reinterpret_cast<const float*>(t->c_uv.p);
-    out->cur_velocity = reinterpret_cast<const double*>(t->c_vel.p);
-    out->last_ids = t->last_ids.p;
-    out->last_uv = reinterpret_cast<const float*>(t->last_uv.p);
+    out->match_ids = t->m_ids;
+    out->match_last_uv = reinterpret_cast<const float*>(t->m_last.get());
+    out->match_uv = reinterpret_cast<const float*>(t->m_uv.get());
+    out->cur_ids = t->c_ids;
+    out->cur_uv = reinterpret_cast<const float*>(t->c_uv.get());
+    out->cur_velocity = reinterpret_cast<const double*>(t->c_vel.get());
+    out->last_ids = t->last_ids;
+    out->last_uv = reinterpret_cast<const float*>(t->last_uv.get());
     out->last_image_time = t->last_time;
     return SRL_OK;
 }

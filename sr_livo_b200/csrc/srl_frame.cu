@@ -186,22 +186,18 @@ struct WordStream {
     srl_ctx* ctx = nullptr;
     const unsigned long long* replay = nullptr;   // host, n_replay words; nullptr: mt19937_64 at its default seed
     size_t n_replay = 0;
-    unsigned long long* d_words = nullptr;        // device copy of words [0, n_words)
+    DevArray<unsigned long long> d_words;         // device copy of words [0, n_words)
     size_t n_words = 0;
     size_t pos = 0;                               // next unused word
     bool host = false;                            // option "shuffle_on_host": draw on the host from a host engine
     std::mt19937_64 host_engine;
-    ~WordStream() { if (d_words) cudaFree(d_words); }
 
     // words [0, need) on the device
     int ensure(size_t need) {
         if (need <= n_words) return SRL_OK;
         if (replay && need > n_replay) return set_err(ctx, SRL_BAD_ARG, "replayed engine stream exhausted");
         const size_t count = replay ? n_replay : std::max(need + 4096, 2 * n_words);
-        unsigned long long* d = nullptr;
-        SRL_CUDA(ctx, cudaMalloc(&d, std::max<size_t>(count, 1) * sizeof(unsigned long long)));
-        if (d_words) { cudaFree(d_words); }
-        d_words = d;
+        SRL_CUDA(ctx, d_words.alloc(std::max<size_t>(count, 1)));
         if (replay) {
             SRL_CUDA(ctx, cudaMemcpyAsync(d_words, replay, count * sizeof(unsigned long long), cudaMemcpyHostToDevice, ctx->stream));
         } else {
@@ -336,9 +332,10 @@ using namespace srl;
 
 struct srl_cloud_frame {
     srl_ctx* ctx = nullptr;
+    int device = 0;
     size_t capacity = 0;
     size_t n = 0;
-    void* mem = nullptr;
+    DevArray<char> mem;
     // the frame, final order
     double *raw = nullptr, *point = nullptr, *imu = nullptr, *rel = nullptr, *alpha = nullptr, *ts = nullptr;
     int* src = nullptr;
@@ -379,6 +376,7 @@ static int frame_reserve(srl_cloud_frame* f, size_t cap) {
     cap = std::max<size_t>(cap, 1024);
     srl_cloud_frame g;   // the grown frame, laid out first to measure it
     g.ctx = ctx;
+    g.device = f->device;
     g.capacity = cap;
     cub::DeviceSelect::Flagged(nullptr, g.sel_bytes, (unsigned int*)nullptr, (unsigned char*)nullptr, (unsigned int*)nullptr, (int*)nullptr, (int)cap);
     cub::DeviceRadixSort::SortKeys(nullptr, g.sw.cub_bytes, (unsigned long long*)nullptr, (unsigned long long*)nullptr, (int)cap, 0, 64);
@@ -386,8 +384,8 @@ static int frame_reserve(srl_cloud_frame* f, size_t cap) {
     frame_layout(g, probe, cap);
     SRL_CUDA(ctx, cudaSetDevice(ctx->device));
     SRL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    SRL_CUDA(ctx, cudaMalloc(&g.mem, probe.used));
-    Carve c{static_cast<char*>(g.mem), 0};
+    SRL_CUDA(ctx, g.mem.alloc(probe.used));
+    Carve c{g.mem, 0};
     frame_layout(g, c, cap);
     if (f->mem && f->n) {   // the frame moves with its block: a build refused after growing still leaves it as it was
         const size_t n = f->n;
@@ -400,8 +398,7 @@ static int frame_reserve(srl_cloud_frame* f, size_t cap) {
         SRL_CUDA(ctx, cudaStreamSynchronize(st));
         g.n = n;
     }
-    if (f->mem) cudaFree(f->mem);
-    *f = g;
+    *f = std::move(g);
     return SRL_OK;
 }
 
@@ -418,16 +415,18 @@ int srl_cloud_frame_create(srl_ctx* ctx, size_t capacity, srl_cloud_frame** out)
     if (!ctx || !out) return SRL_BAD_ARG;
     *out = nullptr;
     if (capacity > 0x7fffffffULL) return set_err(ctx, SRL_BAD_ARG, "srl_cloud_frame_create: capacity must fit in int32");
-    srl_cloud_frame* f = new srl_cloud_frame();
+    std::unique_ptr<srl_cloud_frame> f(new srl_cloud_frame());
     f->ctx = ctx;
-    int rc = frame_reserve(f, capacity);
-    if (rc != SRL_OK) { delete f; return rc; }
-    *out = f;
+    f->device = ctx->device;
+    const int rc = frame_reserve(f.get(), capacity);
+    if (rc != SRL_OK) return rc;
+    *out = f.release();
     return SRL_OK;
 }
 void srl_cloud_frame_destroy(srl_cloud_frame* f) {
     if (!f) return;
-    if (f->mem) { cudaSetDevice(f->ctx->device); cudaStreamSynchronize(f->ctx->stream); cudaFree(f->mem); }
+    cudaSetDevice(f->device);
+    cudaDeviceSynchronize();   // the last build's kernels and copies have finished
     delete f;
 }
 size_t srl_cloud_frame_size(const srl_cloud_frame* f) { return f ? f->n : 0; }
@@ -597,6 +596,7 @@ int srl_shuffle_replay(srl_ctx* ctx, const uint64_t* words, size_t n_words, size
     SRL_CUDA(ctx, cudaSetDevice(ctx->device));
     srl_cloud_frame f;
     f.ctx = ctx;
+    f.device = ctx->device;
     int rc = frame_reserve(&f, n);
     if (rc != SRL_OK) return rc;
     WordStream ws;
@@ -618,8 +618,6 @@ int srl_shuffle_replay(srl_ctx* ctx, const uint64_t* words, size_t n_words, size
         }
     }
     cudaStreamSynchronize(ctx->stream);
-    cudaFree(f.mem);
-    f.mem = nullptr;
     return rc;
 }
 

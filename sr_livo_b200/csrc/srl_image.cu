@@ -259,7 +259,7 @@ int srl_image_create(srl_ctx* ctx, const srl_image_params* p, int cols, int rows
         return set_err(ctx, SRL_BAD_ARG, "srl_image_create: the output (image_width, image_height) / scale factor must be 16..32767 pixels each way");
     double ir[9];
     if (!inv3(K, ir)) return set_err(ctx, SRL_BAD_ARG, "srl_image_create: the scaled camera_intrinsic has no finite inverse");
-    auto* im = new srl_image;
+    std::unique_ptr<srl_image> im(new srl_image);
     im->ctx = ctx;
     im->device = ctx->device;
     vio_initial_covariance(im->cov);
@@ -278,13 +278,13 @@ int srl_image_create(srl_ctx* ctx, const srl_image_params* p, int cols, int rows
     im->th = (im->rows + (pad ? t - im->rows % t : 0)) / t;
     const size_t n = (size_t)im->cols * im->rows;
     cudaError_t e = cudaSetDevice(ctx->device);
-    if (e == cudaSuccess) e = cudaMalloc(&im->map1, n * sizeof(short2));
-    if (e == cudaSuccess) e = cudaMalloc(&im->map2, n * sizeof(uint16_t));
-    if (e == cudaSuccess) e = cudaMalloc(&im->planes, n * kImgPlanes);
-    if (e == cudaSuccess) e = cudaMalloc(&im->lut, (size_t)2 * t * t * 256);
-    for (int i = 0; i < 4 && e == cudaSuccess; ++i) e = cudaEventCreate(&im->ev[i]);
-    for (int i = 0; i < 4 && e == cudaSuccess; ++i) e = cudaEventCreate(&im->vio_ev[i]);
-    if (e == cudaSuccess) e = cudaMalloc(&im->d_vio_out, sizeof(srl::VioOut));
+    if (e == cudaSuccess) e = im->map1.alloc(n);
+    if (e == cudaSuccess) e = im->map2.alloc(n);
+    if (e == cudaSuccess) e = im->planes.alloc(n * kImgPlanes);
+    if (e == cudaSuccess) e = im->lut.alloc((size_t)2 * t * t * 256);
+    for (int i = 0; i < 4 && e == cudaSuccess; ++i) e = im->ev[i].create();
+    for (int i = 0; i < 4 && e == cudaSuccess; ++i) e = im->vio_ev[i].create();
+    if (e == cudaSuccess) e = im->d_vio_out.alloc(1);
     if (e == cudaSuccess) {
         MapArgs a = {};
         for (int k = 0; k < 9; ++k) a.ir[k] = ir[k];
@@ -306,26 +306,14 @@ int srl_image_create(srl_ctx* ctx, const srl_image_params* p, int cols, int rows
         ctx->launches += 1;
     }
     if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-    if (e != cudaSuccess) {
-        srl_image_destroy(im);
-        return cuda_fail(ctx, e, "srl_image_create");
-    }
-    *out = im;
+    if (e != cudaSuccess) return cuda_fail(ctx, e, "srl_image_create");
+    *out = im.release();
     return SRL_OK;
 }
 
 void srl_image_destroy(srl_image* im) {
     if (!im) return;
-    cudaSetDevice(im->device);   // not through im->ctx: a handle may outlive its ctx
-    if (im->map1) cudaFree(im->map1);
-    if (im->map2) cudaFree(im->map2);
-    if (im->planes) cudaFree(im->planes);
-    if (im->lut) cudaFree(im->lut);
-    if (im->d_vio_out) cudaFree(im->d_vio_out);
-    for (auto& e : im->ev)
-        if (e) cudaEventDestroy(e);
-    for (auto& e : im->vio_ev)
-        if (e) cudaEventDestroy(e);
+    cudaSetDevice(im->device);
     delete im;
 }
 

@@ -5,7 +5,10 @@
 #include <math_constants.h>
 
 #include <cstdint>
+#include <memory>
 #include <string>
+#include <type_traits>
+#include <utility>
 #include <vector>
 
 #include "../../include/srlivo_b200.h"
@@ -13,6 +16,66 @@
 #include "srl_math.cuh"
 
 namespace srl {
+
+// ---- ownership of the library's CUDA resources ------------------------------------------------------------------
+// Every device array, pinned host array and event a handle uses is held by one of these move-only owners, which frees
+// it in its destructor, so a handle is released by deleting it and a failed create leaks nothing.  alloc() frees the
+// array it replaces only once the new one exists: on failure the owner holds what it held.  The caller has set the
+// handle's device.  cudaFree waits for the device to go idle: nothing may be freed or replaced between launch_iekf_loop
+// and the wait in iekf_loop_finish, where the persistent ESIKF block spins on passes the host has yet to enqueue.
+enum class MemSpace { Device, Pinned, Mapped };   // cudaMalloc, cudaMallocHost, cudaHostAlloc(cudaHostAllocMapped)
+template <class T, MemSpace S = MemSpace::Device> class Owned {
+    using Elem = std::conditional_t<std::is_void<T>::value, char, T>;   // Owned<void> counts bytes
+    T *p_ = nullptr, *d_ = nullptr;    // the allocation and its device-side address (they differ for Mapped only)
+    size_t n_ = 0;
+
+public:
+    Owned() = default;
+    Owned(Owned&& o) noexcept : p_(std::exchange(o.p_, nullptr)), d_(std::exchange(o.d_, nullptr)), n_(std::exchange(o.n_, 0)) {}
+    Owned& operator=(Owned&& o) noexcept {
+        if (this != &o) { reset(); p_ = std::exchange(o.p_, nullptr); d_ = std::exchange(o.d_, nullptr); n_ = std::exchange(o.n_, 0); }
+        return *this;
+    }
+    ~Owned() { reset(); }
+    // a new array of `count` elements in place of the held one
+    cudaError_t alloc(size_t count) {
+        void *p = nullptr, *d = nullptr;
+        const size_t bytes = count * sizeof(Elem);
+        cudaError_t e = S == MemSpace::Device ? cudaMalloc(&p, bytes)
+                      : S == MemSpace::Pinned ? cudaMallocHost(&p, bytes) : cudaHostAlloc(&p, bytes, cudaHostAllocMapped);
+        if (e == cudaSuccess && S == MemSpace::Mapped && (e = cudaHostGetDevicePointer(&d, p, 0)) != cudaSuccess) cudaFreeHost(p);
+        if (e != cudaSuccess) return e;
+        reset();
+        p_ = static_cast<T*>(p); d_ = static_cast<T*>(S == MemSpace::Mapped ? d : p); n_ = count;
+        return cudaSuccess;
+    }
+    // `count` elements unless an array is held already: then nothing is allocated or released
+    cudaError_t ensure(size_t count) { return p_ ? cudaSuccess : alloc(count); }
+    void reset() {
+        if (p_) { if (S == MemSpace::Device) cudaFree(p_); else cudaFreeHost(p_); }
+        p_ = d_ = nullptr; n_ = 0;
+    }
+    T* get() const { return p_; }
+    operator T*() const { return p_; }
+    T* operator->() const { return p_; }
+    T* dev() const { return d_; }
+    size_t size() const { return n_; }     // elements
+};
+template <class T> using DevArray = Owned<T, MemSpace::Device>;
+template <class T> using PinnedArray = Owned<T, MemSpace::Pinned>;
+template <class T> using MappedArray = Owned<T, MemSpace::Mapped>;
+
+class Event {
+    cudaEvent_t e_ = nullptr;
+
+public:
+    Event() = default;
+    Event(Event&& o) noexcept : e_(std::exchange(o.e_, nullptr)) {}
+    Event& operator=(Event&& o) noexcept { std::swap(e_, o.e_); return *this; }   // o destroys what this held
+    ~Event() { if (e_) cudaEventDestroy(e_); }
+    cudaError_t create() { return e_ ? cudaSuccess : cudaEventCreate(&e_); }   // default flags; a held event is kept
+    operator cudaEvent_t() const { return e_; }
+};
 
 constexpr int kK1Warps = 8;
 constexpr int kK1Threads = kK1Warps * 32;
@@ -451,52 +514,54 @@ struct srl_ctx {
     int64_t launches = 0;
     // optional CUDA-event timing of k1_assoc
     bool timing = false;
-    cudaEvent_t ev0[2] = {nullptr, nullptr}, ev1[2] = {nullptr, nullptr};   // two pairs: the pass in flight and the one before
+    srl::Event ev0[2], ev1[2];      // two pairs: the pass in flight and the one before
     bool ev_pending[2] = {false, false};
     int ev_cur = 0;
     double k1_ms = 0.0;
     int64_t k1_launches = 0;
     // per-pass scratch
-    double* d_partials = nullptr;   // [max_grid][32]
+    srl::DevArray<double> d_partials;   // [max_grid][32]
     int max_grid = 0;
-    unsigned int* d_ticket = nullptr;
-    unsigned int* d_chunk_tickets = nullptr;   // [max_grid / 32 + 1], zero between passes
-    double* d_chunk_sums = nullptr;            // [max_grid / 32 + 1][32]
-    double* d_out32 = nullptr;
-    double* h_out32 = nullptr;      // pinned + mapped: [0,32) sums, [32] sequence flag written by the pass's last kernel, [33..64) scratch
-    double* d_h_out32 = nullptr;    // device-side address of h_out32
+    srl::DevArray<unsigned int> d_ticket;
+    srl::DevArray<unsigned int> d_chunk_tickets;   // [max_grid / 32 + 1], zero between passes
+    srl::DevArray<double> d_chunk_sums;            // [max_grid / 32 + 1][32]
+    srl::DevArray<double> d_out32;
+    srl::MappedArray<double> h_out32;   // [0,32) sums, [32] sequence flag written by the pass's last kernel, [33..64) scratch
     unsigned long long host_seq = 0;
-    long long* d_k2_state = nullptr;
-    unsigned long long* d_cap_chunks = nullptr;   // device-resident loop: k2_cap_reduce counts the capped chunks that did work
+    srl::DevArray<long long> d_k2_state;
+    srl::DevArray<unsigned long long> d_cap_chunks;   // device-resident loop: k2_cap_reduce counts the capped chunks that did work
     int64_t cap_chunks_run = 0;              // counter "cap_chunks_run": capped chunks processed by the last update's passes
     bool cap_chunks_on_device = false;       // ... still to be read from d_cap_chunks
-    srl::PassStats* d_stats = nullptr;
-    double* d_fast_out = nullptr;            // k1_fast's 32 sums, added by the exact-fallback launch
+    srl::DevArray<srl::PassStats> d_stats;
+    srl::DevArray<double> d_fast_out;        // k1_fast's 32 sums, added by the exact-fallback launch
     bool force_exact = false;
     int force_amb_mod = 0;                   // test knob for the k1_fast -> k1_assoc hand-over
     int variant = 0;                         // 0 auto, 1 = k1_fast, 2 = k1_assoc only, 3 = k1_scan + k1_fit (1 and 3 with the exact fallback)
     srl::KernelChoice choice;
-    unsigned long long* d_scan_count = nullptr;
+    srl::DevArray<unsigned long long> d_scan_count;
     // device-resident updateIEKF loop (row N1)
     bool kernels_preloaded = false;          // the instances `choice` can launch are loaded; setting an integer option clears it
     int shuffle_rule = 0;                    // option "shuffle_rule": srl_build_frame's draws, 0 Lemire (libstdc++ with __int128), 1 division
     bool shuffle_on_host = false;            // option "shuffle_on_host": srl_build_frame's shuffles as a host Fisher-Yates + upload
     int concurrent_kernels = -1;             // -1 not probed yet; 0: kernels of this process are serialised (profiler): host loop
     bool device_loop = true;                 // option "device_loop" / SRL_DEVICE_LOOP: 0 = the host-driven loop of round 1
-    srl::IekfDev* d_iekf = nullptr;
-    srl::IekfHostOut* h_iekf = nullptr;      // pinned + mapped
-    srl::IekfHostOut* d_h_iekf = nullptr;    // its device-side address
+    srl::DevArray<srl::IekfDev> d_iekf;
+    srl::MappedArray<srl::IekfHostOut> h_iekf;
     unsigned long long iekf_seq = 0;
     unsigned long long loop_base = 64;       // ticket of the next sweep's pass 0 (grows by 64 per sweep)
     cudaStream_t loop_stream = nullptr;      // side stream of the persistent ESIKF block
     double step_cycles_sum = 0.0;            // counter "iekf_step_cycles_avg": clock ticks from "sums seen" to "pose published"
     long long step_cycles_n = 0;
-    cudaEvent_t loop_ev0[srl::kLoopMaxPasses] = {nullptr}, loop_ev1[srl::kLoopMaxPasses] = {nullptr};   // timing mode: one pair per enqueued pass
+    srl::Event loop_ev0[srl::kLoopMaxPasses], loop_ev1[srl::kLoopMaxPasses];   // timing mode: one pair per enqueued pass
     // generic scratch (map insert)
-    void* d_scratch = nullptr;
+    srl::DevArray<void> d_scratch;
     size_t scratch_bytes = 0;
-    void* h_pinned = nullptr;
+    srl::PinnedArray<void> h_pinned;
     size_t pinned_bytes = 0;
+    ~srl_ctx() {   // srl_ctx_destroy has waited for both streams
+        if (loop_stream) cudaStreamDestroy(loop_stream);
+        if (own_stream && stream) cudaStreamDestroy(stream);
+    }
 };
 
 namespace srl {
@@ -521,16 +586,16 @@ struct srl_image {
     int tiles = 0, tw = 0, th = 0;     // CLAHE's grid and its tile size
     double scale = 1.;                 // image_scale_factor
     double K[9] = {0};                 // the scaled intrinsics
-    short2* map1 = nullptr;
-    uint16_t* map2 = nullptr;
-    uint8_t* planes = nullptr;
-    uint8_t* lut = nullptr;
-    cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};   // call start, image uploaded, remapped, equalised
+    srl::DevArray<short2> map1;
+    srl::DevArray<uint16_t> map2;
+    srl::DevArray<uint8_t> planes;
+    srl::DevArray<uint8_t> lut;
+    srl::Event ev[4];                  // call start, image uploaded, remapped, equalised
     bool timed = false;
     // the camera updates (srl_vio.cu)
     double cov[121] = {0};             // imageProcessing::covariance
-    srl::VioOut* d_vio_out = nullptr;  // device
-    cudaEvent_t vio_ev[4] = {nullptr, nullptr, nullptr, nullptr};   // before / after the esikf kernel, the photometric kernel
+    srl::DevArray<srl::VioOut> d_vio_out;
+    srl::Event vio_ev[4];              // before / after the esikf kernel, the photometric kernel
     bool vio_ran[2] = {false, false}, vio_timed[2] = {false, false};
     int vio_iterations[2] = {0, 0}, vio_points[2] = {0, 0};
     double vio_acc[2] = {0., 0.};
@@ -539,15 +604,23 @@ struct srl_image {
 namespace srl {
 // Device array that grows in place: virtual address space for its limit is reserved once, and physical memory is mapped
 // behind it on demand (CUDA VMM), so its address never changes and growing copies nothing.  Newly mapped bytes are zero.
+// The destructor waits for the device before it unmaps (srl_map.cu): unmapping does not wait, and the zero fill of the
+// last growth may still be running.
 struct VmArray {
     unsigned long long base = 0;    // CUdeviceptr
     size_t granularity = 0, reserved = 0, mapped = 0;
     std::vector<std::pair<unsigned long long, size_t>> chunks;   // (CUmemGenericAllocationHandle, bytes), in address order
+    VmArray() = default;
+    VmArray(VmArray&& o) noexcept { swap(o); }
+    VmArray& operator=(VmArray&& o) noexcept { swap(o); return *this; }   // o releases what this held
+    void swap(VmArray& o) { std::swap(base, o.base); std::swap(granularity, o.granularity); std::swap(reserved, o.reserved); std::swap(mapped, o.mapped); chunks.swap(o.chunks); }
+    ~VmArray();
 };
 }  // namespace srl
 
 struct srl_map {
     srl_ctx* ctx = nullptr;
+    int device = 0;
     double voxel_size = 1.0;
     int cap = 20;
     int block_pts = srl::kBlockCap; // points per block of the pool (block stride = 4 * block_pts floats): kBlockCap for
@@ -556,19 +629,20 @@ struct srl_map {
     size_t committed_voxels = 0;    // blocks backed by memory; grows inside the insert / upload entry points only
     size_t capacity = 0;            // slots (power of two, >= 2 x committed_voxels): rebuilt when the map grows, so the
                                     // pass kernels take d_slots / capacity from the map at every call
-    srl::Slot* d_slots = nullptr;
+    srl::DevArray<srl::Slot> d_slots;
     srl::VmArray blocks_mem;
     float* d_blocks = nullptr;      // == blocks_mem.base
     int64_t n_voxels = 0;           // host mirror of the block count
-    long long* d_counters = nullptr;   // [0] n_points, [1] scratch
+    srl::DevArray<long long> d_counters;   // [0] n_points, [1] scratch
     srl_color_map* owner = nullptr; // the colour map whose voxel map this is: its per-voxel arrays grow with the blocks
 };
 
 struct srl_comm {
     srl_ctx* ctx = nullptr;
+    int device = 0;
     int rank = 0, world = 1;
-    unsigned long long* d_seq = nullptr;            // device counter of the exchanges run (CommDev::seq)
-    srl::Mailbox* d_mail = nullptr;                 // this rank's mailbox
+    srl::DevArray<unsigned long long> d_seq;        // device counter of the exchanges run (CommDev::seq)
+    srl::DevArray<srl::Mailbox> d_mail;             // this rank's mailbox
     srl::Mailbox* peer[srl::kMaxRanks] = {nullptr}; // mapped peers (peer[rank] == d_mail)
     bool opened[srl::kMaxRanks] = {false};
     bool connected = false;
@@ -576,22 +650,23 @@ struct srl_comm {
 
 struct srl_sweep {
     srl_ctx* ctx = nullptr;
+    int device = 0;
     size_t capacity = 0;
     size_t n = 0;
     size_t shard_begin = 0, shard_end = 0;
-    double* d_raw = nullptr;        // capacity*3
-    unsigned* d_order = nullptr;    // capacity: Morton order of the keypoints (lazily computed per upload)
+    srl::DevArray<double> d_raw;        // capacity*3
+    srl::DevArray<unsigned> d_order;    // capacity: Morton order of the keypoints (lazily computed per upload)
     bool order_valid = false;
-    bool flags_clean = false;       // d_flags holds zeros outside the range the current shard rewrites every pass
-    unsigned char* d_flags = nullptr;   // capacity
-    unsigned* d_cand_rows = nullptr;    // split form: 24 words per keypoint (k1_scan -> k1_fit)
-    double* d_rows = nullptr;       // capacity*8, lazily allocated (cap mode)
-    int* d_status = nullptr;        // capacity, lazily allocated
+    bool flags_clean = false;           // d_flags holds zeros outside the range the current shard rewrites every pass
+    srl::DevArray<unsigned char> d_flags;   // capacity
+    srl::DevArray<unsigned> d_cand_rows;    // split form: 24 words per keypoint (k1_scan -> k1_fit)
+    srl::DevArray<double> d_rows;       // capacity*8, lazily allocated (cap mode)
+    srl::DevArray<int> d_status;        // capacity, lazily allocated
     // debug buffers, lazily allocated
-    double* d_dbg_world = nullptr;
-    short* d_dbg_nbr = nullptr;
-    double* d_dbg_nbr_dist = nullptr;
-    double* d_dbg_plane = nullptr;
+    srl::DevArray<double> d_dbg_world;
+    srl::DevArray<short> d_dbg_nbr;
+    srl::DevArray<double> d_dbg_nbr_dist;
+    srl::DevArray<double> d_dbg_plane;
     int dbg_K = 0;
 };
 
@@ -631,7 +706,7 @@ template <class Layout> int carve_scratch(srl_ctx* ctx, Layout&& layout) {
     layout(probe);
     const int rc = ensure_scratch(ctx, probe.used);
     if (rc != SRL_OK) return rc;
-    Carve c{static_cast<char*>(ctx->d_scratch), 0};
+    Carve c{static_cast<char*>(ctx->d_scratch.get()), 0};
     layout(c);
     return SRL_OK;
 }

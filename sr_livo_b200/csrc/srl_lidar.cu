@@ -24,19 +24,18 @@ using namespace srl;
 
 struct srl_lidar {
     srl_ctx* ctx = nullptr;
+    int device = 0;
     srl_lidar_params p{};
     double scale = 1.0;                 // time_unit_scale: a double holding the float literal
     double last_end_time = -1.0;
     int given_offset_time = 0;
     int sweep_id = 0;
     // the queue: points [head, tail) of three device arrays of cap points
-    double* d_xyz = nullptr;
-    double* d_rel = nullptr;
-    double* d_ts = nullptr;
+    DevArray<double> d_xyz, d_rel, d_ts;
     size_t cap = 0, head = 0, tail = 0;
     double front_ts = NAN, back_ts = NAN;
-    void* d_out = nullptr;              // LidarOut
-    void* h_out = nullptr;              // pinned
+    DevArray<void> d_out;               // LidarOut
+    PinnedArray<void> h_out;
 };
 
 namespace {
@@ -494,18 +493,17 @@ int reserve(srl_lidar* l, size_t extra) {
     if (l->tail + extra <= l->cap) return SRL_OK;
     size_t cap = l->cap;
     if (size + extra > cap || l->head == 0) cap = std::max(2 * cap, size + extra);
-    double *xyz = nullptr, *rel = nullptr, *ts = nullptr;
-    SRL_CUDA(ctx, cudaMalloc(&xyz, cap * 3 * sizeof(double)));
-    SRL_CUDA(ctx, cudaMalloc(&rel, cap * sizeof(double)));
-    SRL_CUDA(ctx, cudaMalloc(&ts, cap * sizeof(double)));
+    DevArray<double> xyz, rel, ts;
+    SRL_CUDA(ctx, xyz.alloc(cap * 3));
+    SRL_CUDA(ctx, rel.alloc(cap));
+    SRL_CUDA(ctx, ts.alloc(cap));
     if (size) {
         SRL_CUDA(ctx, cudaMemcpyAsync(xyz, l->d_xyz + 3 * l->head, size * 3 * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream));
         SRL_CUDA(ctx, cudaMemcpyAsync(rel, l->d_rel + l->head, size * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream));
         SRL_CUDA(ctx, cudaMemcpyAsync(ts, l->d_ts + l->head, size * sizeof(double), cudaMemcpyDeviceToDevice, ctx->stream));
     }
     SRL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    cudaFree(l->d_xyz); cudaFree(l->d_rel); cudaFree(l->d_ts);
-    l->d_xyz = xyz; l->d_rel = rel; l->d_ts = ts;
+    l->d_xyz = std::move(xyz); l->d_rel = std::move(rel); l->d_ts = std::move(ts);
     l->cap = cap;
     l->tail = size;
     l->head = 0;
@@ -524,7 +522,7 @@ int emit_and_finish(srl_lidar* l, const LivoxArgs& la, const CloudArgs& ca, cons
     SRL_CUDA(ctx, cub::DeviceScan::ExclusiveSum(cub_tmp, cub_bytes, flags, pos, n_all, st));
     k_emit<kLivox><<<grid, 256, 0, st>>>(la, ca, s.key, s.val, d_count, d_bad, ring_first, flags, pos, q);
     k_finish<kLivox><<<1, 1, 0, st>>>(la, ca, s.key, d_count, d_bad, flags, pos, n_all, q, (long long)l->head,
-                                      static_cast<LidarOut*>(l->d_out), nullptr);
+                                      static_cast<LidarOut*>(l->d_out.get()), nullptr);
     ctx->launches += 4;
     SRL_CUDA(ctx, cudaGetLastError());
     SRL_CUDA(ctx, cudaMemcpyAsync(h, l->d_out, sizeof(LidarOut), cudaMemcpyDeviceToHost, st));
@@ -551,26 +549,25 @@ int srl_lidar_create(srl_ctx* ctx, const srl_lidar_params* params, size_t initia
         return set_err(ctx, SRL_BAD_ARG, "srl_lidar_create: n_scans, scan_rate and point_filter_num must be >= 1");
     if (initial_capacity > 0x7fffffffULL) return set_err(ctx, SRL_BAD_ARG, "srl_lidar_create: capacity must fit in int32");
     SRL_CUDA(ctx, cudaSetDevice(ctx->device));
-    srl_lidar* l = new srl_lidar();
+    std::unique_ptr<srl_lidar> l(new srl_lidar());
     l->ctx = ctx;
+    l->device = ctx->device;
     l->p = p;
     // setTimeUnit: float literals held in a double
     l->scale = p.time_unit == 0 ? (double)1.e3f : p.time_unit == 2 ? (double)1.e-3f : p.time_unit == 3 ? (double)1.e-6f : (double)1.f;
-    cudaError_t e = cudaMalloc(&l->d_out, sizeof(LidarOut));
-    if (e == cudaSuccess) e = cudaMallocHost(&l->h_out, sizeof(LidarOut));
-    if (e != cudaSuccess) { srl_lidar_destroy(l); return cuda_fail(ctx, e, "srl_lidar_create"); }
-    const int rc = reserve(l, std::max<size_t>(initial_capacity, 1));
-    if (rc != SRL_OK) { srl_lidar_destroy(l); return rc; }
-    *out = l;
+    cudaError_t e = l->d_out.alloc(sizeof(LidarOut));
+    if (e == cudaSuccess) e = l->h_out.alloc(sizeof(LidarOut));
+    if (e != cudaSuccess) return cuda_fail(ctx, e, "srl_lidar_create");
+    const int rc = reserve(l.get(), std::max<size_t>(initial_capacity, 1));
+    if (rc != SRL_OK) return rc;
+    *out = l.release();
     return SRL_OK;
 }
 
 void srl_lidar_destroy(srl_lidar* l) {
     if (!l) return;
-    cudaSetDevice(l->ctx->device);
-    cudaStreamSynchronize(l->ctx->stream);
-    cudaFree(l->d_xyz); cudaFree(l->d_rel); cudaFree(l->d_ts); cudaFree(l->d_out);
-    if (l->h_out) cudaFreeHost(l->h_out);
+    cudaSetDevice(l->device);
+    cudaDeviceSynchronize();   // the last message's copy into the pinned summary has landed
     delete l;
 }
 
@@ -617,7 +614,7 @@ int srl_lidar_livox(srl_lidar* l, const uint8_t* records, size_t n, size_t strid
     rc = run_sort(ctx, s, L, n, d_count, nullptr);
     if (rc != SRL_OK) return rc;
     s.counters += 1;
-    LidarOut& h = *static_cast<LidarOut*>(l->h_out);
+    LidarOut& h = *static_cast<LidarOut*>(l->h_out.get());
     rc = emit_and_finish<true>(l, la, ca, s, d_count, nullptr, nullptr, flags, pos, cub_tmp, cub_bytes, (int)n, &h);
     if (rc != SRL_OK) return rc;
     apply_out(l, h);
@@ -685,7 +682,7 @@ int srl_lidar_process(srl_lidar* l, const uint8_t* data, size_t n, const srl_clo
     rc = run_sort(ctx, s, L, n, d_count, d_bad);
     if (rc != SRL_OK) return rc;
     s.counters += 1;
-    LidarOut& h = *static_cast<LidarOut*>(l->h_out);
+    LidarOut& h = *static_cast<LidarOut*>(l->h_out.get());
     rc = emit_and_finish<false>(l, la, ca, s, d_count, d_bad, ring_first, flags, pos, cub_tmp, cub_bytes, (int)n, &h);
     if (rc != SRL_OK) return rc;
     if (h.bad) return set_err(ctx, SRL_BAD_ARG, h.bad == 1 ? "srl_lidar_process: ring >= n_scans" : "srl_lidar_process: NaN sort key");
@@ -712,10 +709,10 @@ int srl_lidar_cut(srl_lidar* l, double t, int64_t* count, const double** raw_xyz
     if (rc != SRL_OK) return rc;
     SRL_CUDA(ctx, cudaMemsetAsync(first, 0xff, sizeof(unsigned long long), st));
     k_cut<<<grid_for(l->tail - head), 256, 0, st>>>(l->d_ts, (long long)head, (long long)l->tail, t, first);
-    k_cut_finish<<<1, 1, 0, st>>>(l->d_ts, (long long)head, (long long)l->tail, first, static_cast<LidarOut*>(l->d_out));
+    k_cut_finish<<<1, 1, 0, st>>>(l->d_ts, (long long)head, (long long)l->tail, first, static_cast<LidarOut*>(l->d_out.get()));
     ctx->launches += 2;
     SRL_CUDA(ctx, cudaGetLastError());
-    LidarOut& h = *static_cast<LidarOut*>(l->h_out);
+    LidarOut& h = *static_cast<LidarOut*>(l->h_out.get());
     SRL_CUDA(ctx, cudaMemcpyAsync(&h, l->d_out, sizeof(LidarOut), cudaMemcpyDeviceToHost, st));
     SRL_CUDA(ctx, cudaStreamSynchronize(st));
     l->head += (size_t)h.cut_count;

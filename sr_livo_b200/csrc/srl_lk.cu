@@ -298,27 +298,17 @@ struct srl_lk {
     float min_eig = 1e-4f;
     int cols = 0, rows = 0;         // the first image's size; 0 before it
     int lcols[kLkMaxLevels] = {0}, lrows[kLkMaxLevels] = {0};
-    uint8_t* img[2][kLkMaxLevels] = {{nullptr}};
-    short2* der[2][kLkMaxLevels] = {{nullptr}};
+    DevArray<uint8_t> img[2][kLkMaxLevels];
+    DevArray<short2> der[2][kLkMaxLevels];
     int prev = 0;                   // the set holding the previous image
     bool have_prev = false;
-    unsigned long long* d_count = nullptr;
-    cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};   // call start, pyramid built, points tracked
+    DevArray<unsigned long long> d_count;
+    Event ev[3];                    // call start, pyramid built, points tracked
     bool timed = false;
 };
 srl_ctx* srl::lk_ctx(const srl_lk* lk) { return lk->ctx; }
 
 namespace {
-
-void lk_free(srl_lk* lk) {
-    for (int s = 0; s < 2; ++s)
-        for (int l = 0; l < kLkMaxLevels; ++l) {
-            if (lk->img[s][l]) cudaFree(lk->img[s][l]);
-            if (lk->der[s][l]) cudaFree(lk->der[s][l]);
-            lk->img[s][l] = nullptr;
-            lk->der[s][l] = nullptr;
-        }
-}
 
 // The first image: the level count of opencvBuildOpticalFlowPyramid (:561-624) and both buffer sets
 int lk_allocate(srl_lk* lk, int cols, int rows) {
@@ -335,8 +325,8 @@ int lk_allocate(srl_lk* lk, int cols, int rows) {
     for (int s = 0; s < 2; ++s)
         for (int l = 0; l <= top; ++l) {
             const size_t px = (size_t)(lk->lcols[l] + 2 * lk->win_w) * (lk->lrows[l] + 2 * lk->win_h);
-            SRL_CUDA(ctx, cudaMalloc(&lk->img[s][l], px));
-            SRL_CUDA(ctx, cudaMalloc(&lk->der[s][l], px * sizeof(short2)));
+            SRL_CUDA(ctx, lk->img[s][l].alloc(px));
+            SRL_CUDA(ctx, lk->der[s][l].alloc(px));
         }
     lk->cols = cols;
     lk->rows = rows;
@@ -381,7 +371,7 @@ int srl_lk_create(srl_ctx* ctx, const srl_lk_params* p, srl_lk** out) {
     if (p->win_w < 3 || p->win_w > 31 || p->win_h < 3 || p->win_h > 31)
         return set_err(ctx, SRL_BAD_ARG, "srl_lk_create: the window must be 3..31 pixels in each dimension");
     if (p->max_level < 0 || p->max_level > kLkMaxLevels - 1) return set_err(ctx, SRL_BAD_ARG, "srl_lk_create: max_level must be 0..8");
-    auto* lk = new srl_lk;
+    std::unique_ptr<srl_lk> lk(new srl_lk);
     lk->ctx = ctx;
     lk->device = ctx->device;
     lk->win_w = p->win_w;
@@ -393,23 +383,16 @@ int srl_lk_create(srl_ctx* ctx, const srl_lk_params* p, srl_lk** out) {
     lk->flags = p->flags;
     lk->min_eig = (float)p->min_eig_threshold;
     cudaError_t e = cudaSetDevice(ctx->device);
-    if (e == cudaSuccess) e = cudaMalloc(&lk->d_count, sizeof(unsigned long long));
-    for (int i = 0; i < 3 && e == cudaSuccess; ++i) e = cudaEventCreate(&lk->ev[i]);
-    if (e != cudaSuccess) {
-        srl_lk_destroy(lk);
-        return cuda_fail(ctx, e, "srl_lk_create");
-    }
-    *out = lk;
+    if (e == cudaSuccess) e = lk->d_count.alloc(1);
+    for (int i = 0; i < 3 && e == cudaSuccess; ++i) e = lk->ev[i].create();
+    if (e != cudaSuccess) return cuda_fail(ctx, e, "srl_lk_create");
+    *out = lk.release();
     return SRL_OK;
 }
 
 void srl_lk_destroy(srl_lk* lk) {
     if (!lk) return;
-    cudaSetDevice(lk->device);   // not through lk->ctx: a handle may outlive its ctx (cudaFree waits for the device itself)
-    lk_free(lk);
-    if (lk->d_count) cudaFree(lk->d_count);
-    for (auto& e : lk->ev)
-        if (e) cudaEventDestroy(e);
+    cudaSetDevice(lk->device);
     delete lk;
 }
 
@@ -427,8 +410,8 @@ int srl_lk_track_image(srl_lk* lk, const uint8_t* gray, int cols, int rows, size
     SRL_CUDA(ctx, cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->stream;
     if (!lk->cols) {
-        int rc = lk_allocate(lk, cols, rows);
-        if (rc != SRL_OK) { lk_free(lk); lk->cols = lk->rows = 0; return rc; }
+        int rc = lk_allocate(lk, cols, rows);   // sets cols and rows only once every level exists
+        if (rc != SRL_OK) return rc;
     }
     const bool img_dev = mem_kind(gray) == MemKind::Device;
     Staged<const float> in_pts(last_pts);

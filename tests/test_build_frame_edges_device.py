@@ -35,7 +35,7 @@ def L():
 
 @pytest.fixture
 def new_frame(L):
-    """CloudFrame(L.ctx, capacity) closed at the test's end, also when it fails: a frame must not outlive its context."""
+    """CloudFrame(L.ctx, capacity) closed at the test's end, also when it fails, so that its device memory goes with the test."""
     from sr_livo_b200 import lio
     made = []
 
